@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- BASELINE.json's metric on synthetic Llama-70B-shape matrices.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over the workload `w4a16_gemv_llama70b`: the W4A16 (uint4, group 128, GPTQ-style
 quantized zeros, interleaved storage) GEMV at M=1 for the Llama-2-70B linear shapes BASELINE.json configs[1] names
@@ -14,6 +14,9 @@ the three Llama (N,K) pairs + M=4096 N=K=12288, TFLOPS) and the W2A8 path are me
 activations (pinned H2D copy + D2H of the result inside the timed region, synchronised every step).  With --gpus N>1
 (launched under torchrun) the weights are sharded along N across ranks (column parallel) and the outputs gathered:
 strong scaling, max-over-ranks device time.
+
+--dump-outputs DIR writes the four outputs of the last timed GEMV step as DIR/gemv_N{N}_K{K}.npy (float32).  Every input is
+generated from fixed seeds, so two builds of the project run with the same arguments can be compared output for output.
 
 --impl reference times the reference's only CPU implementation of this path -- the torch dequantise+matmul reference
 program of its tests (testing/python/operators/test_general_matmul_ops_backend_tl.py:227-273), restated in
@@ -50,17 +53,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf=d["bf16_tflops"], tf_sustained=d.get("bf16_tflops_sustained"), src="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tf=1590.0, tf_sustained=1400.0, src="fallback (B200_PROFILING.md)")
-
-
-def profiled_traffic():
-    """DRAM bytes per launch of the dominant kernels, from the committed ncu capture (profiles/r2_traffic.json, written by
-    tools/ncu_traffic.py out of an `ncu --set full` report; keyed to the commit it was taken at).  None if absent."""
-    p = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    try:
-        return json.load(open(p))
-    except Exception:
-        return {}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense FP16/BF16 -- not reached figures
+    return dict(hbm=3350.0, tf=989.0, tf_sustained=None, src="H100 SXM data sheet")
 
 
 def gemv_bytes(N, K, M=1, bits=4, g=GROUP, zeros="quantized", a_bytes=2, out_bytes=2):
@@ -72,7 +66,7 @@ def gemv_bytes(N, K, M=1, bits=4, g=GROUP, zeros="quantized", a_bytes=2, out_byt
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -243,7 +237,7 @@ def make_linear(bitblas, N_local, K, dev, *, a_dtype="float16", w_dtype="uint4",
 
 def oracle_gate(bitblas, dev):
     """Correctness gate, run before any timing: W4A16 at a BASELINE shape built from real quantised fields through the product's
-    own device weight transform; M = 1 (the streaming kernel) and M = 16 (the tcgen05 kernel); 512 output features compared with
+    own device weight transform; M = 1 (the streaming kernel) and M = 16 (the wgmma kernel); 512 output features compared with
     the CPU oracle (rtol = atol = 1e-2 like the reference's tests).  Raises on mismatch."""
     sys.path.insert(0, os.path.join(ROOT, "oracle"))
     import bitblas_oracle as O
@@ -294,10 +288,10 @@ def timed(fn, steps, warmup, barrier=None):
 
 def rotating_kernel_time(op, prm, A, out, reps=5, min_bytes=300 * 1024 * 1024):
     """per-launch kernel time with a cold L2: back-to-back launches cycling through enough read-only copies of the parameters
-    that the working set (> 2x the 126 MB L2) can never be resident; median of `reps` passes.  The pass is captured in a CUDA
+    that the working set (> 2x the 50 MB L2) can never be resident; median of `reps` passes.  The pass is captured in a CUDA
     graph (the launches keep their programmatic-dependent-launch edges) so that a ~10 us kernel is not timed against the ~10 us
     Python call that launches it; if capture is unavailable the launches are issued directly.  (No write-flush: dirty lines
-    left in L2 by a flush kernel are written back DURING the timed kernel and charged to it -- measured +10..25 us.)"""
+    left in L2 by a flush kernel are written back DURING the timed kernel and charged to it.)"""
     wbytes = prm["W"].numel()
     ncopies = max(2, -(-min_bytes // wbytes))
     copies = [prm] + [{k: (v.clone() if v is not None else None) for k, v in prm.items()} for _ in range(ncopies - 1)]
@@ -374,7 +368,11 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--skip-cpu", action="store_true", help="skip the cpu_baseline leg (profiling runs)")
     ap.add_argument("--only", default="", help="comma list of sections to run: gemm,llama,w2a8,formats,e2e (default all; the GEMV step always runs)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed GEMV step to DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     if args.impl == "reference":
         return run_reference(args)
 
@@ -392,7 +390,8 @@ def main():
     from bitblas_b200 import _lib
     lib = _lib.load()
     pk = peaks()
-    traffic = profiled_traffic()
+    if args.dump_outputs and world > 1:
+        raise SystemExit("--dump-outputs needs a single GPU (--gpus 1)")
     only = set(x for x in args.only.split(",") if x)
     want = lambda s: not only or s in only  # noqa: E731
     warmup = max(3, args.warmup)
@@ -480,7 +479,7 @@ def main():
     result = {"oracle_gate": gate}
     sampler = ClockSampler(torch.cuda.current_device())
     # ---------------- GEMV (the headline workload) ----------------
-    # Every step streams parameters that cannot be L2-resident: at world = 1 the step's own 357 MB exceed the 126 MB L2; with the
+    # Every step streams parameters that cannot be L2-resident: at world = 1 the step's own 357 MB exceed the 50 MB L2; with the
     # weights sharded over `world` GPUs the per-GPU share shrinks below it, so the step cycles through `nsets` independent
     # parameter sets (>= 300 MB per GPU in total) -- step i uses set i % nsets.
     total_bytes = sum(gemv_bytes(N, K) for N, K in GEMV_SHAPES)
@@ -489,12 +488,13 @@ def main():
     if world > 1 and nsets % 2:
         nsets += 1                # the fused path alternates two symmetric output buffers per projection: keep the cycle even
     sets = []
+    ga = torch.Generator(device=dev).manual_seed(1234)   # activations: identical from run to run (--dump-outputs)
     for c in range(nsets):
         ops_c = []
         for i, (N, K) in enumerate(GEMV_SHAPES):
             if c == 0:
                 op, prm = make_linear(bitblas, N // world, K, dev, seed=i)
-                A = (torch.rand((1, K), device=dev) - 0.5).half()
+                A = (torch.rand((1, K), generator=ga, device=dev) - 0.5).half()
                 out = torch.empty((1, N // world), dtype=torch.float16, device=dev)
             else:
                 op, prm0, A, out = sets[0][i][:4]
@@ -593,6 +593,12 @@ def main():
     torch.cuda.synchronize()
     barrier()
     ms_step = ev0.elapsed_time(ev1) / args.steps
+    if args.dump_outputs:
+        # every parameter set shares the four output buffers: they hold the last timed step's results
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for op, prm, A, out, N, K in sets[0]:
+            np.save(os.path.join(args.dump_outputs, f"gemv_N{N}_K{K}.npy"), out.float().cpu().numpy())
     # kernels of this library launched inside the timed region (replayed graph launches are not seen by the library's counter)
     launches = (launches_per_step * args.steps) if step_graphs is not None else (lib.bb_launch_count() - launches0)
     ms_step = max_over_ranks(ms_step)
@@ -610,10 +616,8 @@ def main():
                           "frac_hbm": round(b / (t * 1e-3) / 1e9 / pk["hbm"], 3), "kernel": op.kernel_for(1), "copies": ncopies,
                           "cuda_graph": graphed})
     tgt = per_shape[-1]
-    tr = traffic.get("gemv_m1_12288") if world == 1 else None
     roofline = {"bound": "hbm", "kernel": f"{tgt['kernel']} (W4A16 m=1 N=K=12288)", "achieved": tgt["GBps"],
                 "peak": pk["hbm"], "unit": "GB/s", "frac": tgt["frac_hbm"],
-                "traffic": tr.get("dram_bytes") if tr else None, "traffic_source": tr.get("source") if tr else None,
                 "algorithmic_bytes": gemv_bytes(12288 // world, 12288), "us": tgt["us"], "peak_source": pk["src"],
                 "timing": "CUDA events around back-to-back launches (one CUDA graph per pass) cycling through >= 300 MB of read-only parameter copies (cold L2), per-launch average, median of 5"}
     result["gemv_shapes"] = per_shape
@@ -634,12 +638,10 @@ def main():
         M, N, K = GEMM_SHAPE
         op, prm = make_linear(bitblas, N // world, K, dev, seed=11)
         g4 = gemm_point(op, prm, M, N, K, 10)
-        trg = traffic.get("gemm_m4096_12288") if world == 1 else None
         result["gemm"] = {"M": M, "N": N, "K": K, "ms": round(g4["us"] / 1e3, 4), "TFLOPS": g4["TFLOPS"], "kernel": g4["kernel"],
                           "roofline": {"bound": "tensor", "achieved": g4["TFLOPS"], "peak": pk["tf"], "unit": "TFLOP/s",
                                        "frac": g4["frac_tensor"],
                                        "frac_of_sustained": round(g4["TFLOPS"] / pk["tf_sustained"], 3) if pk["tf_sustained"] else None,
-                                       "traffic": trg.get("dram_bytes") if trg else None, "traffic_source": trg.get("source") if trg else None,
                                        "algorithmic_flops": 2.0 * M * N * K, "peak_source": pk["src"],
                                        "note": "A (100 MB) + W (75 MB) exceed L2; 10 back-to-back launches"}}
         result["gemm_small_m"] = [gemm_point(op, prm, m, N, K, 20) for m in (16, 128)]
@@ -678,7 +680,7 @@ def main():
         result["w2a8"] = w2
         result["int8_peak_tops_measured"] = round(i8peak, 1) if i8peak else None
 
-    # ---------------- table formats (NF4) on the fast kernels: decode GEMV and tcgen05 GEMM at the target shape ----------------
+    # ---------------- table formats (NF4) on the fast kernels: decode GEMV and wgmma GEMM at the target shape ----------------
     if want("formats") and world == 1:
         N, K = 12288, 12288
         cfgn = bitblas.MatmulConfig(M=[1, 4096], N=N, K=K, A_dtype="float16", W_dtype="nf4", accum_dtype="float16", out_dtype="float16",
@@ -787,7 +789,7 @@ def main():
                 "warmup": warmup, "ms_per_step": round(ms_step, 4), "higher_is_better": True,
                 "scaling": "strong", "vs_baseline": None, "dtype": "f16", "data": "synthetic", "config": CONFIG,
                 "config_detail": {"parallelism": par,
-                                  "l2": f"inputs larger than L2: each step streams {per_gpu / 1e6:.0f} MB per GPU and steps cycle through {nsets} independent parameter set(s) (>= 300 MB per GPU vs the 126 MB L2); per-shape numbers rotate >= 300 MB of parameter copies"},
+                                  "l2": f"inputs larger than L2: each step streams {per_gpu / 1e6:.0f} MB per GPU and steps cycle through {nsets} independent parameter set(s) (>= 300 MB per GPU vs the 50 MB L2); per-shape numbers rotate >= 300 MB of parameter copies"},
                 "roofline": roofline, "cpu_baseline": cpu, "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks}
         line.update(result)
         print(json.dumps(line), flush=True)

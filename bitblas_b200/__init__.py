@@ -1,4 +1,4 @@
-"""bitblas_b200 -- a B200-native (sm_100a) implementation of the BitBLAS low-bit-weight matmul operator API.
+"""bitblas_b200 -- a H100-native (sm_90a) implementation of the BitBLAS low-bit-weight matmul operator API.
 
 Public surface mirrors ``bitblas/__init__.py:169-175``: ``Matmul``, ``MatmulConfig``, ``Linear``,
 ``auto_detect_nvidia_target``, ``set_log_level``, ``__version__`` (+ ``bitblas.cache``, ``bitblas.quantization``,

@@ -2,9 +2,9 @@
 //
 // Dispatch mirrors the reference's run-time choice (bitblas/ops/general_matmul/tilelang/dequantize/
 // matmul_dequantize.py:93-111: M < 8 -> SIMT GEMV, else MMA GEMM; and the per-opt_M if-chain emitted into
-// `call`, bitblas/builder/wrapper/tl.py:278-300) but is keyed on the B200 regimes instead:
+// `call`, bitblas/builder/wrapper/tl.py:278-300) but is keyed on the H100 regimes instead:
 //   m <= 8   : memory-bound streaming kernels (bb_gemv.cu)
-//   m  > 8   : tcgen05 tensor-core kernel (bb_gemm_ts.cu), split-K when the tile grid is smaller than the chip
+//   m  > 8   : wgmma tensor-core kernel (bb_gemm_ts.cu), split-K when the tile grid is smaller than the chip
 //   anything the fast kernels do not cover: the generic SIMT kernel (bb_generic.cu).
 #include <cstring>
 #include <mutex>
@@ -35,7 +35,7 @@ int device_sm_count() {
   const int dev = current_device();
   int n = g_sm_count[dev].load(std::memory_order_relaxed);
   if (n == 0) {
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) { cudaGetLastError(); n = 148; }
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) { cudaGetLastError(); n = 132; }
     g_sm_count[dev].store(n, std::memory_order_relaxed);
   }
   return n;
@@ -98,7 +98,7 @@ static int select(const bb_matmul_desc& d, int m) {
     if (gemm_ts_supported(d, m)) return d.a_dtype == BB_I8 ? BB_KERNEL_GEMM_TS_I8 : BB_KERNEL_GEMM_TS;
     return BB_KERNEL_GENERIC;
   }
-  // m <= 8 (one n8 MMA tile): streaming kernels; above that the tcgen05 kernel (split-K keeps the SMs busy at small m)
+  // m <= 8 (one n8 MMA tile): streaming kernels; above that the wgmma kernel (split-K keeps the SMs busy at small m)
   // is faster (12288^2 sweep, tools/smallm_sweep.py); the streaming kernels stay as the fallback up to m = 32.
   if (m <= 8) {
     if (gemv_slab_supported(d, m)) return BB_KERNEL_GEMV_SLAB;
@@ -170,7 +170,9 @@ int bb_init(int device) {
   // queries only: the caller's current device is left untouched (torch owns it)
   int major = 0;
   BB_CHECK_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-  if (major != 10) { set_error("bitblas_b200 needs an sm_100a device (compute capability 10.x), found %d.x", major); return 2; }
+  int minor = 0;
+  BB_CHECK_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
+  if (major != 9 || minor != 0) { set_error("bitblas_b200 is built for sm_90a (H100, compute capability 9.0), found %d.%d", major, minor); return 2; }
   int n = 0;
   BB_CHECK_CUDA(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device));
   if (device < BB_MAX_DEVICES && n > 0) g_sm_count[device].store(n);
@@ -188,8 +190,8 @@ const char* bb_kernel_name(int id) {
     case BB_KERNEL_GENERIC: return "generic_simt";
     case BB_KERNEL_GEMV_MMA: return "gemv_mma";
     case BB_KERNEL_GEMV_I8: return "gemv_i8";
-    case BB_KERNEL_GEMM_TS: return "gemm_ts_tcgen05";
-    case BB_KERNEL_GEMM_TS_I8: return "gemm_ts_tcgen05_i8";
+    case BB_KERNEL_GEMM_TS: return "gemm_ts_wgmma";
+    case BB_KERNEL_GEMM_TS_I8: return "gemm_ts_wgmma_i8";
     case BB_KERNEL_GEMV_STREAMK: return "gemv_streamk";
     case BB_KERNEL_GEMV_SLAB: return "gemv_slab";
   }

@@ -1,4 +1,4 @@
-// bb_common.cuh -- shared host/device helpers for the sm_100a kernels.
+// bb_common.cuh -- shared host/device helpers for the sm_90a kernels.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

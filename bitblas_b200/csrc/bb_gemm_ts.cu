@@ -1,24 +1,23 @@
-// bb_gemm_ts.cu -- the tensor-core path: tcgen05.mma with the dequantised weights as the TMEM ("TS") operand.
+// bb_gemm_ts.cu -- the tensor-core path: Hopper wgmma with the dequantised weights as the register ("RS") operand.
 //
 // Replaces the reference's generated mma.sync GEMM (bitblas/ops/general_matmul/tilelang/dequantize/
 // matmul_dequantize_mma.py:333-506: cp.async -> smem(int8) -> regs -> LOP3 decode -> smem(fp16) -> ldmatrix
-// -> mma.sync m16n8k16).  On B200 the decoded weights never touch shared memory:
+// -> mma.sync m16n8k16).  On H100 the decoded weights never touch shared memory:
 //
 //     C^T[n, m] = sum_k  Wdeq[n, k] * A[m, k]            (the operands are swapped: W is the MMA "A"/M side)
 //
 //   TMA warp      : per k-block, one 2-D tile of activations A[BM x 64] (fp16/bf16; 128 int8) into 128B-swizzled
-//                   shared memory (the MMA "B"/N operand, K-major) and one tile of PACKED weights
+//                   shared memory (the wgmma "B"/N operand, K-major) and one tile of PACKED weights
 //                   W[128 rows x 32 B] (4-bit) -- 8x fewer bytes than a dequantised tile;
-//   dequant warps : 8 warps, thread <-> weight row (= TMEM lane).  ld.shared 16 B -> LOP3 decode + (w-z)*s
-//                   in registers -> tcgen05.st into a ring of TMEM operand slots (32 columns per k-block);
-//   MMA warp      : one elected thread issues tcgen05.mma.kind::f16 (or kind::i8) M=128, N=BM, K=16 (32),
-//                   A operand from TMEM, B operand from the swizzled smem descriptor, fp32 (s32) accumulator
-//                   in TMEM; tcgen05.commit releases the smem stage and the TMEM slot through mbarriers;
-//   epilogue      : the dequant warps read the accumulator with tcgen05.ld, cast, add bias, store C[m, n].
+//   2 warpgroups  : each owns 64 weight rows.  A thread reads the packed bytes of its two fragment rows (g, g + 8) from
+//                   shared memory, decodes them with LOP3 / PRMT + (w-z)*s straight into the register layout of the wgmma
+//                   A fragment, and issues wgmma.mma_async m64nBMk16 (k32 for int8) with the activation tile as the smem
+//                   descriptor operand; fp32 (s32) accumulators stay in registers.  Fragments are double-buffered: the
+//                   decode of k-block kb + 1 overlaps the MMAs of kb, and wgmma.wait_group 1 releases the smem stage of kb - 1;
+//   epilogue      : the accumulators are cast, biased and stored as C[m, n].
 //
-// Shared-memory traffic per k-block is therefore A-tile (TMA write + MMA read) + 4 KB packed W, instead of
-// also writing and re-reading a 16-32 KB dequantised W tile -- the difference between fitting and not fitting
-// the 128 B/clk/SM shared-memory budget at full tensor rate (DESIGN.md §4).
+// Shared-memory traffic per k-block is therefore A-tile (TMA write + MMA read) + 4 KB packed W, instead of also writing and
+// re-reading a 16-32 KB dequantised W tile (DESIGN.md §3.1).
 #include <cuda.h>
 
 #include <algorithm>
@@ -30,17 +29,9 @@ namespace bb {
 
 namespace {
 
-constexpr int TS_ROWS = 128;    // weight rows per CTA = MMA M
-// 16 dequant warps = 4 TMEM lane quadrants x 4.  Two organisations (dq_groups(BM)):
-//  * BM > 128 (one CTA per SM, 36 KB stages, 6 of them): 2 groups x (4 quadrants x 2 column halves); a thread decodes HALF a row
-//    of its group's k-blocks.  A k-block leaves the dequant stage quickly, so at most two smem stages are pinned by decoding.
-//  * BM <= 128 (small stages, 8 of them): 4 groups x 4 quadrants; a thread decodes its WHOLE row (both halves) per iteration,
-//    so the barrier / slot bookkeeping -- about as many instructions as one half's decode -- is paid once per 64 weights
-//    (m = 16: 47 -> 38 us; with the large tile this organisation pins 4 of 6 stages and starves the TMA ring: 1285 -> 866 TFLOPS).
-constexpr int DQ_WARPS = 16;
-__host__ __device__ constexpr int dq_groups(int BM) { return BM > 128 ? 2 : 4; }
-constexpr int TS_THREADS = (2 + DQ_WARPS) * 32;
-constexpr int TA_SLOTS = 4;     // TMEM operand slots (2 per dequant group with 2 groups, 1 per group with 4)
+constexpr int TS_ROWS = 128;               // weight rows per CTA = two wgmma M = 64 warpgroups
+constexpr int TS_CONSUMER_WARPS = 8;       // warps 0-7: two consumer warpgroups (wgmma needs warpgroup-aligned warps)
+constexpr int TS_THREADS = (TS_CONSUMER_WARPS + 1) * 32;   // + warp 8: TMA producer
 
 // ---------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -89,78 +80,27 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// D[tmem] (+)= A[tmem] * B[smem desc]
-template <bool INT8>
-__device__ __forceinline__ void tc_mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (INT8) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], [%1], %2, %3, p;\n}\n" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n}\n" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-
-__device__ __forceinline__ void tmem_st_x16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_x8(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr)
-               : "memory");
-}
-
-// K-major, 128B-swizzled shared-memory operand descriptor (rows of 128 B, 8-row swizzle atoms = 1024 B)
+// K-major, 128B-swizzled shared-memory operand descriptor (rows of 128 B, 8-row swizzle atoms = 1024 B); the tile is
+// 1024-byte aligned, so the base-offset field stays 0.  Advancing k by 32 bytes inside the atom adds 2 to the address field.
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= uint64_t((smem_addr & 0x3FFFFu) >> 4);  // start address, 16-byte units
-  d |= uint64_t(0) << 16;                      // leading byte offset: unused for swizzled K-major
+  d |= uint64_t(1) << 16;                      // leading byte offset: unused for swizzled K-major
   d |= uint64_t(1024 >> 4) << 32;              // stride byte offset: 8 rows * 128 B
-  d |= uint64_t(1) << 46;                      // descriptor version (sm_100)
-  d |= uint64_t(2) << 61;                      // SWIZZLE_128B
+  d |= uint64_t(1) << 62;                      // SWIZZLE_128B
   return d;
 }
+
+// D[64 x N] (+)= A[64 x 16] (registers) * B[N x 16] (smem descriptor), and the int8 m64nNk32 variant (A unsigned or signed,
+// B = int8 activations).  acc = 0 overwrites D.
+template <int N>
+struct Wgmma;
+#include "bb_wgmma.inc"
 
 // ---------------------------------------------------------------------------------------------
 struct TsParams {
@@ -175,14 +115,12 @@ struct TsParams {
   int out_dtype;
   int a_dtype;
   int m_tiles;
-  int stages;        // smem pipeline depth (even; <= TsSmem::kStages)
   int splits;        // split-K factor (>1: fp32 / int32 partials go to `ws`, reduced by splitk_reduce_kernel)
   int kb_per_split;  // k-blocks per split
   void* ws;          // [splits][M][N] partials
   const void* lut;   // NF4 table (16 x A_dtype), null otherwise
   int w_fmt;         // bb_wfmt (the table formats run the FMT = 1 instances)
   int w_tiled;       // BB_TILE_SLAB weight storage: tmW is the 4-D map {512 B, 32 rows, segments per row, row blocks}
-  int staged_epi;    // 16-bit outputs: transpose the accumulator tile through shared memory, 16-byte row-major stores (see epilogue)
 };
 
 template <typename T>
@@ -196,23 +134,15 @@ struct ElemInfo<int8_t> {
   static constexpr int kKB = 128;
 };
 
-template <int BM>
-struct TsTmem {
-  static constexpr int kAcol0 = BM < 32 ? 32 : BM;
-  static constexpr int kSlots = TA_SLOTS;
-  static constexpr int kNeed = kAcol0 + kSlots * 32;
-  static constexpr int kCols = kNeed <= 64 ? 64 : (kNeed <= 128 ? 128 : (kNeed <= 256 ? 256 : 512));
-};
-
 template <typename T, int BITS, int BM>
 struct TsSmem {
   static constexpr int kPRB = ElemInfo<T>::kKB * BITS / 8;  // packed bytes per row per k-block
   static constexpr int kActBytes = BM * 128;
   static constexpr int kWBytes = TS_ROWS * kPRB;
   static constexpr int kStageBytes = kActBytes + kWBytes;
-  static constexpr int kStagesRaw = (220 * 1024) / kStageBytes;
-  static constexpr int kStages = (kStagesRaw > 8 ? 8 : kStagesRaw) & ~1;  // even: stage parity is static per dequant group
-  static constexpr int kBarBytes = 512;   // full[8] + empty[8] + a_ready[8] + a_free[8] + acc_full + tmem slot word
+  static constexpr int kStagesRaw = (200 * 1024) / kStageBytes;
+  static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
+  static constexpr int kBarBytes = 256;   // full[8] + empty[8]
   static constexpr int kTotal = kStages * kStageBytes + kBarBytes + 1024;  // + alignment slack
 };
 
@@ -221,212 +151,190 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
   asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
   return v;
 }
-__device__ __forceinline__ uint2 lds64(uint32_t addr) {
-  uint2 v;
-  asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr));
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
   return v;
 }
 
-// decode this thread's half of the k-block (PRB/2 packed bytes at shared address `src`) into 16 registers of
-// natural-k-order 16-bit operand pairs.  MODE: 0 none, 1 scale, 2 original, 3 rescale, 4 quantized.
-// IL = LOP3-interleaved storage (fast_decoding); !IL = plain compressed storage, re-ordered with byte permutes.
-template <typename T, int BITS, int MODE, bool IL>
-__device__ __forceinline__ void dequant_half_row(uint32_t src, uint32_t (&out)[16], const DqConst& c) {
-  constexpr bool HI = IL && std::is_same<T, __half>::value && BITS == 4;
+// byte t of each of four words: (w0.t, w1.t, w2.t, w3.t)
+__device__ __forceinline__ uint32_t gather_byte(uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3, uint32_t sel) {
+  return __byte_perm(__byte_perm(w0, w1, sel), __byte_perm(w2, w3, sel), 0x5410);
+}
+
+// One weight row's share of a k-block in wgmma A-fragment order.  Thread t (= lane % 4) of a quad owns, per 16-element k
+// step s (32 for int8), the element pairs (quads) at k = 2t (4t) and k = 2t + 8 (4t + 16):  out[2s] and out[2s + 1].  `src` is
+// the shared address of the row's packed k-block.  16-bit targets return dequantised A_dtype pairs; int8 returns signed or
+// unsigned bytes.  MODE: 0 none, 1 scale, 2 original, 3 rescale, 4 quantized.  IL = LOP3-interleaved storage (fast_decoding);
+// !IL = plain compressed storage.  FMT: 0 integer, 1 16-entry table (NF4 / fp4), 2 8-bit float.
+template <typename T, int BITS, int MODE, bool IL, int FMT>
+__device__ __forceinline__ void dequant_row(uint32_t src, int t, uint32_t (&out)[8], const DqConst& c, const Lut4& lut,
+                                            bool e5m2) {
   constexpr uint32_t M = TypeTraits<T>::kMagic;
-  auto fin = [&](uint32_t x, uint32_t mz) -> uint32_t { return dq_finish<T, MODE, BITS>(x, mz, c); };
-  if constexpr (BITS == 4) {
-    const uint4 pk = lds128(src);
-    const uint32_t w[4] = {pk.x, pk.y, pk.z, pk.w};
+  constexpr uint32_t MBYTES = ((M >> 8) & 0xffu) * 0x01010101u;  // magic high byte (0x64 / 0x43)
+  auto fin = [&](uint32_t x) -> uint32_t { return dq_finish<T, MODE, BITS>(x, c.mz_lo, c); };
+  const uint32_t bsel = uint32_t(t) | (uint32_t(t + 4) << 4);
+  if constexpr (FMT == 2) {
+    // 8-bit floats: the pair at k = 16s + 2t is half (t & 1) of word 4s + t/2.  e5m2 is the top byte of an fp16
+    // (quantization.py:179-182); e4m3 follows the reference's bit trick (quantization.py:169-176); bf16 widens exactly.
+    const uint32_t hsel = (t & 1) ? 0x3424u : 0x1404u;   // (byte 2j) << 8 | (byte 2j+1) << 24
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      if constexpr (HI) {
-        // odd nibbles extracted in place: mantissa bits 4..7 under exponent 2^6 (0x5400) read exactly 64 + u
-        const uint32_t x = w[i], y = w[i] >> 8;
-        out[4 * i + 0] = fin(lop3_and_or(x, 0x000f000fu, M), c.mz_lo);
-        out[4 * i + 1] = fin(lop3_and_or(x, 0x00f000f0u, 0x54005400u), c.mz_hi);
-        out[4 * i + 2] = fin(lop3_and_or(y, 0x000f000fu, M), c.mz_lo);
-        out[4 * i + 3] = fin(lop3_and_or(y, 0x00f000f0u, 0x54005400u), c.mz_hi);
-      } else if constexpr (IL) {
-        uint32_t h[4];
-        decode_u4x8_raw<T>(w[i], h);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) out[4 * i + j] = fin(h[j], c.mz_lo);
-      } else {
-        // compressed: nibbles e0..e7 in order.  bytes t = (e0,e2,e4,e6), u = (e1,e3,e5,e7)
-        constexpr uint32_t MB = (M >> 8) & 0xffu, MBYTES = MB * 0x01010101u;  // magic high byte (0x64 / 0x43)
-        const uint32_t t = w[i] & 0x0f0f0f0fu, u = (w[i] >> 4) & 0x0f0f0f0fu;
-        const uint32_t x = __byte_perm(t, u, 0x5140), y = __byte_perm(t, u, 0x7362);  // (e0,e1,e2,e3), (e4,e5,e6,e7)
-        out[4 * i + 0] = fin(__byte_perm(x, MBYTES, 0x4140), c.mz_lo);
-        out[4 * i + 1] = fin(__byte_perm(x, MBYTES, 0x4342), c.mz_lo);
-        out[4 * i + 2] = fin(__byte_perm(y, MBYTES, 0x4140), c.mz_lo);
-        out[4 * i + 3] = fin(__byte_perm(y, MBYTES, 0x4342), c.mz_lo);
-      }
-    }
-  } else {
-    const uint2 pk = lds64(src);
-    const uint32_t w[2] = {pk.x, pk.y};
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      if constexpr (IL) {
-        uint32_t h[8];
-        decode_u2x16_raw_interleaved<T>(w[i], h);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) out[8 * i + j] = fin(h[j], c.mz_lo);
-      } else {
-        // compressed: fields e0..e15 in order.  byte planes s_k = (e_k, e_{k+4}, e_{k+8}, e_{k+12})
-        constexpr uint32_t MB = (M >> 8) & 0xffu, MBYTES = MB * 0x01010101u;
-        const uint32_t s0 = w[i] & 0x03030303u, s1 = (w[i] >> 2) & 0x03030303u, s2 = (w[i] >> 4) & 0x03030303u,
-                       s3 = (w[i] >> 6) & 0x03030303u;
-        const uint32_t a01 = __byte_perm(s0, s1, 0x5140), a23 = __byte_perm(s2, s3, 0x5140);  // (e0,e1,e4,e5) (e2,e3,e6,e7)
-        const uint32_t b01 = __byte_perm(s0, s1, 0x7362), b23 = __byte_perm(s2, s3, 0x7362);  // (e8,e9,e12,e13) ...
-        out[8 * i + 0] = fin(__byte_perm(a01, MBYTES, 0x4140), c.mz_lo);
-        out[8 * i + 1] = fin(__byte_perm(a23, MBYTES, 0x4140), c.mz_lo);
-        out[8 * i + 2] = fin(__byte_perm(a01, MBYTES, 0x4342), c.mz_lo);
-        out[8 * i + 3] = fin(__byte_perm(a23, MBYTES, 0x4342), c.mz_lo);
-        out[8 * i + 4] = fin(__byte_perm(b01, MBYTES, 0x4140), c.mz_lo);
-        out[8 * i + 5] = fin(__byte_perm(b23, MBYTES, 0x4140), c.mz_lo);
-        out[8 * i + 6] = fin(__byte_perm(b01, MBYTES, 0x4342), c.mz_lo);
-        out[8 * i + 7] = fin(__byte_perm(b23, MBYTES, 0x4342), c.mz_lo);
-      }
-    }
-  }
-}
-
-// table formats (NF4 / fp4), compressed storage: 16 packed bytes -> 32 values in natural k order; MODE 0 none, 1 scale
-template <typename T, int MODE>
-__device__ __forceinline__ void dequant_half_row_lut(uint32_t src, uint32_t (&out)[16], const Lut4& t, uint32_t s2) {
-  const uint4 pk = lds128(src);
-  const uint32_t w[4] = {pk.x, pk.y, pk.z, pk.w};
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    uint32_t h[4];
-    lut4_decode8(w[i], t, h);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) out[4 * i + j] = MODE == 1 ? mul2<T>(h[j], s2) : h[j];
-  }
-}
-
-// 8-bit float weights (e4m3_float8 / e5m2_float8 with 16-bit activations): 32 bytes -> 32 values in natural k order.
-// e5m2 is the top byte of an fp16 (quantization.py:179-182); e4m3 follows the reference's bit trick (quantization.py:169-176:
-// sign | ((v & 63) << 7 | e4 << 8 | e4 << 7) ^ 0x2000 with e4 = v & 0x40), evaluated on two bytes at a time.  bf16 activations:
-// the fp16 pair is widened exactly (every fp8 value is representable in bf16).
-template <typename T, int MODE>
-__device__ __forceinline__ void dequant_half_row_fp8(uint32_t src, uint32_t (&out)[16], bool e5m2, uint32_t s2) {
-  const uint4 p0 = lds128(src), p1 = lds128(src + 16);
-  const uint32_t w[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      const uint32_t x = __byte_perm(w[i], 0u, j ? 0x3424 : 0x1404);   // (byte 2j) << 8 | (byte 2j+1) << 24
+    for (int j = 0; j < 8; ++j) {
+      const uint32_t w = lds32(src + uint32_t((j >> 1) * 4 + (j & 1) * 2 + (t >> 1)) * 4u);
+      const uint32_t x = __byte_perm(w, 0u, hsel);
       uint32_t h = x;
       if (!e5m2) h = ((x & 0xC000C000u) | ((x >> 1) & 0x3F803F80u)) ^ 0x20002000u;
       if constexpr (std::is_same<T, __nv_bfloat16>::value) {
         const float2 f = __half22float2(u32_as_h2(h));
         h = b2_as_u32(__floats2bfloat162_rn(f.x, f.y));
       }
-      out[2 * i + j] = MODE == 1 ? mul2<T>(h, s2) : h;
+      out[j] = MODE == 1 ? mul2<T>(h, c.s2) : h;
+    }
+  } else if constexpr (BITS == 4) {
+    const uint4 p0 = lds128(src), p1 = lds128(src + 16);
+    const uint32_t w[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};   // word j = k 8j .. 8j + 7
+    if constexpr (IL && FMT == 0) {
+      // interleaved: the pair (2t, 2t+1) of a word is nibble t of its low and high half
+#pragma unroll
+      for (int j = 0; j < 8; ++j) out[j] = fin(lop3_and_or(w[j] >> (4 * t), 0x000f000fu, M));
+    } else {
+      // compressed: the pair (2t, 2t+1) of a word is its byte t (low nibble first)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t pk = gather_byte(w[4 * h], w[4 * h + 1], w[4 * h + 2], w[4 * h + 3], bsel);
+        if constexpr (FMT == 1) {
+          uint32_t v[4];
+          lut4_decode8(pk, lut, v);
+#pragma unroll
+          for (int i = 0; i < 4; ++i) out[4 * h + i] = MODE == 1 ? mul2<T>(v[i], c.s2) : v[i];
+        } else {
+          const uint32_t lo = pk & 0x0f0f0f0fu, hi = (pk >> 4) & 0x0f0f0f0fu;
+          const uint32_t x = __byte_perm(lo, hi, 0x5140), y = __byte_perm(lo, hi, 0x7362);
+          out[4 * h + 0] = fin(__byte_perm(x, MBYTES, 0x4140));
+          out[4 * h + 1] = fin(__byte_perm(x, MBYTES, 0x4342));
+          out[4 * h + 2] = fin(__byte_perm(y, MBYTES, 0x4140));
+          out[4 * h + 3] = fin(__byte_perm(y, MBYTES, 0x4342));
+        }
+      }
+    }
+  } else {
+    const uint4 pk = lds128(src);
+    const uint32_t w[4] = {pk.x, pk.y, pk.z, pk.w};   // word s = k 16s .. 16s + 15
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      if constexpr (IL) {
+        // interleaved: bytes (even 0-7, odd 0-7, even 8-15, odd 8-15) -- decode_u2x16_raw_interleaved
+        const uint32_t lo = __byte_perm(w[s], 0, 0x4140), hi = __byte_perm(w[s], 0, 0x4342);
+        out[2 * s] = fin(lop3_and_or(lo >> (2 * t), 0x00030003u, M));
+        out[2 * s + 1] = fin(lop3_and_or(hi >> (2 * t), 0x00030003u, M));
+      } else {
+        // compressed: e_{2t}, e_{2t+1} at bits 4t, 4t + 2; e_{2t+8}, e_{2t+9} 16 bits up
+        const uint32_t x = w[s] >> (4 * t);
+        const uint32_t L = lop3_and_or(x, 0x00030003u, M), H = lop3_and_or(x >> 2, 0x00030003u, M);
+        out[2 * s] = fin(__byte_perm(L, H, 0x5410));
+        out[2 * s + 1] = fin(__byte_perm(L, H, 0x7632));
+      }
     }
   }
 }
 
+// int8 activations (k32 steps): the quad at k = 32s + 4t of word (4-bit: 4s + t/2; 2-bit: 2s), and 16 further.
 template <int BITS, bool IL>
-__device__ __forceinline__ void dequant_half_row_i8(uint32_t src, uint32_t (&out)[16], uint32_t zp4) {
-  if constexpr (BITS == 2) {
-    const uint4 pk = lds128(src);
-    const uint32_t w[4] = {pk.x, pk.y, pk.z, pk.w};
+__device__ __forceinline__ void dequant_row_i8(uint32_t src, int t, uint32_t (&out)[8], uint32_t zp4) {
+  const uint32_t orv = zp4 ? 0x80808080u : 0u;
+  if constexpr (BITS == 4) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      uint32_t h[4];
+    for (int j = 0; j < 8; ++j) {
+      const uint32_t w = lds32(src + uint32_t((j >> 1) * 4 + (j & 1) * 2 + (t >> 1)) * 4u);
+      uint32_t h;
       if constexpr (IL) {
-        decode_u2x16_to_u8(w[i], zp4 ? 0x80808080u : 0u, h);
+        h = lop3_and_or(w >> (4 * (t & 1)), 0x0f0f0f0fu, orv);   // elements 0-3: low nibbles, 4-7: high nibbles
       } else {
-        const uint32_t orv = zp4 ? 0x80808080u : 0u;
-        const uint32_t s0 = lop3_and_or(w[i], 0x03030303u, orv), s1 = lop3_and_or(w[i] >> 2, 0x03030303u, orv),
-                       s2 = lop3_and_or(w[i] >> 4, 0x03030303u, orv), s3 = lop3_and_or(w[i] >> 6, 0x03030303u, orv);
-        const uint32_t a = __byte_perm(s0, s1, 0x5140), b = __byte_perm(s2, s3, 0x5140);
-        const uint32_t a2 = __byte_perm(s0, s1, 0x7362), b2 = __byte_perm(s2, s3, 0x7362);
-        h[0] = __byte_perm(a, b, 0x5410); h[1] = __byte_perm(a, b, 0x7632);
-        h[2] = __byte_perm(a2, b2, 0x5410); h[3] = __byte_perm(a2, b2, 0x7632);
+        const uint32_t x = w >> (16 * (t & 1));
+        h = __byte_perm(lop3_and_or(x, 0x0f0f0f0fu, orv), lop3_and_or(x >> 4, 0x0f0f0f0fu, orv), 0x5140);
       }
-#pragma unroll
-      for (int j = 0; j < 4; ++j) out[4 * i + j] = zp4 ? bytes_sub_zp(h[j], zp4) : h[j];
+      out[j] = zp4 ? bytes_sub_zp(h, zp4) : h;
     }
   } else {
-    const uint4 p0 = lds128(src);
-    const uint4 p1 = lds128(src + 16);
-    const uint32_t w[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
+    const uint4 p0 = lds128(src), p1 = lds128(src + 16);
+    const uint32_t w[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};   // word j = k 16j .. 16j + 15
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      uint32_t h[2];
+    for (int j = 0; j < 8; ++j) {
+      uint32_t h;
       if constexpr (IL) {
-        decode_u4x8_to_u8(w[i], zp4 ? 0x80808080u : 0u, h);
+        h = lop3_and_or(w[j] >> (2 * t), 0x03030303u, orv);          // decode_u2x16_to_u8
       } else {
-        const uint32_t orv = zp4 ? 0x80808080u : 0u;
-        const uint32_t t = lop3_and_or(w[i], 0x0f0f0f0fu, orv), u = lop3_and_or(w[i] >> 4, 0x0f0f0f0fu, orv);
-        h[0] = __byte_perm(t, u, 0x5140); h[1] = __byte_perm(t, u, 0x7362);
+        const uint32_t v = __byte_perm(w[j], 0, uint32_t(t) * 0x1111u);  // byte t (elements 4t .. 4t + 3) in every byte
+        h = (v & 0x03u) | ((v >> 2) & 0x0300u) | ((v >> 4) & 0x030000u) | ((v >> 6) & 0x03000000u) | orv;
       }
-#pragma unroll
-      for (int j = 0; j < 2; ++j) out[2 * i + j] = zp4 ? bytes_sub_zp(h[j], zp4) : h[j];
+      out[j] = zp4 ? bytes_sub_zp(h, zp4) : h;
     }
   }
 }
+
+// Per-row group parameters, fetched one group ahead so their latency never sits in front of a decode.
+template <int MODE, int BITS>
+struct RowGroup {
+  const uint16_t* sc;
+  const uint16_t* z;
+  const uint8_t* qz;
+  size_t qz_stride;
+  uint32_t qz_shift;
+  uint16_t s_raw = 0, z_raw = 0;
+  uint32_t qz_raw = 0;
+  __device__ __forceinline__ void fetch(int gi) {
+    if constexpr (MODE != 0) s_raw = __ldg(sc + gi);
+    if constexpr (MODE == 2 || MODE == 3) z_raw = __ldg(z + gi);
+    if constexpr (MODE == 4) qz_raw = __ldg(qz + size_t(gi) * qz_stride);
+  }
+  __device__ __forceinline__ void apply(DqConst& c, uint32_t magic) const {
+    c.s2 = uint32_t(s_raw) * 0x00010001u;
+    if constexpr (MODE == 2 || MODE == 3) {
+      c.z2 = uint32_t(z_raw) * 0x00010001u;
+      c.negz2 = c.z2 ^ 0x80008000u;
+    }
+    if constexpr (MODE == 4) c.mz_lo = magic + ((qz_raw >> qz_shift) & ((1u << BITS) - 1u)) * 0x00010001u;
+  }
+};
 
 // FMT: 0 = integer formats (LOP3 magic-number decode), 1 = 16-entry table formats (NF4 / fp4; BITS = 4, compressed storage),
 //      2 = 8-bit float weights (e4m3 / e5m2; BITS = 8)
 template <typename T, int BITS, int BM, bool IL, int FMT = 0>
-__global__ void __launch_bounds__(TS_THREADS, BM <= 128 ? 2 : 1)
+__global__ void __launch_bounds__(TS_THREADS, 1)
 gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const TsParams p) {
   using SM = TsSmem<T, BITS, BM>;
   using EI = ElemInfo<T>;
-  // the pipeline depth is a launch parameter only where two CTAs share an SM (BM <= 128: split-K / small grids); the
-  // large-tile instance keeps it a compile-time constant (stage addressing folds into immediates: measured -12 % time)
-  const int S = BM > 128 ? SM::kStages : p.stages;
+  constexpr int S = SM::kStages;
   constexpr int KB = EI::kKB;
   constexpr int PRB = SM::kPRB;
   constexpr bool INT8 = EI::kInt8;
-  constexpr int ACOL0 = TsTmem<BM>::kAcol0;
-  constexpr int NCOLS = TsTmem<BM>::kCols;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sW = smem + S * SM::kActBytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * SM::kStageBytes);
-  uint64_t* full = bars;                 // [S]   TMA -> dequant + MMA
-  uint64_t* empty = bars + S;            // [S]   MMA commit -> TMA
-  uint64_t* a_ready = bars + 2 * S;      // [TA]  dequant -> MMA
-  uint64_t* a_free = a_ready + TA_SLOTS; // [TA]  MMA commit -> dequant
-  uint64_t* acc_full = a_free + TA_SLOTS;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
+  uint64_t* full = bars;                 // [S]   TMA -> consumers
+  uint64_t* empty = bars + S;            // [S]   consumer warps -> TMA
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // split-K exists only for the small-M instances (BM <= 128); the large-tile instance keeps these compile-time constants
-  constexpr bool SPLITK = BM <= 128;
-  const int split = SPLITK ? blockIdx.x % p.splits : 0;
-  const int tile = SPLITK ? blockIdx.x / p.splits : blockIdx.x;
+  const int split = blockIdx.x % p.splits;
+  const int tile = blockIdx.x / p.splits;
   const int m_tile = tile % p.m_tiles;
   const int n_tile = tile / p.m_tiles;
-  const int kb0 = SPLITK ? split * p.kb_per_split : 0;  // first k-block of this CTA
+  const int kb0 = split * p.kb_per_split;  // first k-block of this CTA
   const int m0 = m_tile * BM, n0 = n_tile * TS_ROWS;
-  const int num_kb = SPLITK ? p.kb_per_split : p.K / KB;
+  const int num_kb = p.kb_per_split;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == TS_CONSUMER_WARPS && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmW);
-    for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < TA_SLOTS; ++i) { mbar_init(&a_ready[i], DQ_WARPS / dq_groups(BM)); mbar_init(&a_free[i], 1); }
-    mbar_init(acc_full, 1);
+    for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], TS_CONSUMER_WARPS); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<NCOLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == TS_CONSUMER_WARPS) {
     // ===== TMA producer =====
     if (lane == 0) {
       int s = 0;
@@ -444,297 +352,178 @@ gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (++s == S) { s = 0; par ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      uint32_t idesc;
-      if constexpr (INT8) {
-        const uint32_t a_signed = p.zp_const ? 1u : 0u;
-        idesc = (2u << 4) | (a_signed << 7) | (1u << 10) | (uint32_t(BM >> 3) << 17) | (uint32_t(TS_ROWS >> 4) << 24);
-      } else {
-        const uint32_t f = std::is_same<T, __nv_bfloat16>::value ? 1u : 0u;
-        idesc = (1u << 4) | (f << 7) | (f << 10) | (uint32_t(BM >> 3) << 17) | (uint32_t(TS_ROWS >> 4) << 24);
-      }
-      int s = 0, t = 0;
-      uint32_t spar = 0, tpar = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[s], spar);
-        mbar_wait(&a_ready[t], tpar);
-        tc_fence_after();
-        const uint64_t bdesc = make_sw128_desc(smem_u32(sA + s * SM::kActBytes));
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          tc_mma_ts<INT8>(tmem_base, tmem_base + ACOL0 + t * 32 + kk * 8, bdesc + uint64_t(kk * 2), idesc,
-                          (kb > 0 || kk > 0) ? 1u : 0u);
-        }
-        tc_commit(&empty[s]);
-        tc_commit(&a_free[t]);
-        if (++s == S) { s = 0; spar ^= 1; }
-        if (++t == TsTmem<BM>::kSlots) { t = 0; tpar ^= 1; }
-      }
-      tc_commit(acc_full);
-    }
-  } else {
-    // ===== dequant warps (then epilogue) =====
-    const int quad = warp & 3;                         // TMEM lane quadrant this warp may touch
-    constexpr int DQ_GROUPS = dq_groups(BM);
-    constexpr int DQ_WARPS_PER_GROUP = DQ_WARPS / DQ_GROUPS;
-    constexpr bool WHOLE_ROW = DQ_GROUPS == 4;          // this thread decodes both halves of its row
-    const int half = WHOLE_ROW ? 0 : ((warp - 2) >> 2) & 1;   // which half of the k-block's columns (2-group organisation)
-    const int grp = (warp - 2) / DQ_WARPS_PER_GROUP;   // which k-blocks (kb % DQ_GROUPS == grp)
-    const int row = quad * 32 + lane;       // weight row inside the tile == TMEM lane
-    const int n = n0 + row;
-    const uint32_t lane_addr = tmem_base + (uint32_t(quad * 32) << 16);
-    constexpr uint32_t MAGIC = INT8 ? 0u : TypeTraits<typename std::conditional<INT8, __half, T>::type>::kMagic;
-    using TF = typename std::conditional<INT8, __half, T>::type;  // float-ish type for the 16-bit path
+    return;
+  }
 
-    constexpr bool HI = IL && !INT8 && std::is_same<TF, __half>::value && BITS == 4;
-    constexpr uint32_t MAGIC_HI = HI ? 0x54005400u : MAGIC;
-    constexpr int ZSH = HI ? 16 : 1;  // odd-nibble values are 64 + u: the folded zero point sits 4 mantissa bits up
-    constexpr int NSLOT = TsTmem<BM>::kSlots;
-    constexpr int SPG = NSLOT / DQ_GROUPS;   // operand slots per dequant group (1 or 2)
-    static_assert(NSLOT <= TA_SLOTS && SPG * DQ_GROUPS == NSLOT && (SPG == 1 || SPG == 2), "slot ownership is static per group");
-    const int kb_per_g = p.g / KB;
-    const uint16_t* sc_row = reinterpret_cast<const uint16_t*>(p.scale) + size_t(n) * p.G;
-    const uint16_t* z_row = reinterpret_cast<const uint16_t*>(p.zeros) + size_t(n) * p.G;
+  // ===== consumer warpgroups: decode + wgmma, then the epilogue =====
+  const int g8 = lane >> 2, t = lane & 3;
+  const int rA = (warp >> 2) * 64 + (warp & 3) * 16 + g8;   // fragment rows rA and rA + 8 of this thread (tile-local)
+  const int nA = n0 + rA, nB = nA + 8;
+  using TF = typename std::conditional<INT8, __half, T>::type;  // 16-bit element type of the float path
+  constexpr uint32_t MAGIC = INT8 ? 0u : TypeTraits<TF>::kMagic;
+  using Acc = typename std::conditional<INT8, uint32_t, float>::type;
+  Acc acc[BM / 2];
+#pragma unroll
+  for (int i = 0; i < BM / 2; ++i) acc[i] = Acc(0);
+
+  Lut4 lut4;
+  if constexpr (FMT == 1) lut4_init(lut4, p.w_fmt, std::is_same<TF, __nv_bfloat16>::value, p.lut);
+  const bool e5m2 = p.w_fmt == BB_W_FP8_E5M2;
+  const uint32_t zp4 = uint32_t(p.zp_const) * 0x01010101u;
+  const uint32_t srcA = smem_u32(sW) + uint32_t(rA * PRB), srcB = srcA + 8u * PRB;
+
+  auto main_loop = [&](auto mode_tag) {
+    constexpr int MODE = decltype(mode_tag)::value;
+    DqConst cA, cB;
+    cA.mz_lo = cA.mz_hi = MAGIC + uint32_t(p.zp_const) * 0x00010001u;
+    cA.z2 = cA.s2 = cA.negz2 = 0;
+    cB = cA;
+    RowGroup<MODE, BITS> gA, gB;
     constexpr int EPB = 8 / BITS;
-    const uint8_t* qz_col = reinterpret_cast<const uint8_t*>(p.zeros) + n / EPB;
-    const size_t qz_stride = size_t(p.N) * BITS / 8;
-    const uint32_t qz_shift = BITS * (n % EPB);
-    const uint32_t src0 = smem_u32(sW) + row * PRB + half * (PRB / 2);
-    const uint32_t tdst0 = lane_addr + ACOL0 + half * 16;
+    gA.sc = reinterpret_cast<const uint16_t*>(p.scale) + size_t(nA) * p.G;
+    gB.sc = reinterpret_cast<const uint16_t*>(p.scale) + size_t(nB) * p.G;
+    gA.z = reinterpret_cast<const uint16_t*>(p.zeros) + size_t(nA) * p.G;
+    gB.z = reinterpret_cast<const uint16_t*>(p.zeros) + size_t(nB) * p.G;
+    gA.qz = reinterpret_cast<const uint8_t*>(p.zeros) + nA / EPB;
+    gB.qz = reinterpret_cast<const uint8_t*>(p.zeros) + nB / EPB;
+    gA.qz_stride = gB.qz_stride = size_t(p.N) * BITS / 8;
+    gA.qz_shift = BITS * (nA % EPB);
+    gB.qz_shift = BITS * (nB % EPB);
+    const int kb_per_g = p.g / KB;
+    int gi = kb0 / kb_per_g;                 // group of the next k-block
+    int g_end = gi * kb_per_g - kb0;         // CTA-local k-block at which group gi starts (<= 0 for the first)
+    if constexpr (MODE != 0) { gA.fetch(gi); gB.fetch(gi); }
 
-    Lut4 lut4;
-    if constexpr (FMT == 1) lut4_init(lut4, p.w_fmt, std::is_same<TF, __nv_bfloat16>::value, p.lut);
-    auto dq_loop = [&](auto mode_tag) {
-      constexpr int MODE = decltype(mode_tag)::value;
-      DqConst c;
-      c.mz_lo = MAGIC + uint32_t(p.zp_const) * 0x00010001u;
-      c.mz_hi = MAGIC_HI + uint32_t(p.zp_const * ZSH) * 0x00010001u;
-      c.z2 = c.s2 = c.negz2 = 0;
-      // group parameters are fetched one needed-group ahead so their latency never sits in front of a decode
-      uint16_t s_raw = 0, z_raw = 0;
-      uint32_t qz_raw = 0;
-      auto fetch_group = [&](int gi) {
-        if constexpr (MODE != 0) s_raw = __ldg(sc_row + gi);
-        if constexpr (MODE == 2 || MODE == 3) z_raw = __ldg(z_row + gi);
-        if constexpr (MODE == 4) qz_raw = __ldg(qz_col + size_t(gi) * qz_stride);
-      };
-      int gi = (kb0 + grp) / kb_per_g;         // group of this warp's first k-block
-      int g_end = (gi + 1) * kb_per_g - kb0;   // first (CTA-local) k-block of the next group
-      bool fresh = true;
-      if constexpr (MODE != 0) fetch_group(gi);
-      int st = grp;                      // smem stage of kb (S % DQ_GROUPS == 0 keeps stage parity per group)
-      uint32_t full_par = 0;
-      uint32_t it = 0;                   // iteration count of this warp: slot = grp + DQ_GROUPS * (it mod SPG)
-      int prev_slot = -1;
-      const bool early_publish = S < DQ_GROUPS + 2;
-      for (int kb = grp; kb < num_kb; kb += DQ_GROUPS) {
-        if constexpr (MODE != 0) {
-          if (kb >= g_end) {
-            do { gi += 1; g_end += kb_per_g; } while (kb >= g_end);
-            fresh = true;
-          }
-          if (fresh) {
-            fresh = false;
-            c.s2 = uint32_t(s_raw) * 0x00010001u;
-            if constexpr (MODE == 2 || MODE == 3) {
-              c.z2 = uint32_t(z_raw) * 0x00010001u;
-              c.negz2 = c.z2 ^ 0x80008000u;
-            }
-            if constexpr (MODE == 4) {
-              const uint32_t zq = (qz_raw >> qz_shift) & ((1u << BITS) - 1u);
-              c.mz_lo = MAGIC + zq * 0x00010001u;
-              c.mz_hi = MAGIC_HI + (zq * ZSH) * 0x00010001u;
-            }
-            // prefetch the parameters of the group this warp enters next: its first own k-block at or past g_end (the
-            // stride DQ_GROUPS need not divide the group length -- g = 192 with four dequant groups skips 1 or 2 groups)
-            const int kbn = kb + ((g_end - kb + DQ_GROUPS - 1) / DQ_GROUPS) * DQ_GROUPS;
-            const int gn = gi + 1 + (kbn - g_end) / kb_per_g;
-            if (kbn < num_kb && gn < p.G) fetch_group(gn);
-          }
+    int st = 0;
+    uint32_t full_par = 0;
+    int prev_st = -1;
+    auto step = [&](int kb, uint32_t (&fa)[8], uint32_t (&fb)[8]) {
+      if constexpr (MODE != 0) {
+        if (kb >= g_end) {   // entering group gi: its parameters were fetched one group ago; fetch the next one now
+          gA.apply(cA, MAGIC);
+          gB.apply(cB, MAGIC);
+          g_end += kb_per_g;
+          ++gi;
+          if (gi < p.G && g_end < num_kb) { gA.fetch(gi); gB.fetch(gi); }
         }
-        // The previous k-block's slot is normally published AFTER this block's first decode (its tcgen05.st hides behind
-        // it).  With a pipeline no deeper than the group stride that order deadlocks: TMA(kb) waits for MMA(kb - S), which
-        // waits for exactly the slot this warp would publish only after TMA(kb) has landed -- publish first then.
-        if (early_publish && prev_slot >= 0) {
-          tmem_wait_st();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&a_ready[prev_slot]);
-          prev_slot = -1;
-        }
-        mbar_wait(&full[st], full_par);
-        uint32_t regs[16];
-        if constexpr (INT8) dequant_half_row_i8<BITS, IL>(src0 + st * SM::kWBytes, regs, uint32_t(p.zp_const) * 0x01010101u);
-        else if constexpr (FMT == 1) dequant_half_row_lut<TF, MODE>(src0 + st * SM::kWBytes, regs, lut4, c.s2);
-        else if constexpr (FMT == 2) dequant_half_row_fp8<TF, MODE>(src0 + st * SM::kWBytes, regs, p.w_fmt == BB_W_FP8_E5M2, c.s2);
-        else dequant_half_row<TF, BITS, MODE, IL>(src0 + st * SM::kWBytes, regs, c);
-        // publish the PREVIOUS k-block's TMEM slot only now: its tcgen05.st had the whole decode above to land
-        if (prev_slot >= 0) {
-          tmem_wait_st();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&a_ready[prev_slot]);
-        }
-        const int slot = grp + DQ_GROUPS * int(it & (SPG - 1));
-        if (it >= SPG) {   // the MMAs that read this slot's previous contents must be done
-          mbar_wait(&a_free[slot], ((it / SPG) - 1) & 1);
-          tc_fence_after();
-        }
-        tmem_st_x16(tdst0 + slot * 32, regs);
-        if constexpr (WHOLE_ROW) {
-          if constexpr (INT8) dequant_half_row_i8<BITS, IL>(src0 + st * SM::kWBytes + PRB / 2, regs, uint32_t(p.zp_const) * 0x01010101u);
-          else if constexpr (FMT == 1) dequant_half_row_lut<TF, MODE>(src0 + st * SM::kWBytes + PRB / 2, regs, lut4, c.s2);
-          else if constexpr (FMT == 2) dequant_half_row_fp8<TF, MODE>(src0 + st * SM::kWBytes + PRB / 2, regs, p.w_fmt == BB_W_FP8_E5M2, c.s2);
-          else dequant_half_row<TF, BITS, MODE, IL>(src0 + st * SM::kWBytes + PRB / 2, regs, c);
-          tmem_st_x16(tdst0 + slot * 32 + 16, regs);
-        }
-        prev_slot = slot;
-        ++it;
-        st += DQ_GROUPS;
-        if (st >= S) { st -= S; full_par ^= 1; }
       }
-      if (prev_slot >= 0) {
-        tmem_wait_st();
-        tc_fence_before();
+      mbar_wait(&full[st], full_par);
+      const uint32_t wofs = uint32_t(st * SM::kWBytes);
+      if constexpr (INT8) {
+        dequant_row_i8<BITS, IL>(srcA + wofs, t, fa, zp4);
+        dequant_row_i8<BITS, IL>(srcB + wofs, t, fb, zp4);
+      } else {
+        dequant_row<TF, BITS, MODE, IL, FMT>(srcA + wofs, t, fa, cA, lut4, e5m2);
+        dequant_row<TF, BITS, MODE, IL, FMT>(srcB + wofs, t, fb, cB, lut4, e5m2);
+      }
+      const uint64_t bdesc = make_sw128_desc(smem_u32(sA + st * SM::kActBytes));
+      wgmma_fence();
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        const uint32_t a[4] = {fa[2 * s], fb[2 * s], fa[2 * s + 1], fb[2 * s + 1]};
+        if constexpr (INT8) {
+          if (p.zp_const) Wgmma<BM>::template i8<true>(acc, a, bdesc + uint64_t(2 * s), 1u);
+          else Wgmma<BM>::template i8<false>(acc, a, bdesc + uint64_t(2 * s), 1u);
+        } else {
+          Wgmma<BM>::template f16<TF>(acc, a, bdesc + uint64_t(2 * s), 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();   // the MMAs of the previous k-block are done: its fragments and smem stage are free
+      if (prev_st >= 0) {
         __syncwarp();
-        if (lane == 0) mbar_arrive(&a_ready[prev_slot]);
+        if (lane == 0) mbar_arrive(&empty[prev_st]);
       }
+      prev_st = st;
+      if (++st == S) { st = 0; full_par ^= 1; }
     };
-    if constexpr (INT8) {
-      dq_loop(std::integral_constant<int, 0>{});
-    } else if constexpr (FMT != 0) {   // table / fp8 formats: no zero points on the fast path (gemm_ts_supported)
-      if (p.mode == 0) dq_loop(std::integral_constant<int, 0>{}); else dq_loop(std::integral_constant<int, 1>{});
-    } else {
-      switch (p.mode) {
-        case 0: dq_loop(std::integral_constant<int, 0>{}); break;
-        case 1: dq_loop(std::integral_constant<int, 1>{}); break;
-        case 2: dq_loop(std::integral_constant<int, 2>{}); break;
-        case 3: dq_loop(std::integral_constant<int, 3>{}); break;
-        default: dq_loop(std::integral_constant<int, 4>{}); break;
-      }
+    uint32_t fa0[8], fb0[8], fa1[8], fb1[8];
+    int kb = 0;
+    for (; kb + 1 < num_kb; kb += 2) {
+      step(kb, fa0, fb0);
+      step(kb + 1, fa1, fb1);
     }
+    if (kb < num_kb) step(kb, fa0, fb0);
+    wgmma_wait<0>();
+  };
+  if constexpr (INT8) {
+    main_loop(std::integral_constant<int, 0>{});
+  } else if constexpr (FMT != 0) {   // table / fp8 formats: no zero points on the fast path (gemm_ts_supported)
+    if (p.mode == 0) main_loop(std::integral_constant<int, 0>{}); else main_loop(std::integral_constant<int, 1>{});
+  } else {
+    switch (p.mode) {
+      case 0: main_loop(std::integral_constant<int, 0>{}); break;
+      case 1: main_loop(std::integral_constant<int, 1>{}); break;
+      case 2: main_loop(std::integral_constant<int, 2>{}); break;
+      case 3: main_loop(std::integral_constant<int, 3>{}); break;
+      default: main_loop(std::integral_constant<int, 4>{}); break;
+    }
+  }
 
-    // ----- epilogue: accumulator[lane = n, column = m] -> C[m, n] -----
-    mbar_wait(acc_full, 0);
-    tc_fence_after();
-    constexpr int CPH = BM / 4;                  // accumulator columns per warp (4 warps share a lane quadrant)
-    constexpr int CH = CPH < 16 ? CPH : 16;      // columns per tcgen05.ld
-    static_assert(CPH % CH == 0 && (CH == 16 || CH == 8), "BM must be >= 32");
-    float bias_f = 0.f;
-    if (p.bias) {
-      if (p.a_dtype == BB_F16) bias_f = __half2float(reinterpret_cast<const __half*>(p.bias)[n]);
-      else if (p.a_dtype == BB_BF16) bias_f = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.bias)[n]);
-      else bias_f = float(reinterpret_cast<const int8_t*>(p.bias)[n]);
+  // ----- epilogue: acc[4i + 2h + j] = C^T[row rA + 8h][column 8i + 2t + j] -> C[m, n] -----
+  float bias_f[2] = {0.f, 0.f};
+  if (p.bias) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int n = h ? nB : nA;
+      if (p.a_dtype == BB_F16) bias_f[h] = __half2float(reinterpret_cast<const __half*>(p.bias)[n]);
+      else if (p.a_dtype == BB_BF16) bias_f[h] = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.bias)[n]);
+      else bias_f[h] = float(reinterpret_cast<const int8_t*>(p.bias)[n]);
     }
-    const int combo = WHOLE_ROW ? grp : grp * 2 + half;   // the four quadrant warps with equal `combo` own the same CPH columns
-    const int cbase = combo * CPH;
-    void* const C0 = p.out.ptr[0];
-    const int ndst = p.out.n;
-    const size_t ld = size_t(p.out.ld), col0 = size_t(p.out.col0);
-    if (!INT8 && p.staged_epi && !(SPLITK && p.splits > 1)) {
-      // Staged epilogue (fp16 / bf16 outputs).  The accumulator is [lane = n][column = m]; stored straight from registers a
-      // warp instruction covers 32 consecutive n of ONE row m with 2-byte elements -- 64 bytes per instruction and, on the
-      // column-parallel path, per peer: 8 destinations x 2-byte stores over NVLink (round-1 verdict: 4 -> 8 GPUs bought 7 %).
-      // Here the four quadrant warps of a column range transpose their [128 n] x [CPH m] tile through the (now idle) pipeline
-      // smem and write 256-byte row segments with 16-byte stores: 1/8 of the store instructions, full 128-byte lines per peer.
-      uint8_t* tile = smem + combo * (CPH * 256);
-      const uint32_t tcol = smem_u32(tile) + uint32_t(quad * 32 + lane) * 2u;
-      for (int c0 = cbase; c0 < cbase + CPH; c0 += CH) {
-        if (m0 + c0 >= p.M) break;  // uniform over the four warps
-        uint32_t v[16];
-        if constexpr (CH == 16) tmem_ld_x16(lane_addr + c0, v); else tmem_ld_x8(lane_addr + c0, v);
-        tmem_wait_ld();
+  }
+  void* const C0 = p.out.ptr[0];
+  const int ndst = p.out.n;
+  const size_t ld = size_t(p.out.ld), col0 = size_t(p.out.col0);
 #pragma unroll
-        for (int c = 0; c < CH; ++c) {
-          const float acc = __uint_as_float(v[c]);
-          uint16_t bits;
-          if (p.out_dtype == BB_F16) {
-            __half h = __float2half_rn(acc);
-            if (p.bias) h = __hadd(h, __float2half_rn(bias_f));
-            bits = __half_as_ushort(h);
-          } else {
-            __nv_bfloat16 h = __float2bfloat16_rn(acc);
-            if (p.bias) h = __hadd(h, __float2bfloat16_rn(bias_f));
-            bits = __bfloat16_as_ushort(h);
-          }
-          asm volatile("st.shared.u16 [%0], %1;" ::"r"(tcol + uint32_t(c0 - cbase + c) * 256u), "h"(bits) : "memory");
-        }
-      }
-      asm volatile("bar.sync %0, %1;" ::"r"(1 + combo), "n"(128) : "memory");
-      const int rows_valid = min(CPH, p.M - (m0 + cbase));
-      const int t128 = quad * 32 + lane;
-#pragma unroll 1
-      for (int id = t128; id < CPH * 16; id += 128) {
-        const int row = id >> 4, c16 = id & 15;
-        if (row >= rows_valid) break;
-        uint4 q;
-        asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(q.x), "=r"(q.y), "=r"(q.z), "=r"(q.w)
-                     : "r"(smem_u32(tile) + uint32_t(row) * 256u + uint32_t(c16) * 16u));
-        const size_t o = (size_t(m0 + cbase + row) * ld + col0 + size_t(n0) + size_t(c16) * 8u) * 2u;
-        *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(C0) + o) = q;
-        for (int d = 1; d < ndst; ++d) *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(p.out.ptr[d]) + o) = q;
-      }
-    } else
-    for (int c0 = cbase; c0 < cbase + CPH; c0 += CH) {
-      if (m0 + c0 >= p.M) break;  // warp-uniform
-      uint32_t v[16];
-      if constexpr (CH == 16) tmem_ld_x16(lane_addr + c0, v); else tmem_ld_x8(lane_addr + c0, v);
-      tmem_wait_ld();
+  for (int i = 0; i < BM / 8; ++i) {
 #pragma unroll
-      for (int c = 0; c < CH; ++c) {
-        const int m = m0 + c0 + c;
-        if (m >= p.M) break;
-        if (SPLITK && p.splits > 1) {  // raw partial accumulator; bias / cast / scatter happen in splitk_reduce_kernel
-          reinterpret_cast<uint32_t*>(p.ws)[(size_t(split) * p.M + m) * p.N + n] = v[c];
+    for (int j = 0; j < 2; ++j) {
+      const int m = m0 + 8 * i + 2 * t + j;
+      if (m >= p.M) continue;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const Acc v = acc[4 * i + 2 * h + j];
+        const int n = h ? nB : nA;
+        if (p.splits > 1) {  // raw partial accumulator; bias / cast / scatter happen in splitk_reduce_kernel
+          reinterpret_cast<Acc*>(p.ws)[(size_t(split) * p.M + m) * p.N + n] = v;
           continue;
         }
         const size_t o = size_t(m) * ld + col0 + size_t(n);
-        // destination 0 (the local output, or this rank's own copy) takes the straight-line path the single-GPU kernel
-        // always had; the peers' copies (column-parallel scatter, NVLink) follow in a loop that is empty otherwise --
-        // indexing the pointer table per element cost ~9 % of the M=4096 GEMM
+        // destination 0 (the local output, or this rank's own copy) takes the straight-line path; the peers' copies
+        // (column-parallel scatter) follow in a loop that is empty otherwise
         if constexpr (INT8) {
-          const int acc = int(v[c]);
-          const int b = int(bias_f);
+          const int a = int(v);
+          const int b = int(bias_f[h]);
           auto put = [&](void* Cd) {
             switch (p.out_dtype) {
-              case BB_I32: reinterpret_cast<int*>(Cd)[o] = acc + b; break;
-              case BB_I8: reinterpret_cast<int8_t*>(Cd)[o] = int8_t(int8_t(acc) + b); break;
-              case BB_F32: reinterpret_cast<float*>(Cd)[o] = float(acc) + float(b); break;
-              case BB_F16: reinterpret_cast<__half*>(Cd)[o] = __hadd(__int2half_rn(acc), __int2half_rn(b)); break;
-              default: reinterpret_cast<__nv_bfloat16*>(Cd)[o] = __hadd(__int2bfloat16_rn(acc), __int2bfloat16_rn(b));
+              case BB_I32: reinterpret_cast<int*>(Cd)[o] = a + b; break;
+              case BB_I8: reinterpret_cast<int8_t*>(Cd)[o] = int8_t(int8_t(a) + b); break;
+              case BB_F32: reinterpret_cast<float*>(Cd)[o] = float(a) + float(b); break;
+              case BB_F16: reinterpret_cast<__half*>(Cd)[o] = __hadd(__int2half_rn(a), __int2half_rn(b)); break;
+              default: reinterpret_cast<__nv_bfloat16*>(Cd)[o] = __hadd(__int2bfloat16_rn(a), __int2bfloat16_rn(b));
             }
           };
           put(C0);
           for (int d = 1; d < ndst; ++d) put(p.out.ptr[d]);
         } else {
-          const float acc = __uint_as_float(v[c]);
           if (p.out_dtype == BB_F16) {
-            __half h = __float2half_rn(acc);
-            if (p.bias) h = __hadd(h, __float2half_rn(bias_f));
-            reinterpret_cast<__half*>(C0)[o] = h;
-            for (int d = 1; d < ndst; ++d) reinterpret_cast<__half*>(p.out.ptr[d])[o] = h;
+            __half r = __float2half_rn(v);
+            if (p.bias) r = __hadd(r, __float2half_rn(bias_f[h]));
+            reinterpret_cast<__half*>(C0)[o] = r;
+            for (int d = 1; d < ndst; ++d) reinterpret_cast<__half*>(p.out.ptr[d])[o] = r;
           } else if (p.out_dtype == BB_BF16) {
-            __nv_bfloat16 h = __float2bfloat16_rn(acc);
-            if (p.bias) h = __hadd(h, __float2bfloat16_rn(bias_f));
-            reinterpret_cast<__nv_bfloat16*>(C0)[o] = h;
-            for (int d = 1; d < ndst; ++d) reinterpret_cast<__nv_bfloat16*>(p.out.ptr[d])[o] = h;
+            __nv_bfloat16 r = __float2bfloat16_rn(v);
+            if (p.bias) r = __hadd(r, __float2bfloat16_rn(bias_f[h]));
+            reinterpret_cast<__nv_bfloat16*>(C0)[o] = r;
+            for (int d = 1; d < ndst; ++d) reinterpret_cast<__nv_bfloat16*>(p.out.ptr[d])[o] = r;
           } else {
-            const float f = acc + (p.bias ? bias_f : 0.f);
+            const float f = v + (p.bias ? bias_f[h] : 0.f);
             reinterpret_cast<float*>(C0)[o] = f;
             for (int d = 1; d < ndst; ++d) reinterpret_cast<float*>(p.out.ptr[d])[o] = f;
           }
         }
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<NCOLS>(tmem_base);
   }
 }
 
@@ -824,7 +613,7 @@ int choose_splits(int tiles, int num_kb, int sms) {
   int best = 1;
   for (int sp = 2; sp <= 8; ++sp) {
     if (num_kb % sp || num_kb / sp < 8) continue;
-    if (tiles * sp <= 2 * sms) best = sp;  // two CTAs per SM are resident for BM <= 128
+    if (tiles * sp <= sms) best = sp;  // one CTA per SM
   }
   return best;
 }
@@ -895,30 +684,11 @@ int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
   p.m_tiles = (a.m + BM - 1) / BM;
   const int num_kb_total = a.d.K / EI::kKB;
   const int tiles = p.m_tiles * (a.d.N / TS_ROWS);
-  p.splits = BM <= 128 ? choose_splits(tiles, num_kb_total, device_sm_count()) : 1;
+  p.splits = a.m <= 128 ? choose_splits(tiles, num_kb_total, device_sm_count()) : 1;
   if (p.splits > 1 && a.workspace_bytes < size_t(p.splits) * a.m * a.d.N * 4) p.splits = 1;  // no scratch given
   p.kb_per_split = num_kb_total / p.splits;
   p.ws = a.workspace;
-  // two CTAs per SM when the kernel is split (or simply small): cap the pipeline so that 2 x smem fits
-  int stages = SM::kStages;
-  if (BM <= 128 && tiles * p.splits > device_sm_count()) {
-    // more CTAs than SMs: keep the pipeline shallow enough for two resident CTAs (their windows add up); with at most
-    // one CTA per SM the full depth is needed to cover the TMA latency
-    const int cap = ((110 * 1024 - SM::kBarBytes - 1024) / SM::kStageBytes) & ~1;
-    if (cap >= dq_groups(BM) && cap < stages) stages = cap;   // (a dequant group's first stage index is its group id)
-  }
-  p.stages = stages;
-  {
-    // staged epilogue: default on the column-parallel (multi-destination) path; BB_TS_STAGED=0/1 forces it.  Needs 16-byte
-    // aligned row segments in every destination and BM x 256 B of (idle) pipeline smem
-    static const int force = [] { const char* e = getenv("BB_TS_STAGED"); return e ? atoi(e) : -1; }();
-    const OutSpec& o = p.out;
-    bool ok = !EI::kInt8 && (a.d.out_dtype == BB_F16 || a.d.out_dtype == BB_BF16) && (o.ld % 8) == 0 && (o.col0 % 8) == 0 &&
-              size_t(stages) * SM::kStageBytes >= size_t(BM) * 256;
-    for (int i = 0; i < o.n && ok; ++i) ok = (reinterpret_cast<uintptr_t>(o.ptr[i]) & 15) == 0;
-    p.staged_epi = ok && (force < 0 ? o.n > 1 : force != 0) ? 1 : 0;
-  }
-  const size_t smem_bytes = size_t(stages) * SM::kStageBytes + SM::kBarBytes + 1024;
+  const size_t smem_bytes = SM::kTotal;
   CUtensorMap tmA, tmW;
   const CUtensorMapDataType adt = EI::kInt8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
                                             : (std::is_same<T, __half>::value ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
@@ -946,34 +716,16 @@ int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
   return 0;
 }
 
-template <typename T, int BITS, bool IL>
-int launch_ts_bm2(const MatmulArgs& a, const TsParams& p) {
-  if (a.m <= 32) return launch_ts_inst<T, BITS, 32, IL>(a, p);
-  if (a.m <= 64) return launch_ts_inst<T, BITS, 64, IL>(a, p);
-  if (a.m <= 128) return launch_ts_inst<T, BITS, 128, IL>(a, p);
-  // tuning hook: BB_TS_BM=128 runs large m on the 128-column tile (two CTAs per SM: one CTA's epilogue overlaps the other's main loop,
-  // at twice the decode work per output)
-  static const int force_bm = [] { const char* e = getenv("BB_TS_BM"); return e ? atoi(e) : 0; }();
-  if (force_bm == 128) return launch_ts_inst<T, BITS, 128, IL>(a, p);
-  return launch_ts_inst<T, BITS, 256, IL>(a, p);
-}
-template <typename T>
-int launch_ts_lut(const MatmulArgs& a, const TsParams& p) {
-  if (a.m <= 32) return launch_ts_inst<T, 4, 32, false, 1>(a, p);
-  if (a.m <= 64) return launch_ts_inst<T, 4, 64, false, 1>(a, p);
-  if (a.m <= 128) return launch_ts_inst<T, 4, 128, false, 1>(a, p);
-  return launch_ts_inst<T, 4, 256, false, 1>(a, p);
-}
-template <typename T>
-int launch_ts_fp8(const MatmulArgs& a, const TsParams& p) {
-  if (a.m <= 32) return launch_ts_inst<T, 8, 32, false, 2>(a, p);
-  if (a.m <= 64) return launch_ts_inst<T, 8, 64, false, 2>(a, p);
-  if (a.m <= 128) return launch_ts_inst<T, 8, 128, false, 2>(a, p);
-  return launch_ts_inst<T, 8, 256, false, 2>(a, p);
+// activation rows per CTA: the wgmma N extent (m > 128 runs several 128-row tiles)
+template <typename T, int BITS, bool IL, int FMT>
+int launch_ts_bm(const MatmulArgs& a, const TsParams& p) {
+  if (a.m <= 32) return launch_ts_inst<T, BITS, 32, IL, FMT>(a, p);
+  if (a.m <= 64) return launch_ts_inst<T, BITS, 64, IL, FMT>(a, p);
+  return launch_ts_inst<T, BITS, 128, IL, FMT>(a, p);
 }
 template <typename T, int BITS>
-int launch_ts_bm(const MatmulArgs& a, const TsParams& p) {
-  return a.d.w_layout == BB_LAYOUT_COMPRESSED ? launch_ts_bm2<T, BITS, false>(a, p) : launch_ts_bm2<T, BITS, true>(a, p);
+int launch_ts_layout(const MatmulArgs& a, const TsParams& p) {
+  return a.d.w_layout == BB_LAYOUT_COMPRESSED ? launch_ts_bm<T, BITS, false, 0>(a, p) : launch_ts_bm<T, BITS, true, 0>(a, p);
 }
 
 }  // namespace
@@ -1034,11 +786,13 @@ int launch_gemm_ts(const MatmulArgs& a) {
   p.out_dtype = d.out_dtype; p.a_dtype = d.a_dtype; p.m_tiles = 1;
   p.lut = d.w_fmt == BB_W_NF ? a.lut : nullptr;
   p.w_fmt = d.w_fmt;
-  if (d.w_fmt == BB_W_NF || d.w_fmt == BB_W_FP4) return d.a_dtype == BB_F16 ? launch_ts_lut<__half>(a, p) : launch_ts_lut<__nv_bfloat16>(a, p);
-  if (d.w_fmt == BB_W_FP8_E4M3 || d.w_fmt == BB_W_FP8_E5M2) return d.a_dtype == BB_F16 ? launch_ts_fp8<__half>(a, p) : launch_ts_fp8<__nv_bfloat16>(a, p);
-  if (d.a_dtype == BB_I8) return d.w_bits == 4 ? launch_ts_bm<int8_t, 4>(a, p) : launch_ts_bm<int8_t, 2>(a, p);
-  if (d.a_dtype == BB_F16) return d.w_bits == 4 ? launch_ts_bm<__half, 4>(a, p) : launch_ts_bm<__half, 2>(a, p);
-  return d.w_bits == 4 ? launch_ts_bm<__nv_bfloat16, 4>(a, p) : launch_ts_bm<__nv_bfloat16, 2>(a, p);
+  if (d.w_fmt == BB_W_NF || d.w_fmt == BB_W_FP4)
+    return d.a_dtype == BB_F16 ? launch_ts_bm<__half, 4, false, 1>(a, p) : launch_ts_bm<__nv_bfloat16, 4, false, 1>(a, p);
+  if (d.w_fmt == BB_W_FP8_E4M3 || d.w_fmt == BB_W_FP8_E5M2)
+    return d.a_dtype == BB_F16 ? launch_ts_bm<__half, 8, false, 2>(a, p) : launch_ts_bm<__nv_bfloat16, 8, false, 2>(a, p);
+  if (d.a_dtype == BB_I8) return d.w_bits == 4 ? launch_ts_layout<int8_t, 4>(a, p) : launch_ts_layout<int8_t, 2>(a, p);
+  if (d.a_dtype == BB_F16) return d.w_bits == 4 ? launch_ts_layout<__half, 4>(a, p) : launch_ts_layout<__half, 2>(a, p);
+  return d.w_bits == 4 ? launch_ts_layout<__nv_bfloat16, 4>(a, p) : launch_ts_layout<__nv_bfloat16, 2>(a, p);
 }
 
 }  // namespace bb

@@ -2,7 +2,7 @@
 //
 // Replaces the reference's generated SIMT GEMV (bitblas/ops/general_matmul/tilelang/dequantize/
 // gemv_dequantize_simt.py:164-262: 128-bit A loads, 4-byte packed-B loads, LOP3 decode, fp16 FMA /
-// __dp4a, shuffle all-reduce).  B200 design:
+// __dp4a, shuffle all-reduce).  Design:
 //   * the packed weights are the only HBM stream that matters (N*K*bits/8 bytes).  A warp owns 16 weight rows
 //     and a contiguous K range; KS warps (one CTA) split K for a row block.  KS is chosen on the host so that
 //     ~16 warps per SM are resident and EVERY CTA is resident at once: equal work per warp + a shared memory
@@ -33,10 +33,8 @@ namespace {
 
 constexpr int MAX_KS = 8;  // warps per CTA = K splits per 16-row block
 constexpr int PF = 4;      // weight steps in flight per warp (register queue of plain 128-bit ld.global.nc loads).
-                           // tools/membench.cu on B200, 12288^2 weights (profiles/r2_membench.txt): this pattern (16 rows x
-                           // 64 B per warp load, depth 4, 3 K-splits) reads at the linear-read rate (15.0 us per 75.5 MB
-                           // launch, of which ~4 us are launch gap and tail); the same addresses through cp.async (LDGSTS)
-                           // take 17.3 us, a depth-8 queue 17.2 us.
+                           // tools/membench.cu compares this pattern (16 rows x 64 B per warp load, depth 4, 3 K-splits)
+                           // with the linear-read rate, the same addresses through cp.async (LDGSTS) and deeper queues.
 
 struct GemvParams {
   const void* A;
@@ -83,8 +81,8 @@ __device__ __forceinline__ float raw_to_float(uint16_t b) {
 // Programmatic dependent launch (PDL).  A decode step is a chain of dependent GEMVs (qkv -> o -> gate_up -> down); the
 // weights, scales and zeros of the next one do not depend on the previous result, only its activations do.  Each streaming
 // kernel therefore (1) lets the next kernel in the stream start once every CTA of its own has finished its weight stream
-// (pdl_launch_dependents before the epilogue; triggering at kernel entry was measured: the early CTAs of kernel i+1 then
-// compete with kernel i and the big shapes got 15-20 % slower) and (2) starts its own weight prefetch immediately but
+// (pdl_launch_dependents before the epilogue; triggered at kernel entry, the early CTAs of kernel i+1
+// would compete with kernel i for the weight stream) and (2) starts its own weight prefetch immediately but
 // executes pdl_wait -- which
 // returns once the preceding kernel has completed and flushed -- before the first activation load.  Launch latency and the
 // first DRAM round trip of kernel i+1 then overlap the tail of kernel i.  Both instructions are no-ops when the launch
@@ -115,9 +113,8 @@ __device__ __forceinline__ void split_range(int total, int parts, int idx, int& 
 //   ZK: 0 no zeros (constant zero point of the "int" formats only), 1 "original", 2 "rescale", 3 "quantized"
 //   SC: with_scaling
 // ---------------------------------------------------------------------------------------------
-// (A variant that staged the activations and the row block's group parameters in shared memory before the weight stream was
-// measured and removed: 39.2 us vs 30.7 us on 12288^2 -- the staging prologue of a short-lived CTA costs more than the in-order
-// load stalls it removes.)
+// (Activations and group parameters are not staged in shared memory before the weight stream: the staging prologue of a
+// short-lived CTA costs more than the in-order load stalls it removes.)
 template <typename T, int BITS, bool IL, int NT, int ZK, bool SC>
 __global__ void __launch_bounds__(NT == 1 ? 128 : MAX_KS * 32)
 __maxnreg__(NT == 1 ? ((ZK == 1 || ZK == 2) ? 112 : 96) : (NT == 2 ? ((ZK == 1 || ZK == 2) ? 168 : 128) : ((ZK == 1 || ZK == 2) ? 232 : 192)))
@@ -416,8 +413,8 @@ gemv_mma_kernel(const GemvParams p) {
 //    as soon as chunk t sits in registers -- plus, whenever the stream enters a new window of 8 quantisation groups, the
 //    scales [16 rows x 8 groups] and packed zeros [8 groups x 16 B] into a 2-deep window ring.  The warps therefore issue
 //    NO global loads: nothing queues behind DRAM round trips (loads of a warp complete in order), all latency hiding is
-//    the ring's, and there are no inter-warp barriers at all.  (A dedicated producer warp serving 8 consumers was tried
-//    first: its serialised UTMALDG issue -- ~440 cycles per chunk -- capped the CTA at 2.6 TB/s chip-wide.)
+//    the ring's, and there are no inter-warp barriers at all.  (A dedicated producer warp serving 8 consumers
+//    would serialise the UTMALDG issue of the whole CTA.)
 //  * a range whose FIRST segment starts inside a row block parks that segment's fp32 partial sums in its workspace slot and
 //    raises a flag (a per-call 64-bit nonce, so undefined workspace contents cannot be mistaken for it).  The range that
 //    holds the BEGINNING of a row block owns it: when it reaches the end of its share -- by then the other contributors,
@@ -684,7 +681,7 @@ gemv_sk_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ 
         // The whole chunk is in registers: request the chunk DEPTH ahead into this slot while we compute.  No proxy fence:
         // the ld.shared above were issued (in order, by every lane -- __syncwarp) before the request, complete within tens
         // of cycles, and the TMA write lands after an L2 / DRAM round trip; a fence.proxy.async here (MEMBAR.ALL.CTA +
-        // FENCE.VIEW.ASYNC) measured ~10 % of all issue-stall samples.
+        // FENCE.VIEW.ASYNC) would stall every chunk.
         if (ti < t1) {
           __syncwarp();
           issue_chunk();
@@ -996,8 +993,8 @@ GemvParams make_params(const MatmulArgs& a) {
 
 // K splits per 16-row block (= warps per CTA): the largest count for which EVERY CTA of the grid is resident at once
 // (occupancy queried from the runtime for this kernel instantiation, cached).  When not even two warps per CTA fit in one wave
-// (N >= ~24k rows), the full split is used and the grid runs in several waves: measured 40.9 us vs 44.4 us for one resident
-// warp per row block on 28672 x 8192 (20 instead of 12 warps per SM; `BB_GEMV_KS` sweeps it).
+// (N >= ~24k rows), the full split is used and the grid runs in several waves rather than with one resident warp per row
+// block (`BB_GEMV_KS` sweeps it).
 template <typename KernelT>
 int pick_ks(KernelT kernel, int (&occ_cache)[MAX_KS + 1], int max_ks, int row_blocks, int steps, int stage_bytes) {
   const int sms = device_sm_count();

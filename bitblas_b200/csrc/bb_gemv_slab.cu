@@ -2,16 +2,14 @@
 //
 // Replaces the reference's generated SIMT GEMV (bitblas/ops/general_matmul/tilelang/dequantize/gemv_dequantize_simt.py:164-262)
 // and supersedes the round-1 register-queue kernel (bb_gemv.cu: 0.40 of the HBM roofline, bound by instruction issue and by
-// DRAM round trips sitting on the warps' scoreboards).  Design, top down (every choice below was measured on B200; the
-// intermediate versions and their ablations are in profiles/r2_slab_v*.txt):
+// DRAM round trips sitting on the warps' scoreboards).  Design, top down:
 //
 //   * WORK UNIT = [32 weight rows] x [1024 k] = 16 KB of packed weights out of the unchanged [N, K/2] storage, fetched by ONE TMA
-//     request: box {128 x u32 = 512 B, 32 rows}, no swizzle.  The TMA engine pays per request and per box row: a GEMM-style
-//     128B-swizzled box ({128 B, 16 rows, 8 slices}) streamed DRAM at 1.2-1.6 TB/s, sixteen 1 KB cp.async.bulk copies per unit
-//     at 2.1 TB/s, boxes with long rows at the linear-read rate (tools/slabbench.cu); bandwidth then depends only on the bytes
-//     in flight.  Units are ordered (row-block group, k, member) and cut into equal contiguous ranges over a persistent grid
+//     request: box {128 x u32 = 512 B, 32 rows}, no swizzle.  The TMA engine pays per request and per box row, so one box
+//     with long rows streams closer to the linear-read rate than a GEMM-style 128B-swizzled box or many small bulk copies
+//     (tools/slabbench.cu compares them); bandwidth then depends only on the bytes in flight.  Units are ordered (row-block group, k, member) and cut into equal contiguous ranges over a persistent grid
 //     (CTA-level stream-K): every SM streams the same number of bytes whatever N, K are; a 1024-row tensor-parallel shard
-//     still fills all 148 SMs.
+//     still fills all 132 SMs of an H100.
 //   * a CTA = NG consumer GROUPS of 4 warps + an issuer warp + NF finisher warps around an S-stage mbarrier ring.  Group g
 //     consumes the units whose row block is g (mod NG) -- whole row blocks per group, so a group reduces, exchanges stream-K
 //     partials and stores on its own, with a 128-thread named barrier; nothing ever synchronises the whole CTA.  The
@@ -27,8 +25,8 @@
 //   * the ISSUER requests, the moment a ring slot is free, everything the unit needs: the weight box, the activation slab
 //     (bulk copy) and the RAW group parameters (cp.async, 16 B per row); a FINISHER turns the slab into (SM, S) per step on the
 //     tensor cores and the raw parameters into fp32 (c1, c2) pairs, then completes the stage barrier.  The DRAM system runs
-//     saturated, so by Little's law EVERY request -- also a 1-byte parameter load -- takes (bytes in flight)/bandwidth ~ 3 us:
-//     anything fetched with plain loads "a few units ahead" stalls its warp on every unit (measured: 17.7 vs 13.2 us).
+//     saturated, so by Little's law EVERY request -- also a 1-byte parameter load -- takes (bytes in flight)/bandwidth, microseconds:
+//     anything fetched with plain loads "a few units ahead" stalls its warp on every unit.
 //   * stream-K fix-up: a range that starts inside a row block parks its group-reduced partial row sums in tagged 64-bit
 //     workspace slots {call nonce, fp32}; the range holding the block's first unit adds them in fixed order (bit-reproducible)
 //     and stores.  Ranges are handed out in reverse CTA order so an owner only waits for CTAs dispatched before it.
@@ -119,9 +117,8 @@ __device__ __forceinline__ void gs_mbar_wait(uint32_t bar, uint32_t parity) {
       "GS_DONE_%=:\n"
       "}\n" ::"r"(bar), "r"(parity), "r"(GS_SUSPEND_NS) : "memory");
 }
-// (measured and rejected: a nanosleep back-off between the helper warps' barrier probes.  The probe loops are 16 % of all issued
-//  instructions, but removing them made the kernel 1.7 % SLOWER -- the schedulers are not short of issue slots, the consumer warps
-//  are bound by their own dependent-instruction latency; profiles/r2_slab_v7_notes.txt)
+// (No nanosleep back-off between the helper warps' barrier probes: the schedulers are not short of issue slots, the consumer warps
+//  are bound by their own dependent-instruction latency.)
 __device__ __forceinline__ void gs_tma_2d(uint32_t dst, const void* map, int c0, int c1, uint32_t bar) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
                "l"(map), "r"(c0), "r"(c1), "r"(bar)
@@ -212,7 +209,7 @@ __device__ __forceinline__ int gs_range_begin(int ri, int T, int R) { return int
 
 // NG consumer groups per CTA, MINB CTAs per SM: (2, 2) or (4, 1).  SC = ring depth as a compile-time constant (0: p.stages at run
 // time, the tuning / test variant): with a constant depth every stage address is base + immediate -- the run-time variant spends
-// ~40 integer instructions per unit and warp re-deriving the region bases (profiles/r2_gemv_slab_ncu_full.txt, SASS page)
+// ~40 integer instructions per unit and warp re-deriving the region bases
 // NF = finisher warps (S % NF == 0; finisher f serves the units i = f (mod NF) of the range)
 // FMT: 0 = uint4 / int4 (LOP3 magic decode, magic and zero point removed through the activation sums), 1 = 16-entry table formats
 // (NF4 / fp4, compressed storage: PRMT table decode to exact A_dtype values, scale only -- the sums are not needed)
@@ -559,13 +556,10 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
           mma_pair(cc[pr], ha, hb, wi);
         }
       }
-      // (measured and rejected, same box, profiles/r2_slab_v8_ab.txt: issuing the MMAs word-major -- consecutive MMAs to the four
-      //  independent accumulators -- 18.2 vs 17.1 us; folding both corrections into one per-row number in the finisher, which
-      //  removes 13 of the consumer's 334 instructions per unit but makes the finisher's output depend on its own sums, 17.3 vs 17.1 us)
     }
     // the group parameters and activation sums are needed only now: the finisher works on THIS unit while we decode it, so its
-    // latency is off the critical path (with everything behind one barrier the consumers waited ~half the time although the
-    // feed alone ran at 0.84 of the roofline: profiles/r2_slab_v6_*.txt)
+    // latency is off the critical path (with everything behind one barrier the consumers would wait for the slowest part of the
+    // feed)
     gs_mbar_wait(Bb + 8u * (S + slot), fphase);
     if (active) {
       const uint32_t pst = Pb + uint32_t(slot) * GS_PBYTES + poff;

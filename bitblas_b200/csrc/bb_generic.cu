@@ -3,7 +3,7 @@
 // Follows the operator semantics of the reference's TE definition literally
 // (bitblas/ops/general_matmul/tirscript/matmul_dequantize_impl.py:391-478): decode one element, apply
 // zeros/scale in A_dtype arithmetic, accumulate (fp32 stand-in for tensor-core accumulation, or exact
-// int32), cast to out_dtype, add bias.  It is the fallback for shapes/formats the streaming and tcgen05
+// int32), cast to out_dtype, add bias.  It is the fallback for shapes/formats the streaming and wgmma
 // kernels do not cover (odd K, 1-bit, NF4/FP4/FP8 weights, group sizes < 128 ...) and the on-device
 // cross-check for them.  One warp per output column n, up to MT rows of A per warp.
 #include "bb_common.cuh"

@@ -1,4 +1,4 @@
-"""Build bitblas_b200/lib/libbitblas_b200.so with plain nvcc for sm_100a (in-tree, travels to the GPU box)."""
+"""Build bitblas_b200/lib/libbitblas_b200.so with plain nvcc for sm_90a (H100), in-tree."""
 import os
 import subprocess
 import sys
@@ -9,8 +9,8 @@ PKG = os.path.dirname(HERE)
 OUT_DIR = os.path.join(PKG, "lib")
 OBJ_DIR = os.path.join(HERE, "build")
 SOURCES = ["bb_api.cu", "bb_generic.cu", "bb_gemv.cu", "bb_gemv_slab.cu", "bb_gemm_ts.cu", "bb_prep.cu"]
-HEADERS = ["bb_common.cuh", os.path.join(PKG, "..", "include", "bitblas_b200.h")]
-FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC",
+HEADERS = ["bb_common.cuh", "bb_wgmma.inc", os.path.join(PKG, "..", "include", "bitblas_b200.h")]
+FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v" if os.environ.get("BB_PTXAS_V") else "-O3"]
 
 
@@ -51,7 +51,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         list(ex.map(run, jobs))
     out = lib_path()
     if jobs or force or _stale(out, objs):
-        run(["nvcc", "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", out, *objs])
+        run(["nvcc", "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", out, *objs])
     return out
 
 

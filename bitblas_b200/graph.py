@@ -1,6 +1,6 @@
 """CUDA-graph capture of a fixed sequence of operator calls (a decode step).
 
-The reference removes per-call host overhead with a tracing compiler around its generated kernels; on B200 the idiomatic tool is a
+The reference removes per-call host overhead with a tracing compiler around its generated kernels; on H100 the idiomatic tool is a
 CUDA graph: the operators of this package never allocate, synchronise or read host state inside ``forward`` once their workspace
 exists (include/bitblas_b200.h), the decode kernel's launch parameters do not change between replays (its stream-K nonce lives in
 slots that every replay resets), and the programmatic-dependent-launch edges between consecutive matmuls survive capture.  A

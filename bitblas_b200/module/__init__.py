@@ -1,8 +1,8 @@
-"""``bitblas.Linear`` (bitblas/module/__init__.py:77-370) on the B200 library.
+"""``bitblas.Linear`` (bitblas/module/__init__.py:77-370) on the H100 library.
 
 Same constructor, buffers (``qweight`` / ``scales`` / ``zeros`` / ``bias`` or ``weight``; shapes and dtypes as in
 module/__init__.py:164-205 so reference checkpoints load), ``forward``, ``load_and_transform_weight`` and the GPTQ
-repack entry points.  Differences that matter on B200: the output is ``torch.empty`` (the reference memsets with
+repack entry points.  Differences that matter here: the output is ``torch.empty`` (the reference memsets with
 ``torch.zeros`` on every call, :277), the pointer list is built once, and the GPTQ repack runs as device kernels
 (bb_repack_gptq_*_device) instead of Python column loops (:24-74).
 """

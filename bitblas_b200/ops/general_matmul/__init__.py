@@ -1,5 +1,5 @@
 """``MatmulConfig`` / ``Matmul``: the operator API of bitblas/ops/general_matmul/__init__.py, re-hosted on the
-prebuilt sm_100a library.
+prebuilt sm_90a library.
 
 Same fields, defaults and legalisation as the reference ``MatmulConfig`` (general_matmul/__init__.py:58-237), same
 ``Matmul`` surface (``forward/__call__``, ``transform_weight``, ``transform_input``, ``retrieve_weight_shape``,
@@ -98,8 +98,8 @@ class MatmulConfig(OperatorConfig):
         if isinstance(self.optimize_stratety, int) and not isinstance(self.optimize_stratety, OptimizeStrategy):
             self._set("optimize_stratety", OptimizeStrategy(self.optimize_stratety))
         # Weight propagation (general_matmul/__init__.py:113-157).  The reference re-tiles W offline into mma.sync /
-        # ldmatrix fragment order; tcgen05 operands are laid out in TMEM by the kernels themselves, so that particular
-        # permutation has no meaning here.  What an offline layout still buys on B200 is DRAM / TMA locality: a requested
+        # ldmatrix fragment order; wgmma operands are laid out in registers by the kernels themselves, so that particular
+        # permutation has no meaning here.  What an offline layout still buys on H100 is DRAM / TMA locality: a requested
         # propagate_b selects the slab tiling BB_TILE_SLAB (include/bitblas_b200.h: [N/32][row_bytes/512][32][512 B]; one
         # work unit of the decode GEMV = one contiguous 16 KB block).  Default (None / False): the reference's row-major
         # storage, byte-compatible with its checkpoints.  propagate_a never applies (activations are consumed as they are).
@@ -374,7 +374,7 @@ class Matmul(Operator):
         return weight
 
     def transform_input(self, input_tensor):
-        return input_tensor  # no ladder propagation on B200
+        return input_tensor  # no ladder propagation on H100
 
     # ---- forward ------------------------------------------------------------------------------------
     def _check_tensor(self, t: torch.Tensor, name: str, dtype: torch.dtype, numel: Optional[int] = None):
@@ -559,7 +559,7 @@ class Matmul(Operator):
 
     def get_source(self, target=None, kenrel_only=False) -> str:
         ms = self.M if isinstance(self.M, tuple) else (self.M,)
-        lines = [f"// bitblas_b200 prebuilt sm_100a kernels ({_lib.LIB_PATH}); sources: bitblas_b200/csrc/*.cu"]
+        lines = [f"// bitblas_b200 prebuilt sm_90a kernels ({_lib.LIB_PATH}); sources: bitblas_b200/csrc/*.cu"]
         if self._desc is not None:
             lines += [f"// m={m}: {self.kernel_for(m)}" for m in ms]
         return "\n".join(lines)

@@ -2,7 +2,7 @@
 
 Keeps the attributes callers touch (``lib``, ``profile_latency``, ``hardware_aware_finetune``, ``get_source``,
 ``cleanup``; reference: bitblas/ops/operator.py:133,347-382,442-463) -- there is nothing to compile or tune at
-construction time, every configuration is served by the prebuilt sm_100a library.
+construction time, every configuration is served by the prebuilt sm_90a library.
 """
 from __future__ import annotations
 
@@ -38,7 +38,7 @@ class Operator:
         self.profile_tensors = None
 
     def hardware_aware_finetune(self, topk: int = 20, target=None, parallel_build: bool = True):
-        """No-op: kernels are hand-written for sm_100a; selection is a run-time dispatch on m."""
+        """No-op: kernels are hand-written for sm_90a; selection is a run-time dispatch on m."""
         return None
 
     def get_source(self, target=None, kenrel_only: bool = False) -> str:

@@ -8,7 +8,7 @@ in tensor-parallel inference); one exchange step -- an all-gather of the [m, N/G
 
 One process per GPU, ``torch.distributed`` (NCCL over NVLink5/NVSwitch; gloo on CPU for the host-logic tests).
 For large m the all-gather is pipelined against the matmul in row chunks on a side stream so the transfer of
-chunk i overlaps the tcgen05 kernel of chunk i+1.
+chunk i overlaps the wgmma kernel of chunk i+1.
 """
 from __future__ import annotations
 
@@ -27,7 +27,7 @@ class PeerBarrier:
     """Device-side barrier across the ranks of a group, one small kernel per call (bb_peer_barrier): ordered after the peer stores
     of the preceding bb_matmul_scatter launches on the same stream, CUDA-graph capturable, and -- being a programmatic dependent
     launch -- overlapped with the next matmul kernel's weight prefetch.  Replaces the symmetric-memory library barrier on the
-    fused column-parallel path (measured at 2 GPUs: ~14 us per step for the library barrier, profiles/r2_multi_2gpu.txt)."""
+    fused column-parallel path."""
 
     def __init__(self, device, group=None):
         import torch.distributed._symmetric_memory as symm_mem

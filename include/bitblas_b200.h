@@ -1,5 +1,5 @@
 /*
- * bitblas_b200.h -- C ABI of the B200-native low-bit-weight matmul library.
+ * bitblas_b200.h -- C ABI of the H100-native (sm_90a) low-bit-weight matmul library.
  *
  * This is the drop-in boundary for the ONE hot path of microsoft/BitBLAS: the dequantize-matmul behind
  * bitblas.Matmul / bitblas.Linear.  In the reference every operator instance owns a generated .so that
@@ -64,10 +64,10 @@ typedef enum bb_wlayout {
 
 /* Offline tiling of the packed weight matrix (MatmulConfig.propagate_b).  The reference's weight propagation re-tiles W offline
  * so that its mma.sync kernels can use ldmatrix-friendly, conflict-free tiles (bitblas/ops/ladder_permutate/
- * ladder_permutate_impl.py:12-116, bitblas/gpu/matmul_analysis.py:691-801, general_matmul/__init__.py:113-157).  On B200 the
- * tensor-core operand layout is produced in TMEM by the kernels themselves; what an offline layout can still buy is DRAM/TMA
+ * ladder_permutate_impl.py:12-116, bitblas/gpu/matmul_analysis.py:691-801, general_matmul/__init__.py:113-157).  Here the
+ * tensor-core operand layout is produced in registers by the kernels themselves; what an offline layout can still buy is DRAM/TMA
  * locality.  BB_TILE_SLAB stores the packed rows as [N/32][row_bytes/512][32 rows][512 B] (row_bytes = K*bits/8): one 16 KB
- * work unit of the decode GEMV is ONE contiguous block, and the 128-row x k-block tile of the tcgen05 kernel is four 4-D TMA
+ * work unit of the decode GEMV is ONE contiguous block, and the 128-row x k-block tile of the wgmma kernel is four 4-D TMA
  * box rows of it.  Same bytes, same size, same interleave inside each 32-bit word; only the order of 512-byte row segments
  * changes.  Needs N % 32 == 0 and row_bytes % 512 == 0. */
 typedef enum bb_wtile {
@@ -104,10 +104,10 @@ typedef enum bb_kernel_id {
   BB_KERNEL_GENERIC = 1,   /* SIMT, every config (spec-order arithmetic)                     */
   BB_KERNEL_GEMV_MMA = 2,  /* m <= 32, fp16/bf16 A, 4/2-bit W: warp-level mma.sync streaming  */
   BB_KERNEL_GEMV_I8 = 3,   /* m <= 32, int8 A, 4/2-bit W: IMMA streaming, int32 exact         */
-  BB_KERNEL_GEMM_TS = 4,   /* tcgen05 (W dequantised into TMEM as the MMA A operand) + TMA    */
-  BB_KERNEL_GEMM_TS_I8 = 5,/* tcgen05 kind::i8 variant                                        */
+  BB_KERNEL_GEMM_TS = 4,   /* wgmma (W dequantised into registers as the MMA A operand) + TMA */
+  BB_KERNEL_GEMM_TS_I8 = 5,/* wgmma int8 variant                                             */
   BB_KERNEL_GEMV_STREAMK = 6,/* m <= 2, 4-bit W: persistent stream-K + TMA rings; opt-in through
-                              * bb_set_kernel_override only (measured no faster than GEMV_MMA, DESIGN.md) */
+                              * bb_set_kernel_override only */
   BB_KERNEL_GEMV_SLAB = 7    /* m == 1, 4-bit W, fp16/bf16 A: per-CTA TMA slabs + CTA-level stream-K; the default
                               * decode kernel (needs the zero-initialised workspace of bb_workspace_bytes) */
 } bb_kernel_id;
@@ -149,7 +149,7 @@ int bb_peer_barrier(void* const* peer_flags, int n_peers, int rank, void* stream
  * The buffer must be ZERO-INITIALISED once by the caller before its first use (cudaMemset / torch.zeros): the stream-K
  * kernels exchange partial sums through tagged slots and leave every slot zero-tagged again when they finish, so the same
  * buffer can then be reused by later calls ON THE SAME STREAM without clearing (calls that may run concurrently need their
- * own buffers).  The split-K partials of the tcgen05 kernel carry no such requirement. */
+ * own buffers).  The split-K partials of the wgmma kernel carry no such requirement. */
 size_t bb_workspace_bytes(const bb_matmul_desc* desc, int m);
 
 /* which kernel family bb_matmul would run for (desc, m) -- bb_kernel_id; <0 on invalid desc. */

@@ -1,8 +1,8 @@
 // oracle/ref_shim.cu -- TEST INFRASTRUCTURE ONLY.
 //
 // Thin extern "C" wrappers around the REFERENCE's own C++/CUDA decode test header, compiled from the
-// source where it lies (/root/reference/testing/cpp/lop3_type_conversion/fast_decoding.hpp) by
-// oracle/build_ref.py into oracle/_ref/libbitblas_ref.so (git-ignored; travels to the GPU box).
+// source where it lies ($BITBLAS_REFERENCE_DIR/testing/cpp/lop3_type_conversion/fast_decoding.hpp) by
+// oracle/build_ref.py into oracle/_ref/libbitblas_ref.so (git-ignored).
 // No reference source is copied here: this file only #includes the header and calls into it.
 //
 //   host  : ref_general_compress / ref_general_interleave_fp16 / ref_general_interleave_int8

@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA GPU (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA GPU (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

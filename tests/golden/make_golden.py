@@ -1,6 +1,6 @@
-"""Generate golden vectors by RUNNING the reference's own numpy functions (run in the authoring container).
+"""Generate golden vectors by RUNNING the reference's own numpy functions.
 
-Loads /root/reference/bitblas/quantization/utils.py standalone via importlib (it only needs numpy+torch),
+Loads bitblas/quantization/utils.py of the microsoft/BitBLAS checkout at $BITBLAS_REFERENCE_DIR standalone via importlib (it only needs numpy+torch),
 runs general_compress / interleave_weight on seeded inputs and stores inputs+outputs in
 tests/golden/quant_golden.npz.  Cases the reference itself cannot run are recorded as such:
   * interleave 2-bit/float16 raises OverflowError under NumPy 2 (np.int32(0xFF0000FF), utils.py:97)
@@ -17,7 +17,8 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-spec = importlib.util.spec_from_file_location("ref_quant_utils", "/root/reference/bitblas/quantization/utils.py")
+spec = importlib.util.spec_from_file_location(
+    "ref_quant_utils", os.path.join(os.environ["BITBLAS_REFERENCE_DIR"], "bitblas", "quantization", "utils.py"))
 ref = importlib.util.module_from_spec(spec)
 spec.loader.exec_module(ref)
 

@@ -78,12 +78,12 @@ def test_matmul_surface_and_dispatch():
                  "group_size", "fast_decoding", "with_bias", "propagate_a", "propagate_b", "layout", "zeros_mode"):
         assert getattr(op, name) == getattr(cfg, name)
     assert op.hardware_aware_finetune(topk=20) is None
-    assert [op.kernel_for(m) for m in (1, 8, 9, 32, 128, 4096)] == ["gemv_slab", "gemv_mma"] + ["gemm_ts_tcgen05"] * 4
-    assert "gemm_ts_tcgen05" in op.get_source()
+    assert [op.kernel_for(m) for m in (1, 8, 9, 32, 128, 4096)] == ["gemv_slab", "gemv_mma"] + ["gemm_ts_wgmma"] * 4
+    assert "gemm_ts_wgmma" in op.get_source()
     # W2A8 (integration/BitNet/utils_quant.py:55-69)
     op8 = bitblas.Matmul(bitblas.MatmulConfig(M=[1, 128], N=12288, K=12288, A_dtype="int8", W_dtype="int2", accum_dtype="int32",
                                               out_dtype="float32"), enable_tuning=False)
-    assert [op8.kernel_for(m) for m in (1, 128)] == ["gemv_i8", "gemm_ts_tcgen05_i8"]
+    assert [op8.kernel_for(m) for m in (1, 128)] == ["gemv_i8", "gemm_ts_wgmma_i8"]
     # formats without a fast kernel fall to the generic CUDA kernel, never to the CPU
     opn = bitblas.Matmul(bitblas.MatmulConfig(M=1, N=64, K=256, W_dtype="nf4", with_scaling=True, group_size=64), enable_tuning=False)
     assert opn.kernel_for(1) == "generic_simt" and opn.lut is not None and opn.lut.numel() == 16
@@ -150,7 +150,7 @@ def test_bitblas_alias_package():
 
 
 def test_propagate_b_selects_slab_tiling():
-    """MatmulConfig(propagate_b=True): the B200 meaning of weight propagation is the slab tiling (include/bitblas_b200.h,
+    """MatmulConfig(propagate_b=True): the H100 meaning of weight propagation is the slab tiling (include/bitblas_b200.h,
     enum bb_wtile); shapes / formats it does not cover legalise back to the row-major storage like the reference's
     __initialize_propagate does for its own unsupported cases (general_matmul/__init__.py:113-157)."""
     import numpy as np
@@ -173,5 +173,5 @@ def test_propagate_b_selects_slab_tiling():
     plain, tiled = op0.transform_weight(fields), op.transform_weight(fields)
     assert np.array_equal(tiled.numpy(), O.slab_tile(plain.numpy()))
     assert torch.equal(op.tile_weight(tiled, inverse=True), plain)
-    # dispatch: the decode kernel and the tcgen05 kernel take the tiled storage, the register-streaming kernels do not
-    assert op.kernel_for(1) == "gemv_slab" and op.kernel_for(4) == "gemm_ts_tcgen05" and op.kernel_for(512) == "gemm_ts_tcgen05"
+    # dispatch: the decode kernel and the wgmma kernel take the tiled storage, the register-streaming kernels do not
+    assert op.kernel_for(1) == "gemv_slab" and op.kernel_for(4) == "gemm_ts_wgmma" and op.kernel_for(512) == "gemm_ts_wgmma"

@@ -1,4 +1,4 @@
-"""Multi-GPU (NCCL) column-parallel path on real devices: needs >= 2 GPUs (gpurun --gpus 2); skipped otherwise."""
+"""Multi-GPU (NCCL) column-parallel path on real devices: needs >= 2 GPUs; skipped otherwise."""
 import os
 import sys
 
@@ -95,7 +95,7 @@ def test_one_process_two_devices():
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     import helpers as H
     torch.cuda.set_device(0)
-    for M in (1, 4, 300):     # decode GEMV, streaming GEMV, tcgen05 GEMM (> 48 KB of dynamic shared memory on both devices)
+    for M in (1, 4, 300):     # decode GEMV, streaming GEMV, wgmma GEMM (> 48 KB of dynamic shared memory on both devices)
         case = H.make_case(M, 256, 2048, W_dtype="uint4", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized", seed=M)
         ref = H.oracle_output(case)
         op = H.product_operator(case)

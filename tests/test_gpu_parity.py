@@ -9,7 +9,7 @@ pytestmark = pytest.mark.gpu
 
 
 def _run(case, expect_kernel=None, force=None):
-    """force: kernel family id to pin with bb_set_kernel_override (the dispatcher prefers the tcgen05 kernel above m = 8,
+    """force: kernel family id to pin with bb_set_kernel_override (the dispatcher prefers the wgmma kernel above m = 8,
     the streaming kernels still cover m <= 32 and are tested there through the override)."""
     from bitblas_b200 import _lib
     op = H.product_operator(case)
@@ -202,8 +202,7 @@ GEMM_CASES = [
     dict(M=9, N=256, K=1024, W_dtype="uint4", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized"),
     dict(M=16, N=128, K=2048, W_dtype="uint4", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="original", with_bias=True),
     dict(M=32, N=256, K=1024, W_dtype="uint2", group_size=128, with_scaling=True),
-    # more CTAs than SMs at BM = 128: two CTAs per SM, pipeline capped to 4 stages (= the dequant group stride: the TMEM slot of
-    # a k-block must then be published BEFORE waiting for the next TMA stage, or the ring deadlocks)
+    # more CTAs than SMs at BM = 128: several waves of tiles over the SMs
     dict(M=100, N=19200, K=512, W_dtype="uint4", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized"),
     # split-K (few output tiles, long K): fp32 partials in the workspace + reduce kernel
     dict(M=64, N=128, K=4096, W_dtype="uint4", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized", with_bias=True),
@@ -215,9 +214,7 @@ GEMM_CASES = [
     dict(M=96, N=256, K=1024, W_dtype="int4", fast_decoding=False, group_size=-1, with_scaling=True),
     dict(M=128, N=256, K=1024, W_dtype="uint4", A_dtype="bfloat16", out_dtype="bfloat16", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized"),
     dict(M=128, N=128, K=512, W_dtype="uint2", A_dtype="bfloat16", out_dtype="bfloat16", group_size=128, with_scaling=True),
-    # group length (3 k-blocks) that the dequant groups' stride (4 for BM <= 128, 2 for BM = 256) neither divides nor is a multiple
-    # of: a warp's consecutive k-blocks then skip one or two groups, and the parameter prefetch must name the right one
-    # (round-1 advisor finding: kb = 12 consumed group 3's scale)
+    # group length of 3 k-blocks, not a power of two: the one-group-ahead parameter prefetch must name the right group
     dict(M=16, N=128, K=1536, W_dtype="uint4", group_size=192, with_scaling=True, with_zeros=True, zeros_mode="quantized"),
     dict(M=100, N=256, K=1536, W_dtype="uint4", group_size=192, with_scaling=True, with_zeros=True, zeros_mode="original"),
     dict(M=300, N=256, K=3072, W_dtype="uint4", group_size=192, with_scaling=True, with_zeros=True, zeros_mode="rescale"),
@@ -226,10 +223,11 @@ GEMM_CASES = [
 
 
 @pytest.mark.parametrize("kw", GEMM_CASES, ids=lambda k: "-".join(f"{a}{b}" for a, b in k.items()))
+# (the name is kept from the Blackwell build so that test ids stay stable; the kernel under test is gemm_ts_wgmma)
 def test_gemm_tcgen05_parity(kw):
     kw = dict(kw)
     case = H.make_case(kw.pop("M"), kw.pop("N"), kw.pop("K"), **kw)
-    op, got, ref = _run(case, "gemm_ts_tcgen05")
+    op, got, ref = _run(case, "gemm_ts_wgmma")
     H.assert_fp_close(got, ref, "gemm_ts")
 
 
@@ -264,7 +262,7 @@ def test_int8_activation_bit_exact(kw):
     if M <= 32 and il8:
         op, got, ref = _run(case, "gemv_i8", force=_lib.BB_KERNEL_GEMV_I8)
     else:
-        op, got, ref = _run(case, "gemm_ts_tcgen05_i8")
+        op, got, ref = _run(case, "gemm_ts_wgmma_i8")
     assert torch.equal(got, ref)
 
 
@@ -294,7 +292,7 @@ def test_generic_kernel_parity(kw):
     H.assert_fp_close(got, ref, "generic")
 
 
-# 16-entry table formats (NF4 / "fp4") on the fast kernels: PRMT table decode in the decode GEMV (m = 1) and in the tcgen05 dequant
+# 16-entry table formats (NF4 / "fp4") on the fast kernels: PRMT table decode in the decode GEMV (m = 1) and in the wgmma dequant
 # warps (m > 1); reference semantics matmul_dequantize_impl.py:424-430 (nf: LUT[w]) and quantization.py:141-156 (fp4), support
 # matrix README.md:61-88.  Same oracle, same tolerance as every other float case.
 TABLE_CASES = [
@@ -317,7 +315,7 @@ def test_table_formats_fast_kernels(kw):
     M = kw["M"]
     case = H.make_case(kw.pop("M"), kw.pop("N"), kw.pop("K"), **kw)
     bf = kw.get("A_dtype") == "bfloat16"
-    op, got, ref = _run(case, "gemv_slab" if M == 1 else "gemm_ts_tcgen05")
+    op, got, ref = _run(case, "gemv_slab" if M == 1 else "gemm_ts_wgmma")
     H.assert_fp_close(got, ref, f"table format {kw['W_dtype']} M={M}", max_mismatched_ratio=2e-3 if bf else 0.0)
     # and the generic kernel on the same inputs (the spec-order implementation these formats used before)
     from bitblas_b200 import _lib
@@ -329,7 +327,7 @@ def test_table_formats_fast_kernels(kw):
 @pytest.mark.parametrize("M,N,K,adt", [(1, 256, 1024, "float16"), (16, 256, 2048, "float16"), (300, 384, 1024, "float16"),
                                        (64, 128, 8192, "float16"), (128, 256, 1024, "bfloat16")])
 def test_fp8_weights_tcgen05(wd, M, N, K, adt):
-    """8-bit float weights x 16-bit activations on the tcgen05 kernel (README.md:61-88 support matrix; decode formulas
+    """8-bit float weights x 16-bit activations on the wgmma kernel (README.md:61-88 support matrix; decode formulas
     quantization.py:169-182).  e4m3 codes are kept to normal numbers like in the generic-kernel test: the reference's bit trick
     maps the zero / subnormal codes to large garbage values, and sums of those overflow fp16."""
     bf = adt == "bfloat16"
@@ -343,7 +341,7 @@ def test_fp8_weights_tcgen05(wd, M, N, K, adt):
         f = torch.where((f & 0x7C) == 0x7C, f & 0xBF, f)       # no inf / nan codes
         f = torch.where((f & 0x7C) >= 0x48, f & 0xB7 | 0x20, f)  # moderate magnitudes
     case["fields"] = f
-    op, got, ref = _run(case, "gemm_ts_tcgen05")
+    op, got, ref = _run(case, "gemm_ts_wgmma")
     H.assert_fp_close(got, ref, f"{wd} M={M}", max_mismatched_ratio=2e-3 if bf else 0.0)
     from bitblas_b200 import _lib
     _, got2, _ = _run(case, "generic_simt", force=_lib.BB_KERNEL_GENERIC)
@@ -513,7 +511,7 @@ def test_gemm_ts_baseline_shapes(N, K):
     Wd = O.dequantize_weight(fields.to(torch.int32), W_dtype="uint4", group_size=128, with_scaling=True, with_zeros=True,
                              zeros_mode="quantized", scale=scale, zeros=qz).float()
     for M in (16, 128, 4096):
-        assert op.kernel_for(M) == "gemm_ts_tcgen05"
+        assert op.kernel_for(M) == "gemm_ts_wgmma"
         A = (torch.rand((M, K), generator=g) - 0.5).half()
         got = op.forward(A.cuda(), W, scale=sc, zeros=zz).cpu()
         rows = torch.arange(M) if M <= 128 else torch.randperm(M, generator=g)[:64].sort().values

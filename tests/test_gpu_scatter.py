@@ -1,6 +1,6 @@
 """Column-parallel scatter epilogue (bb_matmul_scatter) on ONE device: two local [m, ldc] buffers stand in for the peers'
 symmetric-memory outputs.  The result in every destination must equal the plain bb_matmul output bit for bit (same kernel, same
-arithmetic; only the store path differs -- for the tcgen05 GEMM that is the staged 16-byte-store epilogue), in the right column
+arithmetic; only the store path differs), in the right column
 window, and nothing outside the window may be touched.  The real multi-GPU run is tests/test_gpu_multi.py."""
 import pytest
 import torch
@@ -19,11 +19,11 @@ CASES = [
     # M, N, K, A_dtype, out_dtype, bias, group
     (1, 256, 1024, "float16", "float16", True, 128),      # gemv_slab
     (4, 256, 1024, "float16", "float16", False, 128),     # gemv_mma
-    (16, 128, 8192, "float16", "float16", True, 128),     # tcgen05 BM=32, split-K + reduce kernel
+    (16, 128, 8192, "float16", "float16", True, 128),     # wgmma BM=32, split-K + reduce kernel
     (40, 256, 1024, "float16", "float16", True, 128),     # BM=64, ragged rows
     (100, 384, 2048, "float16", "float16", False, 128),   # BM=128, ragged rows
-    (300, 256, 1024, "float16", "float16", True, 128),    # BM=256: second m-tile has 44 valid rows
-    (512, 512, 2048, "bfloat16", "bfloat16", True, 128),  # bf16 staged path
+    (300, 256, 1024, "float16", "float16", True, 128),    # BM=128: third m-tile has 44 valid rows
+    (512, 512, 2048, "bfloat16", "bfloat16", True, 128),  # bf16 output
     (257, 256, 1024, "float16", "float16", False, -1),    # one valid row in the last tile
 ]
 

@@ -1,5 +1,5 @@
 """MatmulConfig(propagate_b=True): BB_TILE_SLAB weight storage (include/bitblas_b200.h) through every kernel that consumes it --
-the decode GEMV (one contiguous 16 KB bulk copy per unit), the tcgen05 GEMM (4-D TMA box over the tiled tensor) and the generic
+the decode GEMV (one contiguous 16 KB bulk copy per unit), the wgmma GEMM (4-D TMA box over the tiled tensor) and the generic
 kernel (tiled addressing) -- against the CPU oracle, and bit for bit against the same operator on the row-major storage.
 Mirrors the role of the reference's propagate_b cases in testing/python/operators/test_general_matmul_ops.py (weight propagation
 must not change the result)."""
@@ -40,13 +40,13 @@ TILE_CASES = [
     (1, 4096, 4096, "float16", "uint4", "original", False, 128),     # gemv_slab, stream-K over many CTAs
     (1, 1024, 8192, "bfloat16", "uint4", "rescale", False, 128),
     (1, 256, 2048, "float16", "int4", None, False, -1),
-    (4, 256, 2048, "float16", "uint4", "quantized", False, 128),     # small m on the tiled storage: tcgen05 BM=32
+    (4, 256, 2048, "float16", "uint4", "quantized", False, 128),     # small m on the tiled storage: wgmma BM=32
     (16, 128, 8192, "float16", "uint4", "quantized", True, 128),     # split-K
     (100, 384, 2048, "float16", "uint4", "original", False, 128),
-    (300, 256, 4096, "float16", "uint4", "quantized", True, 128),    # BM=256
+    (300, 256, 4096, "float16", "uint4", "quantized", True, 128),    # BM=128, three m-tiles
     (64, 256, 4096, "float16", "uint2", "quantized", False, 128),    # 2-bit: 16-byte box rows
     (1, 256, 4096, "float16", "uint2", "original", False, 128),
-    (1, 256, 4096, "int8", "int2", None, False, -1),                 # W2A8 on the tiled storage (tcgen05 kind::i8)
+    (1, 256, 4096, "int8", "int2", None, False, -1),                 # W2A8 on the tiled storage (wgmma int8)
     (128, 256, 4096, "int8", "int2", None, False, -1),
 ]
 

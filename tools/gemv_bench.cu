@@ -1,6 +1,6 @@
 // tools/gemv_bench.cu -- m = 1 W4A16 GEMV through the C ABI (bb_matmul): full-output check against a double-precision CPU
 // dequantise+dot, then back-to-back timing over rotating weight copies (cold L2), for a list of shapes and tuning knobs.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tools/gemv_bench tools/gemv_bench.cu \
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/gemv_bench tools/gemv_bench.cu \
 //        -Lbitblas_b200/lib -lbitblas_b200 -Xlinker -rpath -Xlinker '$ORIGIN/../bitblas_b200/lib'
 //   tools/gemv_bench [--kernel ID] [--iters N] [--cfg STAGES,GROUPS[,FINISHERS]]... [--tile] [--nocheck] NxK [NxK ...]
 #include <cuda_fp16.h>
@@ -46,7 +46,7 @@ int main(int argc, char** argv) {
   for (auto [N, K] : shapes) {
     const int G = K / g;
     const size_t wbytes = size_t(N) * K / 2;
-    const int copies = std::max(2, int((400ull << 20) / wbytes) + 1);   // > 126 MB of L2 between reuses
+    const int copies = std::max(2, int((400ull << 20) / wbytes) + 1);   // > 50 MB of L2 between reuses
     bb_matmul_desc d; memset(&d, 0, sizeof(d));
     d.N = N; d.K = K; d.a_dtype = BB_F16; d.w_fmt = BB_W_UINT; d.w_bits = 4; d.accum_dtype = BB_F32; d.out_dtype = BB_F16;
     d.group_size = g; d.with_scaling = 1; d.with_zeros = 1; d.zeros_mode = BB_ZEROS_QUANTIZED; d.with_bias = 0;

@@ -1,4 +1,4 @@
-// tools/membench.cu -- load-pattern microbenchmark used to size the GEMV kernel's weight stream on B200.
+// tools/membench.cu -- load-pattern microbenchmark used to size the GEMV kernel's weight stream.
 // Every variant reads the same N x (K/2)-byte packed-weight matrix exactly once and XOR-reduces it.
 //   linear   : each warp reads 512 contiguous bytes per instruction (grid-stride)                       [upper bound]
 //   rows16   : GEMV pattern: a warp owns 16 rows x a K range, lane (r,q) reads 16 B at row r/r+8, 64 B per row per
@@ -199,11 +199,12 @@ int main(int argc, char** argv) {
   std::vector<uint8_t*> bufs(5);
   for (auto& p : bufs) { CK(cudaMalloc(&p, bytes)); CK(cudaMemset(p, 1, bytes)); }
   unsigned* out; CK(cudaMalloc(&out, 4));
+  int sms = 0; CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
   auto rep = [&](const char* name, float ms) { printf("%-28s %8.2f us  %7.1f GB/s\n", name, ms * 1e3, bytes / (ms * 1e-3) / 1e9); };
   printf("N=%d K=%d bytes=%.1f MB\n", N, K, bytes / 1e6);
   for (int bpsm : {4, 8, 16}) {
     char nm[64]; snprintf(nm, 64, "linear %d x256thr/SM", bpsm);
-    rep(nm, time_it([&](uint8_t* w) { k_linear<<<148 * bpsm, 256>>>((const uint4*)w, bytes / 16, out); }, 10, bufs));
+    rep(nm, time_it([&](uint8_t* w) { k_linear<<<sms * bpsm, 256>>>((const uint4*)w, bytes / 16, out); }, 10, bufs));
   }
   for (int ks : {3}) {
     if ((row_bytes / 64) % ks) continue;

@@ -4,7 +4,7 @@
 //   box   : every warp streams its own 16-row block with [16 rows x 128 B] boxes (2 KB), DEPTH boxes in flight   (= gemv_sk_kernel)
 //   slab  : every CTA streams 16-row blocks with [16 rows x SLAB B] boxes (uint32 tensor map, SLAB = 512 / 1024), DEPTH slabs in
 //           flight, the 8 warps of the CTA each "consume" a 128 B K-slice of the slab
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o tools/slabbench tools/slabbench.cu -lcuda
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/slabbench tools/slabbench.cu -lcuda
 // Run:   tools/slabbench [N] [K] [delay_cycles]
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -126,7 +126,7 @@ int main(int argc, char** argv) {
   std::vector<uint8_t*> bufs(5);
   for (auto& p : bufs) { CK(cudaMalloc(&p, bytes)); CK(cudaMemset(p, 1, bytes)); }
   unsigned* out; CK(cudaMalloc(&out, 4));
-  int sms = 148; CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
+  int sms = 0; CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
   cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
   auto time_it = [&](auto launch) {
     for (int i = 0; i < 3; ++i) launch(bufs[i % 5]);
