@@ -21,7 +21,7 @@ BB_TILE_ROW_MAJOR, BB_TILE_SLAB = 0, 1
 BB_TILE_ROWS, BB_TILE_ROW_BYTES = 32, 512
 BB_PEER_FLAG_BYTES = 128
 (BB_KERNEL_AUTO, BB_KERNEL_GENERIC, BB_KERNEL_GEMV_MMA, BB_KERNEL_GEMV_I8, BB_KERNEL_GEMM_TS,
- BB_KERNEL_GEMM_TS_I8, BB_KERNEL_GEMV_STREAMK, BB_KERNEL_GEMV_SLAB) = range(8)
+ BB_KERNEL_GEMM_TS_I8, BB_KERNEL_GEMV_SLAB) = 0, 1, 2, 3, 4, 5, 7
 
 DTYPE_IDS = {"float16": BB_F16, "bfloat16": BB_BF16, "float32": BB_F32, "int8": BB_I8, "int32": BB_I32}
 WFMT_IDS = {"uint": BB_W_UINT, "int": BB_W_INT, "nf": BB_W_NF, "fp": BB_W_FP4, "fp_e4m3": BB_W_FP8_E4M3,

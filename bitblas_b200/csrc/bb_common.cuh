@@ -1,5 +1,6 @@
 // bb_common.cuh -- shared host/device helpers for the sm_90a kernels.
 #pragma once
+#include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -61,15 +62,20 @@ struct MatmulArgs {
 constexpr int BB_MAX_DEVICES = 64;
 int current_device();     // ordinal of the calling thread's current CUDA device, clamped to [0, BB_MAX_DEVICES)
 int device_sm_count();    // SM count of the current device (cached per device)
+// whether the streaming kernels launch with programmatic dependent launch (default on; BB_PDL=0 restores plain stream order)
+bool pdl_enabled();
+
+// the driver's cuTensorMapEncodeTiled, looked up once through the runtime (no libcuda link); null when unavailable
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeTiledFn tensor_map_encoder();
 
 // kernel family entry points (each returns 0 / error code; *_supported says whether the family covers it)
 bool generic_supported(const bb_matmul_desc& d);
 int launch_generic(const MatmulArgs& a);
 bool gemv_mma_supported(const bb_matmul_desc& d, int m);
 int launch_gemv_mma(const MatmulArgs& a);
-bool gemv_streamk_supported(const bb_matmul_desc& d, int m);
-int launch_gemv_streamk(const MatmulArgs& a);
-size_t gemv_streamk_workspace_bytes();  // partial slots + flags
 bool gemv_slab_supported(const bb_matmul_desc& d, int m);
 int launch_gemv_slab(const MatmulArgs& a);
 size_t gemv_slab_workspace_bytes();     // tagged partial slots (must be zero-initialised once by the caller)
@@ -78,7 +84,6 @@ int launch_gemv_i8(const MatmulArgs& a);
 bool gemm_ts_supported(const bb_matmul_desc& d, int m);
 int launch_gemm_ts(const MatmulArgs& a);
 size_t gemm_ts_workspace_bytes(const bb_matmul_desc& d, int m);
-int gemm_ts_init(int device);
 
 // bit position of logical element `o` (0 .. 32/bits-1) inside its 32-bit storage word, for each weight
 // layout (restates bitblas/quantization/utils.py:73-110 + testing/cpp/lop3_type_conversion/fast_decoding.hpp:30-95,607-668)

@@ -18,10 +18,7 @@
 //
 // Shared-memory traffic per k-block is therefore A-tile (TMA write + MMA read) + 4 KB packed W, instead of also writing and
 // re-reading a 16-32 KB dequantised W tile (DESIGN.md §3.1).
-#include <cuda.h>
-
 #include <algorithm>
-#include <mutex>
 
 #include "bb_common.cuh"
 
@@ -621,26 +618,9 @@ int choose_splits(int tiles, int num_kb, int sms) {
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_encode = nullptr;
-std::once_flag g_encode_once;
-
-EncodeTiledFn get_encode() {
-  std::call_once(g_encode_once, [] {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      g_encode = reinterpret_cast<EncodeTiledFn>(fn);
-  });
-  return g_encode;
-}
-
 int make_map_2d(CUtensorMap* map, CUtensorMapDataType dt, const void* base, uint64_t inner, uint64_t outer,
                 uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, CUtensorMapSwizzle sw) {
-  EncodeTiledFn enc = get_encode();
+  EncodeTiledFn enc = tensor_map_encoder();
   if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return 4; }
   cuuint64_t dims[2] = {inner, outer};
   cuuint64_t strides[1] = {row_stride_bytes};
@@ -655,7 +635,7 @@ int make_map_2d(CUtensorMap* map, CUtensorMapDataType dt, const void* base, uint
 // BB_TILE_SLAB storage [N/32][row_bytes/512][32][512 B] as a 4-D tensor; box = {PRB bytes, 32 rows, 1 segment, 4 row blocks}
 // lands in shared memory as the same dense [128 rows][PRB] tile the row-major 2-D box produces
 int make_map_w_tiled(CUtensorMap* map, const void* base, uint64_t row_bytes, uint64_t rows, uint32_t prb) {
-  EncodeTiledFn enc = get_encode();
+  EncodeTiledFn enc = tensor_map_encoder();
   if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return 4; }
   const uint64_t upr = row_bytes / BB_TILE_ROW_BYTES;
   cuuint64_t dims[4] = {BB_TILE_ROW_BYTES, BB_TILE_ROWS, upr, rows / BB_TILE_ROWS};
@@ -767,8 +747,6 @@ size_t gemm_ts_workspace_bytes(const bb_matmul_desc& d, int m) {
   const int sp = choose_splits(tiles, d.K / kb, device_sm_count());
   return sp > 1 ? size_t(sp) * m * d.N * 4 : 0;
 }
-
-int gemm_ts_init(int) { return get_encode() ? 0 : 0; }
 
 int launch_gemm_ts(const MatmulArgs& a) {
   const bb_matmul_desc& d = a.d;

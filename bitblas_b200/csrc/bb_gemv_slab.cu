@@ -10,7 +10,8 @@
 //     (tools/slabbench.cu compares them); bandwidth then depends only on the bytes in flight.  Units are ordered (row-block group, k, member) and cut into equal contiguous ranges over a persistent grid
 //     (CTA-level stream-K): every SM streams the same number of bytes whatever N, K are; a 1024-row tensor-parallel shard
 //     still fills all 132 SMs of an H100.
-//   * a CTA = NG consumer GROUPS of 4 warps + an issuer warp + NF finisher warps around an S-stage mbarrier ring.  Group g
+//   * a CTA = NG = 2 consumer GROUPS of 4 warps + an issuer warp + NF = 1 finisher warp around an S = 4-stage mbarrier ring, two
+//     CTAs per SM.  Group g
 //     consumes the units whose row block is g (mod NG) -- whole row blocks per group, so a group reduces, exchanges stream-K
 //     partials and stores on its own, with a 128-thread named barrier; nothing ever synchronises the whole CTA.  The
 //     consumers issue NO global loads: weights, activations, group parameters and activation sums are all in the stage when its
@@ -33,11 +34,8 @@
 //   * programmatic dependent launch: weights and parameters of the first S units are requested before griddepcontrol.wait,
 //     activations after it; launch_dependents is raised at kernel entry -- the grid is persistent and fully resident, so the
 //     next kernel's CTAs can only take slots that this kernel's CTAs have vacated, and its prefetch overlaps our tail.
-#include <cuda.h>
-
 #include <atomic>
 #include <algorithm>
-#include <cstdlib>
 #include <cstring>
 #include <mutex>
 
@@ -59,12 +57,19 @@ constexpr int GS_PBYTES = GS_STEPS * GS_ROWS * 8;   // (c1, c2) fp32 pairs [step
 constexpr int GS_SBYTES = GS_STEPS * 8;             // (SM, S) fp32 pairs [step]
 constexpr int GS_RAWBYTES = 1024;                   // raw scales [32 rows][8 groups] fp16 + raw zeros (fp16 [32][8] or packed [8 groups][16 B])
 constexpr int GS_RED_GROUP_BYTES = 2 * (2 * GS_GW) * GS_ROWS * 4;   // per group: two buffers x (4 warps x 2 k-halves) partials x 32 rows
-constexpr int GS_MAX_STAGES = 10;
+constexpr int GS_NG = 2;                            // consumer groups per CTA
+constexpr int GS_MINB = 2;                          // CTAs per SM
+constexpr int GS_STAGES = 4;                        // ring depth
+constexpr int GS_NF = 1;                            // finisher warps; finisher f serves the units i = f (mod GS_NF) of the range
+// slot s of the ring always belongs to group s % GS_NG (and finisher s % GS_NF), which therefore sees every phase of the slot's
+// barriers (a group that skipped a phase would mistake the parity of a later one for its own)
+static_assert(GS_STAGES % GS_NG == 0 && GS_STAGES % GS_NF == 0, "the ring depth must be a multiple of the group and finisher counts");
+constexpr int GS_THREADS = (GS_GW * GS_NG + 1 + GS_NF) * 32;   // consumers + issuer + finishers
+constexpr int GS_SMEM_BYTES = 1024 + GS_STAGES * (GS_WBYTES + GS_ABYTES + GS_PBYTES + GS_RAWBYTES + GS_SBYTES) +
+                              GS_NG * GS_RED_GROUP_BYTES + 32 * GS_STAGES + 64;
 constexpr uint32_t GS_SUSPEND_NS = 20000;   // try_wait suspend-time hint: a waiting warp sleeps in hardware until the phase flips
                                              // instead of re-issuing the probe (the default limit re-issued it ~12 times per wait: 14 %
                                              // of all issued instructions were wait-loop instructions)
-
-__host__ __device__ constexpr int gs_threads(int NG, int NF) { return (GS_GW * NG + 1 + NF) * 32; }   // consumers + issuer + finishers
 
 struct SlabParams {
   const void* A;
@@ -82,11 +87,8 @@ struct SlabParams {
   int UPR;          // units per 32-row block = ceil(K / 1024)
   int NRB;          // 32-row blocks = ceil(N / 32)
   int T;            // units in total, padded to whole row-block groups
-  int stages;
   unsigned long long* ws;   // [grid][NG][32] tagged partial slots, zero-tagged on entry and on exit
   unsigned int nonce;
-  int dbg;          // tuning diagnostics (BB_GS_DBG): 1 = consumers skip the arithmetic, 4 = no sums, 16 = no parameter conversion
-                    // (results are wrong with any of them set)
   const void* lut;   // NF4 table (16 x A_dtype) for the FMT = 1 instances, else null
   int w_fmt;         // bb_wfmt
   const uint8_t* Wt; // BB_TILE_SLAB storage (else null): unit (rb, ku) is the contiguous 16 KB block number rb * UPR + ku
@@ -207,22 +209,18 @@ __device__ __forceinline__ void gs_store(const SlabParams& p, int n, float v) {
 __device__ __forceinline__ int gs_range_begin(int ri, int T, int R) { return int((long long)ri * T / R); }
 
 
-// NG consumer groups per CTA, MINB CTAs per SM: (2, 2) or (4, 1).  SC = ring depth as a compile-time constant (0: p.stages at run
-// time, the tuning / test variant): with a constant depth every stage address is base + immediate -- the run-time variant spends
-// ~40 integer instructions per unit and warp re-deriving the region bases
-// NF = finisher warps (S % NF == 0; finisher f serves the units i = f (mod NF) of the range)
 // FMT: 0 = uint4 / int4 (LOP3 magic decode, magic and zero point removed through the activation sums), 1 = 16-entry table formats
 // (NF4 / fp4, compressed storage: PRMT table decode to exact A_dtype values, scale only -- the sums are not needed)
-template <typename T, bool IL, int NG, int MINB, int SC, int NF, int FMT = 0>
-__global__ void __launch_bounds__(gs_threads(NG, NF), MINB)
+template <typename T, bool IL, int FMT>
+__global__ void __launch_bounds__(GS_THREADS, GS_MINB)
 gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
   constexpr bool F16 = std::is_same<T, __half>::value;
   constexpr bool HI = F16 && FMT == 0;   // odd nibbles decoded in place (mantissa bits 4..7 under exponent 2^6: exactly 64 + u)
   constexpr uint32_t MAGIC = TypeTraits<T>::kMagic;
   constexpr uint32_t MAGIC_HI = 0x54005400u;
+  constexpr int NG = GS_NG, NF = GS_NF, S = GS_STAGES;
   constexpr int NCW = GS_GW * NG;            // consumer warps
   extern __shared__ uint8_t gs_raw[];
-  const int S = SC > 0 ? SC : p.stages;
   const uint32_t base = (gs_smem_u32(gs_raw) + 1023u) & ~1023u;
   const uint32_t Wb = base;                                   // [S][32 rows][512 B]
   const uint32_t Ab = Wb + uint32_t(S) * GS_WBYTES;           // [S][1024 halves]
@@ -360,87 +358,83 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
     for (int i = f; i < n_units; i += NF) {
       // ---- activation sums ----
       gs_mbar_wait(Bb + 8u * slot, phase);
-      if (!(p.dbg & 4)) {
-        const uint32_t abase = Ab + uint32_t(slot) * GS_ABYTES;
-        // column g8 of the B operand = step g8; its 16-k blocks are visited in an order rotated by g8 (bank spread) -- any order
-        // is fine as long as (physical k) = (MMA k slot) mod 8, which the magic-pattern row relies on; two independent chains
-        uint32_t bf[8][2];
+      const uint32_t abase = Ab + uint32_t(slot) * GS_ABYTES;
+      // column g8 of the B operand = step g8; its 16-k blocks are visited in an order rotated by g8 (bank spread) -- any order
+      // is fine as long as (physical k) = (MMA k slot) mod 8, which the magic-pattern row relies on; two independent chains
+      uint32_t bf[8][2];
 #pragma unroll
-        for (int ms = 0; ms < 8; ++ms) {
-          const uint32_t a = abase + uint32_t(g8 * 128 + ((ms + g8) & 7) * 16 + 2 * t4) * 2u;
-          bf[ms][0] = gs_lds32(a);
-          bf[ms][1] = gs_lds32(a + 16u);
-        }
-        float c0[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int ms = 0; ms < 8; ++ms) {
+        const uint32_t a = abase + uint32_t(g8 * 128 + ((ms + g8) & 7) * 16 + 2 * t4) * 2u;
+        bf[ms][0] = gs_lds32(a);
+        bf[ms][1] = gs_lds32(a + 16u);
+      }
+      float c0[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-        for (int ms = 0; ms < 4; ++ms) {
-          gs_mma<T>(c0, sfrag, bf[ms][0], bf[ms][1]);
-          gs_mma<T>(c1, sfrag, bf[ms + 4][0], bf[ms + 4][1]);
-        }
-        if (g8 < 2) {   // row 0: S -> .y, row 1: SM -> .x
-          const uint32_t d = Sb + uint32_t(slot) * GS_SBYTES + uint32_t(2 * t4) * 8u + (g8 == 0 ? 4u : 0u);
-          gs_sts32f(d, c0[0] + c1[0]);
-          gs_sts32f(d + 8u, c0[1] + c1[1]);
-        }
+      for (int ms = 0; ms < 4; ++ms) {
+        gs_mma<T>(c0, sfrag, bf[ms][0], bf[ms][1]);
+        gs_mma<T>(c1, sfrag, bf[ms + 4][0], bf[ms + 4][1]);
+      }
+      if (g8 < 2) {   // row 0: S -> .y, row 1: SM -> .x
+        const uint32_t d = Sb + uint32_t(slot) * GS_SBYTES + uint32_t(2 * t4) * 8u + (g8 == 0 ? 4u : 0u);
+        gs_sts32f(d, c0[0] + c1[0]);
+        gs_sts32f(d + 8u, c0[1] + c1[1]);
       }
       // ---- group parameters -> fp32 (c1, c2) pairs ----
       gs_mbar_wait(Bb + 8u * (2 * S + slot), phase);
-      if (!(p.dbg & 16)) {
-        uint32_t sc[8], zc[8];   // raw 16-bit scales; raw fp16 zeros or (quantized) the byte holding this row's zero point
-        if (unit_fast(rb, ku)) {
-          const uint32_t raw = RAWb + uint32_t(slot) * GS_RAWBYTES;
-          const uint4 s4 = gs_lds128(raw + uint32_t(lane) * 16u);
-          const uint32_t sw[4] = {s4.x, s4.y, s4.z, s4.w};
+      uint32_t sc[8], zc[8];   // raw 16-bit scales; raw fp16 zeros or (quantized) the byte holding this row's zero point
+      if (unit_fast(rb, ku)) {
+        const uint32_t raw = RAWb + uint32_t(slot) * GS_RAWBYTES;
+        const uint4 s4 = gs_lds128(raw + uint32_t(lane) * 16u);
+        const uint32_t sw[4] = {s4.x, s4.y, s4.z, s4.w};
 #pragma unroll
-          for (int st = 0; st < 8; ++st) sc[st] = (st & 1) ? (sw[st >> 1] >> 16) : (sw[st >> 1] & 0xffffu);
-          if (p.zmode == 3) {
+        for (int st = 0; st < 8; ++st) sc[st] = (st & 1) ? (sw[st >> 1] >> 16) : (sw[st >> 1] & 0xffffu);
+        if (p.zmode == 3) {
 #pragma unroll
-            for (int st = 0; st < 8; ++st) zc[st] = gs_lds8(raw + 512u + uint32_t(st) * 16u + uint32_t(lane >> 1));
-          } else {
-            const uint4 z4 = gs_lds128(raw + 512u + uint32_t(lane) * 16u);
-            const uint32_t zw[4] = {z4.x, z4.y, z4.z, z4.w};
-#pragma unroll
-            for (int st = 0; st < 8; ++st) zc[st] = (st & 1) ? (zw[st >> 1] >> 16) : (zw[st >> 1] & 0xffffu);
-          }
+          for (int st = 0; st < 8; ++st) zc[st] = gs_lds8(raw + 512u + uint32_t(st) * 16u + uint32_t(lane >> 1));
         } else {
-          // slow path (group size != 128, unaligned parameter tensors, N % 32 != 0, a row block's ragged last unit): synchronous loads
-          const int n = rb * GS_ROWS + lane;
-          const int kstep = ku * GS_STEPS;
-          int gi = kstep / p.g128, rem = kstep - gi * p.g128;
+          const uint4 z4 = gs_lds128(raw + 512u + uint32_t(lane) * 16u);
+          const uint32_t zw[4] = {z4.x, z4.y, z4.z, z4.w};
 #pragma unroll
-          for (int st = 0; st < 8; ++st) {
-            sc[st] = 0u; zc[st] = 0u;
-            if (kstep + st < steps_total && n < p.N) {
-              if (p.with_scaling) sc[st] = __ldg(scale16 + size_t(n) * p.G + gi);
-              if (p.zmode == 1 || p.zmode == 2) zc[st] = __ldg(zeros16 + size_t(n) * p.G + gi);
-              else if (p.zmode == 3) zc[st] = __ldg(zeros8 + size_t(gi) * (p.N >> 1) + (n >> 1));
-            }
-            if (++rem == p.g128) { rem = 0; ++gi; }
-          }
+          for (int st = 0; st < 8; ++st) zc[st] = (st & 1) ? (zw[st >> 1] >> 16) : (zw[st >> 1] & 0xffffu);
         }
-        const uint32_t pbase = Pb + uint32_t(slot) * GS_PBYTES + uint32_t(lane) * 8u;
-        // the zero-point mode is hoisted out of the per-step loop (a switch inside it compiles to eight indirect branches)
-        auto body = [&](auto zm_tag, auto sc_tag) {
-          constexpr int ZM = decltype(zm_tag)::value;
-          constexpr bool SC = decltype(sc_tag)::value;
+      } else {
+        // slow path (group size != 128, unaligned parameter tensors, N % 32 != 0, a row block's ragged last unit): synchronous loads
+        const int n = rb * GS_ROWS + lane;
+        const int kstep = ku * GS_STEPS;
+        int gi = kstep / p.g128, rem = kstep - gi * p.g128;
 #pragma unroll
-          for (int st = 0; st < 8; ++st) {
-            const float c1 = SC ? gs_raw_to_float<T>(sc[st]) : 1.f;
-            float c2;
-            if constexpr (ZM == 0) c2 = -c1 * float(p.zp_const);
-            else if constexpr (ZM == 1) c2 = -c1 * gs_raw_to_float<T>(zc[st]);
-            else if constexpr (ZM == 2) c2 = -gs_raw_to_float<T>(zc[st]);
-            else c2 = -c1 * float((zc[st] >> zsh) & 15u);
-            gs_sts64f(pbase + uint32_t(st) * (GS_ROWS * 8u), c1, c2);
+        for (int st = 0; st < 8; ++st) {
+          sc[st] = 0u; zc[st] = 0u;
+          if (kstep + st < steps_total && n < p.N) {
+            if (p.with_scaling) sc[st] = __ldg(scale16 + size_t(n) * p.G + gi);
+            if (p.zmode == 1 || p.zmode == 2) zc[st] = __ldg(zeros16 + size_t(n) * p.G + gi);
+            else if (p.zmode == 3) zc[st] = __ldg(zeros8 + size_t(gi) * (p.N >> 1) + (n >> 1));
           }
-        };
-        using std::integral_constant;
-        if (!p.with_scaling) body(integral_constant<int, 0>{}, std::false_type{});   // (zeros need scaling: gemv_slab_supported)
-        else if (p.zmode == 0) body(integral_constant<int, 0>{}, std::true_type{});
-        else if (p.zmode == 1) body(integral_constant<int, 1>{}, std::true_type{});
-        else if (p.zmode == 2) body(integral_constant<int, 2>{}, std::true_type{});
-        else body(integral_constant<int, 3>{}, std::true_type{});
+          if (++rem == p.g128) { rem = 0; ++gi; }
+        }
       }
+      const uint32_t pbase = Pb + uint32_t(slot) * GS_PBYTES + uint32_t(lane) * 8u;
+      // the zero-point mode is hoisted out of the per-step loop (a switch inside it compiles to eight indirect branches)
+      auto body = [&](auto zm_tag, auto sc_tag) {
+        constexpr int ZM = decltype(zm_tag)::value;
+        constexpr bool SC = decltype(sc_tag)::value;
+#pragma unroll
+        for (int st = 0; st < 8; ++st) {
+          const float c1 = SC ? gs_raw_to_float<T>(sc[st]) : 1.f;
+          float c2;
+          if constexpr (ZM == 0) c2 = -c1 * float(p.zp_const);
+          else if constexpr (ZM == 1) c2 = -c1 * gs_raw_to_float<T>(zc[st]);
+          else if constexpr (ZM == 2) c2 = -gs_raw_to_float<T>(zc[st]);
+          else c2 = -c1 * float((zc[st] >> zsh) & 15u);
+          gs_sts64f(pbase + uint32_t(st) * (GS_ROWS * 8u), c1, c2);
+        }
+      };
+      using std::integral_constant;
+      if (!p.with_scaling) body(integral_constant<int, 0>{}, std::false_type{});   // (zeros need scaling: gemv_slab_supported)
+      else if (p.zmode == 0) body(integral_constant<int, 0>{}, std::true_type{});
+      else if (p.zmode == 1) body(integral_constant<int, 1>{}, std::true_type{});
+      else if (p.zmode == 2) body(integral_constant<int, 2>{}, std::true_type{});
+      else body(integral_constant<int, 3>{}, std::true_type{});
       __syncwarp();
       if (lane == 0) gs_mbar_arrive(Bb + 8u * (S + slot));
       slot += NF;                       // S % NF == 0: the slot sequence of this warp closes on itself
@@ -493,7 +487,9 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
     if (!seg_open) { seg_from0 = (ku == 0); seg_open = true; }
     const bool closes = (ku == UPR - 1);
     gs_mbar_wait(Bb + 8u * slot, fphase);   // weights + activations have landed
-    const bool active = (!closes || ws < nsl_last) && rb < p.NRB && !(p.dbg & 1);
+    // (p.N > 0 always holds; the run-time term keeps ptxas's register allocation of the fp16 compressed-word instance: without it
+    //  that instance spills 38 / 64 B instead of 16 / 24 B, partly inside this loop, and runs 3-5 % slower on an H100)
+    const bool active = (!closes || ws < nsl_last) && rb < p.NRB && p.N > 0;
     float cc[4][4];
     if (active) {
       const uint32_t wst = Wb + uint32_t(slot) * GS_WBYTES + woff;
@@ -641,19 +637,6 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-typedef CUresult (*GsEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-GsEncodeFn gs_encode() {
-  static GsEncodeFn fn = [] {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) f = nullptr;
-    return reinterpret_cast<GsEncodeFn>(f);
-  }();
-  return fn;
-}
-
 // a tensor map is a pure function of (device pointer, N, K): cached, so a steady-state launch makes no driver call
 struct MapEntry { const void* W; int N, K; CUtensorMap map; unsigned long long stamp; };
 constexpr int GS_MAP_CACHE = 256;
@@ -667,7 +650,7 @@ bool get_w_map(CUtensorMap* tm, const void* W, int N, int K) {
   ++g_map_clock;
   for (int i = 0; i < g_map_count; ++i)
     if (g_maps[i].W == W && g_maps[i].N == N && g_maps[i].K == K) { g_maps[i].stamp = g_map_clock; *tm = g_maps[i].map; return true; }
-  GsEncodeFn enc = gs_encode();
+  EncodeTiledFn enc = tensor_map_encoder();
   if (!enc) return false;
   CUtensorMap m;
   const cuuint64_t Kb = cuuint64_t(K) / 2;
@@ -690,49 +673,46 @@ bool get_w_map(CUtensorMap* tm, const void* W, int N, int K) {
 }
 
 
-int gs_smem_bytes(int stages, int NG) {
-  return 1024 + stages * (GS_WBYTES + GS_ABYTES + GS_PBYTES + GS_RAWBYTES + GS_SBYTES) + NG * GS_RED_GROUP_BYTES + 32 * stages + 64;
-}
-
-int env_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return e ? atoi(e) : dflt;
-}
-
-constexpr int GS_MAX_DEVICES = BB_MAX_DEVICES;
-
-template <typename KernelT>
-int gs_occupancy(KernelT k, int variant, int threads, int smem, int dev) {
-  // per (kernel variant, device): opt-in shared memory once (the device maximum); per dynamic size: occupancy, cached
-  struct Entry { int smem, occ; };
-  static std::mutex mu;
-  static Entry cache[32][GS_MAX_DEVICES][8];
-  static int used[32][GS_MAX_DEVICES];
-  static bool attr[32][GS_MAX_DEVICES];
-  static bool init = false;
-  std::lock_guard<std::mutex> lk(mu);
-  if (!init) { memset(cache, 0, sizeof(cache)); memset(used, 0, sizeof(used)); memset(attr, 0, sizeof(attr)); init = true; }
-  if (!attr[variant][dev]) {
+// CTAs per SM of one instance on the current device (< 0: it does not fit), queried once per device; the shared-memory opt-in
+// (the device maximum) is a per-device function attribute
+template <typename T, bool IL, int FMT>
+int gs_occupancy(int dev) {
+  static std::atomic<int> occ_dev[BB_MAX_DEVICES];   // 0 = not queried yet
+  int occ = occ_dev[dev].load(std::memory_order_relaxed);
+  if (occ == 0) {
+    auto k = gemv_slab_kernel<T, IL, FMT>;
     int optin = 0;
     if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess) { cudaGetLastError(); return -1; }
     if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, optin) != cudaSuccess) { cudaGetLastError(); return -1; }
-    attr[variant][dev] = true;
+    int o = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, k, GS_THREADS, size_t(GS_SMEM_BYTES)) != cudaSuccess) { cudaGetLastError(); o = 0; }
+    occ = o < 1 ? -1 : o;
+    occ_dev[dev].store(occ, std::memory_order_relaxed);
   }
-  Entry* e = cache[variant][dev];
-  int& n = used[variant][dev];
-  for (int i = 0; i < n; ++i) if (e[i].smem == smem) return e[i].occ;
-  int o = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, k, threads, size_t(smem)) != cudaSuccess) { cudaGetLastError(); o = 0; }
-  const int occ = o < 1 ? -1 : o;
-  const int slot = n < 8 ? n++ : 7;
-  e[slot] = Entry{smem, occ};
   return occ;
+}
+
+template <typename T, bool IL, int FMT>
+int launch_slab(const MatmulArgs& a, const CUtensorMap& tm, const SlabParams& p) {
+  const int occ = gs_occupancy<T, IL, FMT>(current_device());
+  if (occ < 0) { set_error("gemv_slab: kernel does not fit on this device"); return 4; }
+  const int grid = std::max(1, std::min(p.T, std::min(occ, GS_MINB) * device_sm_count()));
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(GS_THREADS);
+  cfg.dynamicSmemBytes = GS_SMEM_BYTES; cfg.stream = a.stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+  cfg.attrs = attr; cfg.numAttrs = 1;
+  BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemv_slab_kernel<T, IL, FMT>, tm, p));
+  BB_LAUNCH_CHECK();
+  return 0;
 }
 
 }  // namespace
 
-// tagged exchange slots: [CTAs][consumer groups][32 rows]; CTAs x groups <= 4 per SM in every configuration
-size_t gemv_slab_workspace_bytes() { return size_t(4) * size_t(device_sm_count()) * GS_ROWS * 8 + 256; }
+// tagged exchange slots: [CTAs][consumer groups][32 rows], at most GS_MINB CTAs per SM
+size_t gemv_slab_workspace_bytes() { return size_t(GS_MINB * GS_NG) * size_t(device_sm_count()) * GS_ROWS * 8 + 256; }
 
 bool gemv_slab_supported(const bb_matmul_desc& d, int m) {
   if (m != 1) return false;
@@ -767,11 +747,6 @@ int launch_gemv_slab(const MatmulArgs& a) {
     set_error("gemv_slab needs a zero-initialised workspace of %zu bytes (bb_workspace_bytes)", gemv_slab_workspace_bytes());
     return 5;
   }
-  const int dev = current_device();
-  // consumer groups per CTA x CTAs per SM: (4, 1) shares one deep ring between four groups, (2, 2) runs two CTAs per SM
-  const bool table_fmt = d.w_fmt == BB_W_NF || d.w_fmt == BB_W_FP4;
-  const int ng = (!table_fmt && env_int("BB_GS_NG", 2) == 4) ? 4 : 2;
-  const int nf = env_int("BB_GS_NF", 1) == 2 ? 2 : 1;   // finisher warps of the (2 groups, 4 stages) configuration
   SlabParams p;
   p.A = a.A; p.scale = d.with_scaling ? a.scale : nullptr; p.zeros = d.with_zeros ? a.zeros : nullptr;
   p.bias = d.with_bias ? a.bias : nullptr; p.out = make_outspec(a);
@@ -782,15 +757,9 @@ int launch_gemv_slab(const MatmulArgs& a) {
   p.out_dtype = d.out_dtype;
   p.UPR = (d.K + GS_KU - 1) / GS_KU;
   p.NRB = (d.N + GS_ROWS - 1) / GS_ROWS;
-  p.T = ((p.NRB + ng - 1) / ng) * p.UPR * ng;
-  // the ring depth must be a multiple of the group count: slot s then always belongs to group s % NG, which therefore sees every
-  // phase of the slot's barriers (a group that skipped a phase would mistake the parity of a later one for its own)
+  p.T = ((p.NRB + GS_NG - 1) / GS_NG) * p.UPR * GS_NG;
   p.lut = d.w_fmt == BB_W_NF ? a.lut : nullptr;
   p.w_fmt = d.w_fmt;
-  int stages = table_fmt ? 4 : env_int("BB_GS_STAGES", ng == 4 ? 8 : 4);
-  stages = std::max(ng, std::min(GS_MAX_STAGES, stages) / ng * ng);
-  p.stages = stages;
-  p.dbg = env_int("BB_GS_DBG", 0);
   CUtensorMap tm;
   p.Wt = nullptr;
   if (d.w_tile == BB_TILE_SLAB) {
@@ -807,41 +776,10 @@ int launch_gemv_slab(const MatmulArgs& a) {
   p.nonce = nz | 1u;
   const bool il = d.w_layout == BB_LAYOUT_INTERLEAVED_16;
   const bool f16 = d.a_dtype == BB_F16;
-  const int smem = gs_smem_bytes(stages, ng);
-  const int sms = device_sm_count();
-  static const bool pdl = [] { const char* e = getenv("BB_PDL"); return e ? atoi(e) != 0 : true; }();
-
-#define BB_GS_GO(TT, ILV, NGV, MINBV, SCV, NFV, FMTV, VAR)                                                 \
-  {                                                                                                    \
-    auto k = gemv_slab_kernel<TT, ILV, NGV, MINBV, SCV, NFV, FMTV>;                                    \
-    int occ = gs_occupancy(k, VAR, gs_threads(NGV, NFV), smem, dev);                                   \
-    if (occ < 0) { set_error("gemv_slab: kernel does not fit on this device (stages=%d)", stages); return 4; } \
-    occ = std::min(occ, MINBV);                                                                        \
-    const int grid = std::max(1, std::min(p.T, occ * sms));                                            \
-    cudaLaunchConfig_t cfg = {};                                                                       \
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(gs_threads(NGV, NFV));                               \
-    cfg.dynamicSmemBytes = smem; cfg.stream = a.stream;                                                \
-    cudaLaunchAttribute attr[1];                                                                       \
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                   \
-    attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;                                  \
-    cfg.attrs = attr; cfg.numAttrs = 1;                                                                \
-    BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, k, tm, p));                                                 \
-  }
-  // the shipped configuration (2 groups, 4 stages) has the ring depth compiled in; every other knob setting runs the run-time-depth
-  // variants (tuning sweeps, tests of the ring logic)
-#define BB_GS_NG(TT, ILV, VB)                                                  \
-  if (ng == 4) BB_GS_GO(TT, ILV, 4, 1, 0, 2, 0, VB + 0)                           \
-  else if (stages == 4 && nf == 2) BB_GS_GO(TT, ILV, 2, 2, 4, 2, 0, VB + 1)       \
-  else if (stages == 4) BB_GS_GO(TT, ILV, 2, 2, 4, 1, 0, VB + 2)                  \
-  else BB_GS_GO(TT, ILV, 2, 2, 0, 1, 0, VB + 3)
-  if (table_fmt) {   // one instance per activation type: 2 groups x 2 CTAs/SM, 4 stages, 1 finisher
-    if (f16) BB_GS_GO(__half, false, 2, 2, 4, 1, 1, 16) else BB_GS_GO(__nv_bfloat16, false, 2, 2, 4, 1, 1, 17)
-  } else if (f16) { if (il) { BB_GS_NG(__half, true, 0) } else { BB_GS_NG(__half, false, 4) } }
-  else { if (il) { BB_GS_NG(__nv_bfloat16, true, 8) } else { BB_GS_NG(__nv_bfloat16, false, 12) } }
-#undef BB_GS_NG
-#undef BB_GS_GO
-  BB_LAUNCH_CHECK();
-  return 0;
+  if (d.w_fmt == BB_W_NF || d.w_fmt == BB_W_FP4)   // table formats: compressed storage only
+    return f16 ? launch_slab<__half, false, 1>(a, tm, p) : launch_slab<__nv_bfloat16, false, 1>(a, tm, p);
+  if (f16) return il ? launch_slab<__half, true, 0>(a, tm, p) : launch_slab<__half, false, 0>(a, tm, p);
+  return il ? launch_slab<__nv_bfloat16, true, 0>(a, tm, p) : launch_slab<__nv_bfloat16, false, 0>(a, tm, p);
 }
 
 }  // namespace bb

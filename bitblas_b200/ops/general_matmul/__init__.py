@@ -457,7 +457,7 @@ class Matmul(Operator):
 
     def _workspace_for(self, m: int, device, stream=None):
         """scratch the kernel picked for `m` needs (bb_workspace_bytes: split-K partials, stream-K exchange slots); one cached,
-        ZERO-INITIALISED buffer per operator, device and stream, grown on demand.  The stream-K kernels leave their slots
+        ZERO-INITIALISED buffer per operator, device and stream, grown on demand.  The m = 1 slab kernel leaves its slots
         zero-tagged, so the buffer is reused by later calls on the same stream without clearing (include/bitblas_b200.h)."""
         key = (int(m), _lib.OVERRIDE_GEN)
         need = self._ws_need.get(key)

@@ -106,8 +106,6 @@ typedef enum bb_kernel_id {
   BB_KERNEL_GEMV_I8 = 3,   /* m <= 32, int8 A, 4/2-bit W: IMMA streaming, int32 exact         */
   BB_KERNEL_GEMM_TS = 4,   /* wgmma (W dequantised into registers as the MMA A operand) + TMA */
   BB_KERNEL_GEMM_TS_I8 = 5,/* wgmma int8 variant                                             */
-  BB_KERNEL_GEMV_STREAMK = 6,/* m <= 2, 4-bit W: persistent stream-K + TMA rings; opt-in through
-                              * bb_set_kernel_override only */
   BB_KERNEL_GEMV_SLAB = 7    /* m == 1, 4-bit W, fp16/bf16 A: per-CTA TMA slabs + CTA-level stream-K; the default
                               * decode kernel (needs the zero-initialised workspace of bb_workspace_bytes) */
 } bb_kernel_id;
@@ -145,9 +143,10 @@ int bb_matmul_scatter(const bb_matmul_desc* desc, const void* A, const void* W, 
 #define BB_PEER_FLAG_BYTES 128
 int bb_peer_barrier(void* const* peer_flags, int n_peers, int rank, void* stream);
 
-/* scratch (fp32 split-K partials; stream-K slots + flags) the chosen kernel needs for this (desc, m); 0 for most configs.
- * The buffer must be ZERO-INITIALISED once by the caller before its first use (cudaMemset / torch.zeros): the stream-K
- * kernels exchange partial sums through tagged slots and leave every slot zero-tagged again when they finish, so the same
+/* scratch (the m = 1 slab kernel's tagged partial-sum slots; the wgmma kernel's fp32 split-K partials) the chosen kernel
+ * needs for this (desc, m); 0 for most configs.
+ * The buffer must be ZERO-INITIALISED once by the caller before its first use (cudaMemset / torch.zeros): the slab kernel
+ * exchanges partial sums through tagged slots and leaves every slot zero-tagged again when it finishes, so the same
  * buffer can then be reused by later calls ON THE SAME STREAM without clearing (calls that may run concurrently need their
  * own buffers).  The split-K partials of the wgmma kernel carry no such requirement. */
 size_t bb_workspace_bytes(const bb_matmul_desc* desc, int m);

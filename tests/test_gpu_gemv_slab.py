@@ -1,10 +1,9 @@
 """GPU parity of the m = 1 decode kernel (bb_gemv_slab.cu: per-CTA TMA slabs + CTA-level stream-K), through the C ABI
 (Matmul.forward -> bb_matmul), against the CPU oracle on the same seeded inputs -- small shapes that exercise every
-zero-point mode / layout / ragged-K path, the tuning knobs, and the BASELINE.json shapes (C1: Llama-2-70B linears + the
+zero-point mode / layout / ragged-K path, and the BASELINE.json shapes (C1: Llama-2-70B linears + the
 12288^2 target) with the FULL output compared.  Mirrors the reference's
 testing/python/operators/test_general_matmul_ops_backend_tl.py:127-283 (tolerance rtol = atol = 1e-2)."""
 import ctypes
-import os
 
 import pytest
 import torch
@@ -31,6 +30,7 @@ SLAB_CASES = [
     dict(N=2064, K=3840, **Q),                                              # ragged last unit (7 valid slices), N/16 odd
     dict(N=4096, K=4096, **Q),
     dict(N=4112, K=6144, with_bias=True, **Q),                              # ranges start and end inside row blocks
+    dict(N=96, K=11264, with_bias=True, **Q),                               # tiny N, long K: few row blocks over many CTAs
     dict(N=512, K=8192, W_dtype="uint4", group_size=1024, with_scaling=True, with_zeros=True, zeros_mode="quantized"),
     dict(N=512, K=3072, W_dtype="uint4", group_size=384, with_scaling=True, with_zeros=True, zeros_mode="original"),   # 128 | g, g not a power of 2
     dict(N=1024, K=2048, W_dtype="uint4", fast_decoding=False, group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized"),
@@ -44,20 +44,10 @@ def _ids(k):
     return "-".join(f"{a}{b}" for a, b in k.items())
 
 
-def _slab(case, **env):
-    old = {k: os.environ.get(k) for k in env}
-    os.environ.update({k: str(v) for k, v in env.items()})
-    try:
-        op = H.product_operator(case)
-        assert op.kernel_for(1) == "gemv_slab", op.kernel_for(1)
-        got = H.run_product(op, case)
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
-    return op, got
+def _slab(case):
+    op = H.product_operator(case)
+    assert op.kernel_for(1) == "gemv_slab", op.kernel_for(1)
+    return op, H.run_product(op, case)
 
 
 @pytest.mark.parametrize("kw", SLAB_CASES, ids=_ids)
@@ -70,17 +60,6 @@ def test_gemv_slab_parity(kw):
     # the summation order is fixed (CTA reduction + ordered stream-K fix-up): a second run is bit-identical
     got2 = H.run_product(op, case)
     assert torch.equal(got, got2)
-
-
-@pytest.mark.parametrize("stages,groups", [(4, 4), (8, 4), (2, 2), (4, 2), (6, 2)])
-@pytest.mark.parametrize("N,K", [(4112, 6144), (96, 11264)])
-def test_gemv_slab_knobs(stages, groups, N, K):
-    """ring depth and consumer groups per CTA (4 groups x 1 CTA per SM, 2 groups x 2 CTAs per SM) give the same answer: the
-    stream-K boundaries and the padding units past the last row block move with the grid and the group count."""
-    case = H.make_case(1, N, K, with_bias=True, **Q)
-    ref = H.oracle_output(case, fast_decoding=True)
-    _, got = _slab(case, BB_GS_STAGES=stages, BB_GS_NG=groups)
-    H.assert_fp_close(got, ref, f"gemv_slab stages={stages} groups={groups}")
 
 
 # BASELINE.json configs[1] (C1: W4A16 GEMV M=1 on the Llama-2-70B linears) + the 12288^2 target shape, full output vs the oracle

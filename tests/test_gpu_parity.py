@@ -63,89 +63,6 @@ def test_gemv_mma_parity(kw):
     H.assert_fp_close(got, ref, "gemv_mma")
 
 
-# stream-K TMA kernel (m <= 2, 4-bit, group scales, no / quantized zeros, K/group a multiple of 8, N % 32 == 0).  Shapes are
-# chosen so that warp ranges start and end inside row blocks (partials parked in the workspace and collected by the warp
-# that closes the block), cover one warp per chunk (tiny T), several segments per warp, group sizes 128 / 256 / 1024.
-STREAMK_CASES = [
-    dict(M=1, N=32, K=1024, W_dtype="uint4", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized"),
-    dict(M=2, N=96, K=2048, W_dtype="uint4", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized", with_bias=True),
-    dict(M=1, N=4096, K=4096, W_dtype="uint4", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized"),
-    dict(M=2, N=2080, K=3072, W_dtype="uint4", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized"),
-    dict(M=1, N=1056, K=2048, W_dtype="uint4", group_size=256, with_scaling=True, with_zeros=True, zeros_mode="quantized", with_bias=True),
-    dict(M=1, N=512, K=8192, W_dtype="uint4", group_size=1024, with_scaling=True, with_zeros=True, zeros_mode="quantized"),
-    dict(M=1, N=8192, K=1024, W_dtype="int4", group_size=128, with_scaling=True),
-    dict(M=2, N=1024, K=2048, W_dtype="uint4", group_size=128, with_scaling=True),
-    dict(M=1, N=1024, K=2048, W_dtype="uint4", fast_decoding=False, group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized"),
-    dict(M=2, N=1024, K=2048, W_dtype="uint4", A_dtype="bfloat16", out_dtype="bfloat16", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized"),
-    dict(M=1, N=1024, K=2048, W_dtype="uint4", A_dtype="bfloat16", out_dtype="bfloat16", fast_decoding=True, group_size=128, with_scaling=True),
-    dict(M=1, N=1024, K=2048, W_dtype="uint4", out_dtype="float32", accum_dtype="float32", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized"),
-]
-
-
-@pytest.mark.parametrize("kw", STREAMK_CASES, ids=lambda k: "-".join(f"{a}{b}" for a, b in k.items()))
-def test_gemv_streamk_parity(kw):
-    """the stream-K kernel is opt-in (never auto-dispatched): pinned here through bb_set_kernel_override."""
-    import ctypes
-    from bitblas_b200 import _lib
-    kw = dict(kw)
-    case = H.make_case(kw.pop("M"), kw.pop("N"), kw.pop("K"), **kw)
-    lib = _lib.load()
-    prev = lib.bb_set_kernel_override(_lib.BB_KERNEL_GEMV_STREAMK)
-    try:
-        op = H.product_operator(case)
-        assert op.kernel_for(case["M"]) == "gemv_streamk"
-        assert op.lib._c.bb_workspace_bytes(ctypes.byref(op._desc), case["M"]) > 0
-        got = H.run_product(op, case)
-        # same workspace again (flags were reset by the owning warps), bit-identical: the summation order is fixed
-        got2 = H.run_product(op, case)
-    finally:
-        lib.bb_set_kernel_override(prev)
-    ref = H.oracle_output(case, fast_decoding=bool(op.fast_decoding))
-    H.assert_fp_close(got, ref, "gemv_streamk", max_mismatched_ratio=2e-3 if case["cfg"]["out_dtype"] == "bfloat16" else 0.0)
-    assert torch.equal(got, got2)
-    # and against the default streaming kernel on the same inputs (both accumulate in fp32; different summation order)
-    plain = H.run_product(op, case)
-    assert op.kernel_for(case["M"]) in ("gemv_mma", "gemv_slab")
-    assert H.O.rel_fro_error(got, plain) <= 2e-3
-
-
-def test_gemv_streamk_graph_replay_and_errors():
-    """CUDA-graph replay (the per-call nonce is frozen in the graph; flags are reset after use so every replay must still be
-    correct) and the loud failure without a workspace."""
-    import ctypes
-    from bitblas_b200 import _lib
-    case = H.make_case(1, 2048, 4096, W_dtype="uint4", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized")
-    op = H.product_operator(case)
-    lib = _lib.load()
-    dev = "cuda"
-    A = case["A"].to(dev)
-    Wd = H.product_weight(op, case, dev)
-    sc, zr = case["scale"].to(dev), case["zeros"].to(dev)
-    ref = H.oracle_output(case, fast_decoding=bool(op.fast_decoding))
-    prev = lib.bb_set_kernel_override(_lib.BB_KERNEL_GEMV_STREAMK)
-    try:
-        got = H.run_product(op, case)
-        H.assert_fp_close(got, ref, "streamk")
-        out = torch.empty(1, 2048, dtype=torch.float16, device=dev)
-        rc = op.lib._c.bb_matmul(ctypes.byref(op._desc), A.data_ptr(), Wd.data_ptr(), 0, sc.data_ptr(), zr.data_ptr(), 0,
-                                 out.data_ptr(), 1, 0, 0, torch.cuda.current_stream().cuda_stream)
-        assert rc != 0 and "workspace" in _lib.last_error()
-        s = torch.cuda.Stream()
-        with torch.cuda.stream(s):
-            op.forward(A, Wd, scale=sc, zeros=zr, output=out)   # warm-up outside capture (occupancy query, attributes)
-            s.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=s):
-                op.forward(A, Wd, scale=sc, zeros=zr, output=out)
-            for _ in range(3):
-                out.zero_()
-                g.replay()
-                s.synchronize()
-                assert torch.equal(out.cpu(), got.reshape(1, -1)), "graph replay differs"
-    finally:
-        lib.bb_set_kernel_override(prev)
-
-
 def test_gemv_pdl_dependent_chain():
     """Programmatic dependent launch: kernel i+1 starts (and prefetches weights) before kernel i has finished, and must
     still see kernel i's output as its activations and never overwrite a buffer kernel i is still reading.  A chain

@@ -1,5 +1,5 @@
-"""A/B timing of the m<=8 streaming kernels over a few (N, K): run once per env setting (BB_GEMV_TMA=0/1,
-BB_GEMV_TMA_MINB=2/3).  Cold-L2 by rotating over weight copies that exceed L2; back-to-back launches."""
+"""Timing of the m<=8 streaming kernels over a few (N, K) (AB_SHAPES=NxK,..., AB_M=1,2,...): cold L2 by rotating over weight
+copies that exceed L2; back-to-back launches."""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bitblas_b200 as bb
@@ -8,9 +8,6 @@ shapes = [(12288, 12288), (9472, 12288), (14208, 12288), (8192, 8192), (28672, 8
 if os.environ.get("AB_SHAPES"):
     shapes = [tuple(int(v) for v in t.split("x")) for t in os.environ["AB_SHAPES"].split(",")]
 reps_env = int(os.environ.get("AB_REPS", "60"))
-from bitblas_b200 import _lib
-if os.environ.get("AB_KERNEL"):
-    _lib.load().bb_set_kernel_override(int(os.environ["AB_KERNEL"]))
 ms = [int(x) for x in os.environ.get("AB_M", "1").split(",")]
 for (N, K) in shapes:
     for m in ms:
@@ -32,5 +29,5 @@ for (N, K) in shapes:
         e.record(); torch.cuda.synchronize()
         us = s.elapsed_time(e) / reps * 1000
         byt = N * K / 2 + N * (K // 128) * 2.5 + m * K * 2 + m * N * 2
-        print(f"N={N} K={K} m={m} {us:.1f} us  {byt / us / 1e3:.0f} GB/s  kernel={op.kernel_for(m)} depth={os.environ.get('BB_SK_DEPTH','-')}", flush=True)
+        print(f"N={N} K={K} m={m} {us:.1f} us  {byt / us / 1e3:.0f} GB/s  kernel={op.kernel_for(m)}", flush=True)
         del Ws

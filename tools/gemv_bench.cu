@@ -1,8 +1,8 @@
 // tools/gemv_bench.cu -- m = 1 W4A16 GEMV through the C ABI (bb_matmul): full-output check against a double-precision CPU
-// dequantise+dot, then back-to-back timing over rotating weight copies (cold L2), for a list of shapes and tuning knobs.
+// dequantise+dot, then back-to-back timing over rotating weight copies (cold L2), for a list of shapes.
 //   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/gemv_bench tools/gemv_bench.cu \
 //        -Lbitblas_b200/lib -lbitblas_b200 -Xlinker -rpath -Xlinker '$ORIGIN/../bitblas_b200/lib'
-//   tools/gemv_bench [--kernel ID] [--iters N] [--cfg STAGES,GROUPS[,FINISHERS]]... [--tile] [--nocheck] NxK [NxK ...]
+//   tools/gemv_bench [--kernel ID] [--iters N] [--tile] [--nocheck] NxK [NxK ...]
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
@@ -20,24 +20,19 @@
 #define CK(x) do { cudaError_t e = (x); if (e != cudaSuccess) { printf("CUDA error %s at line %d\n", cudaGetErrorString(e), __LINE__); exit(1);} } while (0)
 #define BB(x) do { int rc = (x); if (rc) { printf("bb error %d at line %d: %s\n", rc, __LINE__, bb_last_error()); exit(1);} } while (0)
 
-struct Cfg { int stages, ng, nf; };
-
 int main(int argc, char** argv) {
   int kernel = BB_KERNEL_AUTO, iters = 200;
   bool check = true, tile = false;   // --tile: BB_TILE_SLAB weight storage (MatmulConfig.propagate_b)
-  std::vector<Cfg> cfgs;
   std::vector<std::pair<int, int>> shapes;
   for (int i = 1; i < argc; ++i) {
     std::string a = argv[i];
     if (a == "--kernel") kernel = atoi(argv[++i]);
     else if (a == "--iters") iters = atoi(argv[++i]);
     else if (a == "--nocheck") check = false;
-    else if (a == "--cfg") { Cfg c{4, 2, 1}; sscanf(argv[++i], "%d,%d,%d", &c.stages, &c.ng, &c.nf); cfgs.push_back(c); }
     else if (a == "--tile") tile = true;
     else { int n, k; if (sscanf(a.c_str(), "%dx%d", &n, &k) == 2) shapes.push_back({n, k}); }
   }
   if (shapes.empty()) shapes.push_back({12288, 12288});
-  if (cfgs.empty()) cfgs.push_back(Cfg{4, 2, 1});
   BB(bb_init(0));
   bb_set_kernel_override(kernel);
   cudaStream_t st; CK(cudaStreamCreate(&st));
@@ -106,45 +101,39 @@ int main(int argc, char** argv) {
         ref[n] = acc;
       }
     }
-    for (const Cfg& c : cfgs) {
-      char buf[32];
-      snprintf(buf, 32, "%d", c.stages); setenv("BB_GS_STAGES", buf, 1);
-      snprintf(buf, 32, "%d", c.ng); setenv("BB_GS_NG", buf, 1);
-      snprintf(buf, 32, "%d", c.nf); setenv("BB_GS_NF", buf, 1);
-      double maxerr = -1, maxref = 0;
-      if (check) {
-        CK(cudaMemset(dC, 0xff, N * 2));
-        BB(bb_matmul(&d, dA, dW[0], nullptr, dS, dZ, nullptr, dC, 1, ws, wsb, st));
-        CK(cudaStreamSynchronize(st));
-        std::vector<__half> hC(N);
-        CK(cudaMemcpy(hC.data(), dC, N * 2, cudaMemcpyDeviceToHost));
-        maxerr = 0;
-        int bad = -1;
-        for (int n = 0; n < N; ++n) {
-          const double e = fabs(double(__half2float(hC[n])) - ref[n]);
-          if (!(e <= maxerr)) { maxerr = e; bad = n; }
-          maxref = std::max(maxref, fabs(ref[n]));
-        }
-        if (!(maxerr <= 0.02 * maxref)) printf("  MISMATCH at n=%d: got %f ref %f\n", bad, __half2float(hC[bad]), ref[bad]);
-      }
-      for (int i = 0; i < 10; ++i) BB(bb_matmul(&d, dA, dW[i % copies], nullptr, dS, dZ, nullptr, dC, 1, ws, wsb, st));
+    double maxerr = -1, maxref = 0;
+    if (check) {
+      CK(cudaMemset(dC, 0xff, N * 2));
+      BB(bb_matmul(&d, dA, dW[0], nullptr, dS, dZ, nullptr, dC, 1, ws, wsb, st));
       CK(cudaStreamSynchronize(st));
-      float best = 1e30f, sum = 0;
-      const int reps = 3;
-      for (int r = 0; r < reps; ++r) {
-        CK(cudaEventRecord(e0, st));
-        for (int i = 0; i < iters; ++i) BB(bb_matmul(&d, dA, dW[i % copies], nullptr, dS, dZ, nullptr, dC, 1, ws, wsb, st));
-        CK(cudaEventRecord(e1, st));
-        CK(cudaEventSynchronize(e1));
-        float ms; cudaEventElapsedTime(&ms, e0, e1);
-        best = std::min(best, ms / iters); sum += ms / iters;
+      std::vector<__half> hC(N);
+      CK(cudaMemcpy(hC.data(), dC, N * 2, cudaMemcpyDeviceToHost));
+      maxerr = 0;
+      int bad = -1;
+      for (int n = 0; n < N; ++n) {
+        const double e = fabs(double(__half2float(hC[n])) - ref[n]);
+        if (!(e <= maxerr)) { maxerr = e; bad = n; }
+        maxref = std::max(maxref, fabs(ref[n]));
       }
-      const double us_best = best * 1e3, us_mean = sum / reps * 1e3;
-      printf("N=%d K=%d kernel=%s%s stages=%d groups=%d finishers=%d : %.2f us best %.2f us mean  %.0f GB/s  frac(6576)=%.3f  maxerr=%.3g (max|ref|=%.3g)\n",
-             N, K, bb_kernel_name(kid), tile ? " (slab-tiled W)" : "", c.stages, c.ng, c.nf, us_best, us_mean, alg / (us_mean * 1e-6) / 1e9,
-             alg / (us_mean * 1e-6) / 1e9 / 6576.1, maxerr, maxref);
-      fflush(stdout);
+      if (!(maxerr <= 0.02 * maxref)) printf("  MISMATCH at n=%d: got %f ref %f\n", bad, __half2float(hC[bad]), ref[bad]);
     }
+    for (int i = 0; i < 10; ++i) BB(bb_matmul(&d, dA, dW[i % copies], nullptr, dS, dZ, nullptr, dC, 1, ws, wsb, st));
+    CK(cudaStreamSynchronize(st));
+    float best = 1e30f, sum = 0;
+    const int reps = 3;
+    for (int r = 0; r < reps; ++r) {
+      CK(cudaEventRecord(e0, st));
+      for (int i = 0; i < iters; ++i) BB(bb_matmul(&d, dA, dW[i % copies], nullptr, dS, dZ, nullptr, dC, 1, ws, wsb, st));
+      CK(cudaEventRecord(e1, st));
+      CK(cudaEventSynchronize(e1));
+      float ms; cudaEventElapsedTime(&ms, e0, e1);
+      best = std::min(best, ms / iters); sum += ms / iters;
+    }
+    const double us_best = best * 1e3, us_mean = sum / reps * 1e3;
+    printf("N=%d K=%d kernel=%s%s : %.2f us best %.2f us mean  %.0f GB/s  frac(6576)=%.3f  maxerr=%.3g (max|ref|=%.3g)\n",
+           N, K, bb_kernel_name(kid), tile ? " (slab-tiled W)" : "", us_best, us_mean, alg / (us_mean * 1e-6) / 1e9,
+           alg / (us_mean * 1e-6) / 1e9 / 6576.1, maxerr, maxref);
+    fflush(stdout);
     for (auto p : dW) cudaFree(p);
     cudaFree(dS); cudaFree(dA); cudaFree(dZ); cudaFree(dC); cudaFree(ws);
   }

@@ -1,7 +1,8 @@
 // tools/slabbench.cu -- round-2 hypothesis test for the m = 1 weight stream (DESIGN.md 3.2): does the DRAM side care about the
 // granularity / pacing of the per-row requests?  Pure TMA loads of the N x (K/2)-byte packed-weight matrix, no arithmetic, with an
 // optional spin of `delay` cycles after every consumed tile to emulate compute pacing.
-//   box   : every warp streams its own 16-row block with [16 rows x 128 B] boxes (2 KB), DEPTH boxes in flight   (= gemv_sk_kernel)
+//   box   : every warp streams its own contiguous range of 16-row blocks with [16 rows x 128 B] boxes (2 KB, 128B-swizzled), DEPTH
+//           boxes in flight per warp
 //   slab  : every CTA streams 16-row blocks with [16 rows x SLAB B] boxes (uint32 tensor map, SLAB = 512 / 1024), DEPTH slabs in
 //           flight, the 8 warps of the CTA each "consume" a 128 B K-slice of the slab
 // Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/slabbench tools/slabbench.cu -lcuda
@@ -34,7 +35,7 @@ __device__ __forceinline__ void spin(int cycles) {
   while (clock64() - t0 < cycles) {}
 }
 
-// ---- per-warp 2 KB boxes (the stream-K kernel's pattern) ----
+// ---- per-warp 2 KB boxes, each warp its own TMA producer ----
 template <int DEPTH>
 __global__ void __launch_bounds__(256, 2) k_box(const __grid_constant__ CUtensorMap tm, int row_blocks, int chunks_per_row, int delay, unsigned* out) {
   extern __shared__ uint8_t raw[];
