@@ -21,7 +21,7 @@ def set_log_level(level):
 
 from .ops.operator import OperatorConfig, Operator, TransformKind, OptimizeStrategy  # noqa: E402,F401
 from .ops.general_matmul import Matmul, MatmulConfig  # noqa: E402,F401
-from .module import Linear  # noqa: E402,F401
+from .module import Linear, GroupedLinear  # noqa: E402,F401
 from .utils import auto_detect_nvidia_target  # noqa: E402,F401
 from . import cache, quantization, testing  # noqa: E402,F401
 from .parallel import ColumnParallelLinear  # noqa: E402,F401

@@ -84,6 +84,10 @@ int launch_gemv_i8(const MatmulArgs& a);
 bool gemm_ts_supported(const bb_matmul_desc& d, int m);
 int launch_gemm_ts(const MatmulArgs& a);
 size_t gemm_ts_workspace_bytes(const bb_matmul_desc& d, int m);
+// grouped (mixture-of-experts) matmul, bb_grouped.cu: grouped_supported sets the error message when it returns false
+bool grouped_supported(const bb_matmul_desc& d);
+int launch_grouped(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                   const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream);
 
 // bit position of logical element `o` (0 .. 32/bits-1) inside its 32-bit storage word, for each weight
 // layout (restates bitblas/quantization/utils.py:73-110 + testing/cpp/lop3_type_conversion/fast_decoding.hpp:30-95,607-668)

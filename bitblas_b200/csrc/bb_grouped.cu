@@ -1,0 +1,242 @@
+// bb_grouped.cu -- grouped low-bit matmul for mixture-of-experts layers (bb_matmul_grouped): ONE launch over E experts,
+//   C[offsets[e] : offsets[e+1]] = A[offsets[e] : offsets[e+1]] x dequant(W[e])^T (+ bias[e])     for every e,
+// with the row offsets read on the device.
+//
+// Design:
+//   * the per-expert arithmetic is the decode GEMV's (gemv_mma_tile, bb_gemv_mma.cuh): LOP3 decode into mma.sync fragments,
+//     per-group scale / zero corrections, K split over the warps of a CTA and reduced in shared memory.  Numerics are those of
+//     bb_matmul for the same descriptor.
+//   * the grid is persistent and sized to what is resident on the device (an upper bound of the work, capped at one wave), not to
+//     E: with 128 experts of which 8 are active, no CTA is spent on an empty expert.  Every CTA stages the (clamped) offsets in
+//     shared memory, derives each group's count of work items -- (16-row block of W, chunk of 8 * NT rows of A) -- with one
+//     warp-wide prefix sum, and walks the items blockIdx.x, blockIdx.x + gridDim.x, ...  An item's expert is found by binary
+//     search over the prefix sums; items run expert by expert, row chunk by row chunk, row block by row block.
+//   * rows per pass (NT batch tiles of 8) are chosen on the host from the mean rows per active expert.  A group with more
+//     rows than 8 * NT is served by several passes over its weights (the later passes mostly hit L2).
+//   * programmatic dependent launch: the offsets and the sorted activations are written by the routing kernels right before
+//     this one, and which experts' weights to stream is not known before the offsets are.  So griddepcontrol.wait is the first
+//     instruction; unlike the single-matrix GEMV no weight is prefetched before it.  launch_dependents follows the CTA's last item.
+//   * the offsets are untrusted: each is clamped to [0, T] and a group whose end is below its start is empty, so a malformed
+//     table never reads or writes outside A[0:T] / C[0:T]; rows that no group claims are not written.
+#include <algorithm>
+#include <climits>
+
+#include "bb_gemv_mma.cuh"
+
+namespace bb {
+
+namespace {
+
+struct GroupedParams {
+  GemvParams p;               // the problem of group 0 (p.M unused; p.out: C with row stride N)
+  const int32_t* offsets;     // [E + 1], device
+  int E;                      // groups
+  int T;                      // rows of A and C
+  long long w_stride;         // bytes per group: W, scale, zeros, bias
+  long long s_stride, z_stride, b_stride;
+  int out_bytes;              // bytes per element of C
+};
+
+template <typename T, int BITS, bool IL, int NT, int ZK, bool SC>
+__global__ void __launch_bounds__(NT == 1 ? 128 : MAX_KS * 32) __maxnreg__(gemv_mma_maxnreg(NT, ZK))
+gemv_grouped_kernel(const GroupedParams g) {
+  constexpr int R = 8 * NT;   // rows of A per pass over a 16-row block of W
+  __shared__ float red[MAX_KS][16][8 * NT];
+  __shared__ int row0_s[BB_GROUPED_MAX_GROUPS];       // clamped first row of each group
+  __shared__ int rows_s[BB_GROUPED_MAX_GROUPS];       // rows of each group (0: empty)
+  __shared__ int item0_s[BB_GROUPED_MAX_GROUPS + 1];  // first work item of each group; item0_s[E] = all items
+
+  pdl_wait();   // offsets and A are the preceding kernels' output; nothing is read before this (see the header)
+  const int nb = g.p.N / 16;
+  if (threadIdx.x < 32) {
+    const int lane = threadIdx.x;
+    const int per = (g.E + 31) / 32;   // consecutive groups per lane
+    const int e0 = lane * per;
+    int cnt = 0;
+    for (int i = 0; i < per; ++i) {
+      const int e = e0 + i;
+      if (e < g.E) {
+        const int b = min(max(g.offsets[e], 0), g.T);
+        const int m = max(min(max(g.offsets[e + 1], 0), g.T) - b, 0);
+        row0_s[e] = b;
+        rows_s[e] = m;
+        cnt += nb * ((m + R - 1) / R);
+      }
+    }
+    int incl = cnt;   // inclusive prefix sum over the lanes
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= d) incl += v;
+    }
+    int run = incl - cnt;
+    for (int i = 0; i < per; ++i) {
+      const int e = e0 + i;
+      if (e < g.E) {
+        item0_s[e] = run;
+        run += nb * ((rows_s[e] + R - 1) / R);
+      }
+    }
+    if (lane == 31) item0_s[g.E] = incl;
+  }
+  __syncthreads();
+  const int total = item0_s[g.E];
+
+  for (int item = blockIdx.x; item < total; item += gridDim.x) {
+    // the group of this item: the last e with item0_s[e] <= item (an empty group shares its start with the next one)
+    int lo = 0, hi = g.E - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (item0_s[mid] <= item) lo = mid; else hi = mid - 1;
+    }
+    const int e = lo;
+    const int local = item - item0_s[e];
+    const int chunk = local / nb, rb = local - chunk * nb;
+    const int r0 = row0_s[e] + chunk * R;
+    GemvParams p = g.p;
+    p.out.n = 1;   // one destination: the epilogue's loop over out.ptr then indexes it statically
+    p.M = min(R, rows_s[e] - chunk * R);
+    p.A = reinterpret_cast<const T*>(g.p.A) + size_t(r0) * p.K;
+    p.W = g.p.W + size_t(e) * size_t(g.w_stride);
+    if (SC) p.scale = reinterpret_cast<const uint8_t*>(g.p.scale) + size_t(e) * size_t(g.s_stride);
+    if (ZK) p.zeros = reinterpret_cast<const uint8_t*>(g.p.zeros) + size_t(e) * size_t(g.z_stride);
+    if (g.p.bias) p.bias = reinterpret_cast<const uint8_t*>(g.p.bias) + size_t(e) * size_t(g.b_stride);
+    p.out.ptr[0] = reinterpret_cast<uint8_t*>(g.p.out.ptr[0]) + size_t(r0) * size_t(p.N) * size_t(g.out_bytes);
+    if (item != int(blockIdx.x)) __syncthreads();   // the previous item's epilogue has finished reading `red`
+    gemv_mma_tile<T, BITS, IL, NT, ZK, SC, false>(p, rb, red);
+  }
+  pdl_launch_dependents();
+}
+
+// CTAs of ks warps resident on the device; occ_cache (one per instance) holds the per-SM count, -1 until queried
+template <typename KernelT>
+int resident_ctas(KernelT kernel, int (&occ_cache)[MAX_KS + 1], int ks) {
+  if (occ_cache[ks] < 0) {
+    int occ = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, ks * 32, 0) != cudaSuccess) { cudaGetLastError(); occ = 0; }
+    occ_cache[ks] = occ;
+  }
+  return occ_cache[ks] * device_sm_count();
+}
+
+// K splits (warps per CTA): the largest count for which an upper bound of the work items fits in one resident wave, as the
+// decode GEMV chooses it; the grid is that bound, capped at the resident CTAs.
+template <typename KernelT>
+int launch_grouped_kernel(KernelT kernel, int (&occ_cache)[MAX_KS + 1], GroupedParams g, int max_items, int max_ks,
+                          cudaStream_t stream) {
+  const int steps = g.p.K / 128;
+  int ks = std::max(1, std::min(max_ks, steps));
+  for (int k = ks; k >= 2; --k) {
+    if (max_items <= resident_ctas(kernel, occ_cache, k)) { ks = k; break; }
+  }
+  g.p.ks = ks;
+  const int resident = resident_ctas(kernel, occ_cache, ks);
+  if (resident <= 0) { set_error("grouped matmul: the kernel cannot be resident on this device"); return 2; }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(std::min(max_items, resident));
+  cfg.blockDim = dim3(ks * 32);
+  cfg.dynamicSmemBytes = 0;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, g));
+  BB_LAUNCH_CHECK();
+  return 0;
+}
+
+template <typename T, int BITS, bool IL>
+int launch_grouped_nt(const GroupedParams& g, int nt, const int (&max_items)[3], cudaStream_t s) {
+#define BB_GROUPED_GO(NTV, ZKV, SCV, MAXKS)                                                                   \
+  {                                                                                                          \
+    static int occ_cache[MAX_KS + 1] = {-1, -1, -1, -1, -1, -1, -1, -1, -1};                                 \
+    return launch_grouped_kernel(gemv_grouped_kernel<T, BITS, IL, NTV, ZKV, SCV>, occ_cache, g,             \
+                                 max_items[NTV == 1 ? 0 : (NTV == 2 ? 1 : 2)], MAXKS, s);                    \
+  }
+#define BB_GROUPED_NT(ZKV, SCV)                     \
+  if (nt == 1) BB_GROUPED_GO(1, ZKV, SCV, 4)        \
+  if (nt == 2) BB_GROUPED_GO(2, ZKV, SCV, MAX_KS)   \
+  BB_GROUPED_GO(4, ZKV, SCV, MAX_KS)
+  if (!g.p.with_scaling) { BB_GROUPED_NT(0, false) }
+  if (g.p.zmode == 0) { BB_GROUPED_NT(0, true) }
+  if (g.p.zmode == 1) { BB_GROUPED_NT(1, true) }
+  if (g.p.zmode == 2) { BB_GROUPED_NT(2, true) }
+  BB_GROUPED_NT(3, true)
+#undef BB_GROUPED_NT
+#undef BB_GROUPED_GO
+}
+
+size_t elem_bytes(int dtype) { return dtype == BB_F32 ? 4 : 2; }
+
+}  // namespace
+
+// the configurations the grouped kernel covers (those of gemv_mma, for any m); sets the error message otherwise
+bool grouped_supported(const bb_matmul_desc& d) {
+  if (d.a_dtype != BB_F16 && d.a_dtype != BB_BF16) { set_error("grouped matmul: activations must be float16 or bfloat16"); return false; }
+  if ((d.w_fmt != BB_W_UINT && d.w_fmt != BB_W_INT) || (d.w_bits != 4 && d.w_bits != 2)) {
+    set_error("grouped matmul: weights must be 4- or 2-bit uint / int (w_fmt=%d w_bits=%d)", d.w_fmt, d.w_bits);
+    return false;
+  }
+  if (d.w_tile != BB_TILE_ROW_MAJOR) { set_error("grouped matmul: slab-tiled weights are not supported (row-major storage only)"); return false; }
+  if (d.w_layout == BB_LAYOUT_INTERLEAVED_8) { set_error("grouped matmul: the int8-target interleave is not supported"); return false; }
+  if (d.N % 16 || d.K % 128) { set_error("grouped matmul: needs N %% 16 == 0 and K %% 128 == 0 (N=%d K=%d)", d.N, d.K); return false; }
+  const int g = d.group_size <= 0 ? d.K : d.group_size;
+  if (g % 128) { set_error("grouped matmul: group_size must be a multiple of 128 or -1 (got %d)", d.group_size); return false; }
+  if (!gemv_mma_supported(d, 1)) {
+    set_error("grouped matmul: unsupported scale / zeros / out_dtype combination (zeros need scaling, int weights take no "
+              "zeros, out_dtype float16 | bfloat16 | float32, quantized zeros need N*bits %% 8 == 0)");
+    return false;
+  }
+  return true;
+}
+
+int launch_grouped(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                   const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream) {
+  MatmulArgs a = {};
+  a.d = d; a.A = A; a.W = W; a.scale = scale; a.zeros = zeros; a.bias = bias; a.C = C; a.m = total_rows; a.n_peers = 0;
+  GroupedParams g;
+  GemvParams& p = g.p;
+  p.A = A; p.W = reinterpret_cast<const uint8_t*>(W);
+  p.scale = d.with_scaling ? scale : nullptr;
+  p.zeros = d.with_zeros ? zeros : nullptr;
+  p.bias = d.with_bias ? bias : nullptr;
+  p.out = make_outspec(a);
+  p.M = 0; p.N = d.N; p.K = d.K;
+  p.g = a.gsize(); p.G = a.groups();
+  p.with_scaling = d.with_scaling;
+  p.zmode = d.with_zeros ? (d.zeros_mode + 1) : 0;
+  p.zp_const = (d.w_fmt == BB_W_INT) ? (1 << (d.w_bits - 1)) : 0;
+  p.out_dtype = d.out_dtype;
+  p.ks = 1;
+  const long long N = d.N, G = p.G;
+  g.offsets = offsets; g.E = num_groups; g.T = total_rows;
+  g.w_stride = N * d.K * d.w_bits / 8;
+  g.s_stride = N * G * 2;
+  g.z_stride = d.zeros_mode == BB_ZEROS_QUANTIZED ? G * (N * d.w_bits / 8) : N * G * 2;
+  g.b_stride = N * 2;
+  g.out_bytes = int(elem_bytes(d.out_dtype));
+  // rows per pass: 8, 16 or 32, from the mean rows per active group (T rows over at most min(E, T) groups)
+  const int active = std::min(num_groups, total_rows);
+  const int mean_rows = (total_rows + active - 1) / active;
+  const int nt = mean_rows <= 8 ? 1 : (mean_rows <= 16 ? 2 : 4);
+  // work items: sum_e ceil(m_e / R) row chunks per 16-row block <= T / R + (groups with rows)
+  const long long nb = d.N / 16;
+  int max_items[3];
+  const int R[3] = {8, 16, 32};
+  for (int i = 0; i < 3; ++i) {
+    const long long items = nb * (total_rows / R[i] + active);
+    if (items > INT_MAX) { set_error("grouped matmul: N/16 x (T/rows + groups) exceeds 2^31 work items"); return 1; }
+    max_items[i] = int(items);
+  }
+  const bool il = d.w_layout == BB_LAYOUT_INTERLEAVED_16;
+  if (d.a_dtype == BB_F16) {
+    if (d.w_bits == 4) return il ? launch_grouped_nt<__half, 4, true>(g, nt, max_items, stream) : launch_grouped_nt<__half, 4, false>(g, nt, max_items, stream);
+    return il ? launch_grouped_nt<__half, 2, true>(g, nt, max_items, stream) : launch_grouped_nt<__half, 2, false>(g, nt, max_items, stream);
+  }
+  if (d.w_bits == 4) return il ? launch_grouped_nt<__nv_bfloat16, 4, true>(g, nt, max_items, stream) : launch_grouped_nt<__nv_bfloat16, 4, false>(g, nt, max_items, stream);
+  return il ? launch_grouped_nt<__nv_bfloat16, 2, true>(g, nt, max_items, stream) : launch_grouped_nt<__nv_bfloat16, 2, false>(g, nt, max_items, stream);
+}
+
+}  // namespace bb

@@ -235,4 +235,81 @@ class Linear(nn.Module):
         return self.is_consitent
 
 
-__all__ = ["Linear", "unpack_qzeros", "unpack_qzeros_v2", "unpack_qweight"]
+class GroupedLinear(nn.Module):
+    """E quantized linear layers of one shape -- the experts of a mixture-of-experts projection -- run as one grouped matmul
+    (``Matmul.forward_grouped``).  Constructor arguments after ``num_groups`` are those of ``Linear``; the buffers are
+    ``Linear``'s stacked over the experts: ``qweight`` [E, N, K*bits/8], ``scales`` [E, N, K/g], ``zeros`` [E, N, K/g] (or
+    [E, K/g, N*bits/8] for ``zeros_mode="quantized"``) and ``bias`` [E, N].  ``forward(A, offsets)`` takes the activations sorted
+    by expert and the int32 device row offsets [E + 1]; routing, top-k weighting and combining stay with the caller."""
+
+    def __init__(self, num_groups: int, in_features: int, out_features: int, bias: bool = False, **linear_kwargs):
+        super().__init__()
+        num_groups = int(num_groups)
+        if not 1 <= num_groups <= _lib.BB_GROUPED_MAX_GROUPS:
+            raise ValueError(f"num_groups must be in [1, {_lib.BB_GROUPED_MAX_GROUPS}] (got {num_groups})")
+        # one Linear describes an expert (config, operator, per-expert buffer shapes); it owns no storage used here
+        expert = Linear(in_features, out_features, bias=bias, **linear_kwargs)
+        op = expert.bitblas_matmul
+        if expert.consistent:
+            raise ValueError("GroupedLinear needs a low-bit weight format (A_dtype != W_dtype)")
+        op.check_grouped(num_groups)
+        self.num_groups, self.in_features, self.out_features = num_groups, in_features, out_features
+        self.bitblas_matmul, self.bits, self.group_size = op, expert.bits, expert.group_size
+        self.torch_dtype = expert.torch_dtype
+        self._expert_attrs = {k: getattr(expert, k) for k in ("in_features", "out_features", "group_size", "bits",
+                                                              "torch_dtype", "bitblas_matmul")}
+        for name, shape, dtype in expert._buffer_specs(bias):
+            self.register_buffer(name, torch.zeros((num_groups, *shape), dtype=dtype))
+        if not bias:
+            self.bias = None
+
+    def forward(self, A, offsets, output=None):
+        op = self.bitblas_matmul
+        cfg = op.config
+        return op.forward_grouped(A, self.qweight, offsets, scale=self.scales if cfg.with_scaling else None,
+                                  zeros=self.zeros if cfg.with_zeros else None, bias=self.bias, output=output)
+
+    def load_and_transform_weight(self, weight: torch.Tensor, scales: torch.Tensor = None, zeros: torch.Tensor = None,
+                                  bias: torch.Tensor = None):
+        """weight [E, N, K] of unsigned field values (signed for "int" formats), as Linear.load_and_transform_weight takes
+        per expert; the storage transform works row by row, so the stacked tensor is transformed in one call."""
+        if weight.dim() != 3 or weight.shape[0] != self.num_groups:
+            raise ValueError(f"weight must be [E={self.num_groups}, N, K], got {tuple(weight.shape)}")
+        self.qweight = self.bitblas_matmul.transform_weight(weight)
+        if scales is not None:
+            self.scales = scales
+        if zeros is not None:
+            self.zeros = zeros
+        if bias is not None:
+            self.bias = bias
+
+    def _repack(self, gptq_modules, device, v2: bool):
+        """Linear's device repack (bb_repack_gptq_*_device) per expert, copied into the expert's slice of the stacked buffers."""
+        from types import SimpleNamespace
+        if len(gptq_modules) != self.num_groups:
+            raise ValueError(f"expected {self.num_groups} GPTQ modules, got {len(gptq_modules)}")
+        dev = torch.device(device)
+        if dev.type != "cuda":
+            raise RuntimeError("repack_from_gptq needs a CUDA device: bitblas_b200 has no CPU path")
+        for name in ("qweight", "scales", "zeros", "bias"):
+            t = getattr(self, name)
+            if t is not None and t.device != dev:
+                setattr(self, name, t.to(dev))
+        for e, gm in enumerate(gptq_modules):
+            one = SimpleNamespace(**self._expert_attrs, bias=None if self.bias is None else self.bias[e])
+            Linear._repack(one, gm, dev, v2)
+            self.qweight[e].copy_(one.qweight)
+            self.scales[e].copy_(one.scales)
+            self.zeros[e].copy_(one.zeros)
+            if self.bias is not None:
+                self.bias[e].copy_(one.bias)
+
+    def repack_from_gptq(self, gptq_modules, device="cuda"):
+        """one GPTQ QuantLinear per expert (how GPTQ mixture-of-experts checkpoints store them)"""
+        self._repack(gptq_modules, device, v2=False)
+
+    def repack_from_gptq_v2(self, gptq_modules, device="cuda"):
+        self._repack(gptq_modules, device, v2=True)
+
+
+__all__ = ["Linear", "GroupedLinear", "unpack_qzeros", "unpack_qzeros_v2", "unpack_qweight"]

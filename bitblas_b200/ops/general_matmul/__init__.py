@@ -25,6 +25,14 @@ logger = logging.getLogger(__name__)
 
 WORKSPACE_SIZE = 1024 * 1024 * 256
 
+# Matmul.forward_grouped runs the single grouped launch while T <= GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E rows (E groups);
+# above it each non-empty group runs through bb_matmul, whose dispatcher picks the wgmma GEMM above 8 rows.  tools/moe_bench.py
+# (NVIDIA H100 80GB HBM3, 700 W power limit): with 8 large experts (Mixtral-8x7B down, 4096 x 14336) the single launch is 1.6-2.7x
+# faster up to 8 rows per expert, even at 16 and slower above (0.60x at 32); the fused gate/up (28672 x 4096) is already 0.67x
+# at 16 rows per expert.  With 128 small experts (Qwen3-30B-A3B gate/up) the single launch stays ahead up to ~128 rows per
+# expert because the per-group side issues one call per expert; the constant follows the large-expert crossover.
+GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP = 8
+
 NATIVE_COMPUTE_PATTERNS = [  # general_matmul/__init__.py:33-47
     ("float64", "float64"), ("float32", "float32"), ("float16", "float16"), ("bfloat16", "bfloat16"),
     ("int8", "int8"), ("uint8", "uint8"), ("int4", "int4"), ("uint4", "uint4"),
@@ -265,6 +273,7 @@ class Matmul(Operator):
         self._ws = {}
         self._ws_need = {}
         self._checked_key = None
+        self._grouped_checked_key = None
         self._torch_a_dtype = getattr(torch, config.A_dtype, None)
         self._desc_ref = None
         self.weight_executors = None
@@ -503,6 +512,112 @@ class Matmul(Operator):
                                            arr, n, int(ldc), int(col_offset), int(m), *self._workspace_for(int(m), A.device), stream)
         if rc != 0:
             raise RuntimeError(f"bb_matmul_scatter failed (code {rc}): {_lib.last_error()}")
+
+    # ---- grouped (mixture-of-experts) forward -----------------------------------------------------------------------------
+    def check_grouped(self, num_groups: int) -> None:
+        """raise ValueError unless bb_matmul_grouped covers this operator's config with `num_groups` groups (validated by the
+        library with total_rows = 0: nothing touches the device)."""
+        if self.consistent:
+            raise ValueError("the grouped matmul needs a low-bit weight operator (A_dtype != W_dtype)")
+        rc = self.lib._c.bb_matmul_grouped(self._desc_ref, int(num_groups), 0, 0, 0, 0, 0, 0, 0, 0, 0)
+        if rc != 0:
+            raise ValueError(f"bb_matmul_grouped does not cover this configuration: {_lib.last_error()}")
+
+    def _check_grouped_params(self, E, W, scale, zeros, bias):
+        """stacked parameter tensors: W [E, N, K*bits/8], scale [E, N, K/g], zeros [E, N, K/g] ([E, K/g, N*bits/8] quantized),
+        bias [E, N].  Shapes and dtypes are checked before the device, so a CPU tensor of the wrong shape reports its shape."""
+        c = self.config
+        adt = self._torch_a_dtype
+        G = c.K // (c.group_size if c.group_size and c.group_size > 0 else c.K)
+        specs = [("W", W, torch.int8, (E, *self.retrieve_weight_shape()), True),
+                 ("scale", scale, adt, (E, c.N, G), c.with_scaling),
+                 ("zeros", zeros, torch.int8 if c.zeros_mode == "quantized" else adt,
+                  (E, G, c.N * self.bit // 8) if c.zeros_mode == "quantized" else (E, c.N, G), c.with_zeros),
+                 ("bias", bias, adt, (E, c.N), c.with_bias)]
+        specs = [s for s in specs if s[4]]
+        for name, t, dtype, shape, _ in specs:
+            if t is None:
+                raise ValueError(f"the operator's config needs {name}, got None")
+            if not isinstance(t, torch.Tensor):
+                raise TypeError(f"{name} must be a torch.Tensor")
+            if tuple(t.shape) != shape:
+                raise ValueError(f"{name} has shape {tuple(t.shape)}, expected the stacked shape {shape}")
+        for name, t, dtype, shape, _ in specs:
+            self._check_tensor(t, name, dtype)
+
+    def forward_grouped(self, A, W, offsets, scale=None, zeros=None, bias=None, output=None):
+        """Grouped matmul for mixture-of-experts layers (bb_matmul_grouped): E problems of this operator's config.  A [T, K] holds
+        every group's rows, sorted so that group e owns rows [offsets[e], offsets[e+1]); `offsets` is an int32 CUDA tensor of
+        E + 1 entries.  W, scale, zeros and bias are stacked over the groups (see _check_grouped_params).  For every group e:
+        output[offsets[e]:offsets[e+1]] = A[offsets[e]:offsets[e+1]] x dequant(W[e])^T (+ bias[e]).  Rows no group claims are not
+        written.
+
+        Up to GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E rows this is ONE kernel launch that reads the offsets on the device: no host
+        synchronisation, CUDA-graph capturable.  Above it (prefill) the offsets are copied to the host once and every non-empty
+        group runs through bb_matmul on its row slice, where the dispatcher picks the wgmma GEMM; that path synchronises with the
+        device and cannot be captured in a graph."""
+        if self.consistent:
+            raise NotImplementedError("forward_grouped needs a low-bit weight operator")
+        c = self.config
+        if not isinstance(offsets, torch.Tensor) or offsets.dtype != torch.int32:
+            raise TypeError("offsets must be an int32 torch.Tensor of num_groups + 1 row offsets")
+        if offsets.dim() != 1 or not 2 <= offsets.numel() <= _lib.BB_GROUPED_MAX_GROUPS + 1:
+            raise ValueError(f"offsets must be 1-D with num_groups + 1 entries, 1 <= num_groups <= {_lib.BB_GROUPED_MAX_GROUPS} "
+                             f"(got shape {tuple(offsets.shape)})")
+        E = offsets.numel() - 1
+        key = (E, W.data_ptr(), scale.data_ptr() if scale is not None else 0, zeros.data_ptr() if zeros is not None else 0,
+               bias.data_ptr() if bias is not None else 0)
+        if key != self._grouped_checked_key:
+            self._check_grouped_params(E, W, scale, zeros, bias)
+            self.check_grouped(E)
+            self._grouped_checked_key = key
+        if not isinstance(A, torch.Tensor) or A.dim() != 2 or A.shape[1] != c.K:
+            raise ValueError(f"A must be [T, K={c.K}], got {tuple(A.shape) if isinstance(A, torch.Tensor) else type(A)}")
+        T = A.shape[0]
+        if output is not None and (not isinstance(output, torch.Tensor) or tuple(output.shape) != (T, c.N)):
+            raise ValueError(f"output must be [T={T}, N={c.N}]")
+        self._check_tensor(A, "A", self._torch_a_dtype)
+        self._check_tensor(offsets, "offsets", torch.int32)
+        if offsets.device != A.device or W.device != A.device:
+            raise ValueError("A, W and offsets must be on the same device")
+        dev = A.device
+        if output is None:
+            output = torch.empty((T, c.N), dtype=self.torch_output_dtype, device=dev)
+        else:
+            self._check_tensor(output, "output", self.torch_output_dtype)
+        idx = dev.index if dev.index is not None else torch.cuda.current_device()
+        if idx not in _lib._inited:
+            _lib.ensure_init(idx)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        ptrs = key[1:]
+        with torch.cuda.device(dev):   # the kernels launch on the calling thread's current device
+            if T <= GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E:
+                rc = self.lib._c.bb_matmul_grouped(self._desc_ref, E, offsets.data_ptr(), A.data_ptr(), *ptrs,
+                                                   output.data_ptr(), T, stream)
+                if rc != 0:
+                    raise RuntimeError(f"bb_matmul_grouped failed (code {rc}): {_lib.last_error()}")
+            else:
+                self._forward_grouped_per_group(A, W, offsets, scale, zeros, bias, output, dev, stream)
+        return output
+
+    def _forward_grouped_per_group(self, A, W, offsets, scale, zeros, bias, output, dev, stream):
+        """prefill side of forward_grouped: one bb_matmul per non-empty group on its row slice, with the offsets clamped exactly as
+        the grouped kernel clamps them ([0, T]; a group whose end is below its start is empty)."""
+        T = A.shape[0]
+        bounds = offsets.cpu().clamp(0, T).tolist()
+        for e in range(len(bounds) - 1):
+            r0, r1 = bounds[e], bounds[e + 1]
+            if r1 <= r0:
+                continue
+            m = r1 - r0
+            ws_ptr, ws_bytes = self._workspace_for(m, dev, stream)
+            rc = self.lib._c.bb_matmul(self._desc_ref, A[r0:r1].data_ptr(), W[e].data_ptr(), 0,
+                                       scale[e].data_ptr() if self.with_scaling else 0,
+                                       zeros[e].data_ptr() if self.with_zeros else 0,
+                                       bias[e].data_ptr() if self.with_bias else 0,
+                                       output[r0:r1].data_ptr(), m, ws_ptr, ws_bytes, stream)
+            if rc != 0:
+                raise RuntimeError(f"bb_matmul failed (code {rc}): {_lib.last_error()}")
 
     def _forward_consistent(self, A, W, bias, output):
         """A_dtype == W_dtype (no sub-byte decode; general_matmul/__init__.py:33-51,568-580): a plain library GEMM, outside the

@@ -134,6 +134,23 @@ int bb_matmul_scatter(const bb_matmul_desc* desc, const void* A, const void* W, 
                       const void* zeros, const void* bias, void* const* peer_C, int n_peers, int64_t ldc,
                       int64_t col_offset, int m, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Grouped matmul for mixture-of-experts layers (no reference counterpart; the contract of torch._grouped_mm with offsets).
+ * `num_groups` problems share `desc` and run as ONE kernel launch.  A[total_rows, K] holds the rows of every group, sorted so
+ * that group e owns rows [offsets[e], offsets[e+1]); `offsets` is a DEVICE int32 array of num_groups + 1 entries, read by the
+ * kernel (no host synchronisation: the call is CUDA-graph capturable for every routing).  For every group e:
+ *     C[offsets[e] : offsets[e+1]] = A[offsets[e] : offsets[e+1]] x dequant(W[e])^T (+ bias[e])
+ * with the formula and rounding of bb_matmul for `desc`.  The per-group operands are stacked: W [E, N, K*bits/8] in the storage
+ * of bb_matmul, scale [E, N, K/g], zeros [E, N, K/g] (A_dtype) or [E, K/g, N*bits/8] (quantized), bias [E, N].
+ * Offsets are clamped to [0, total_rows] and a group whose end is below its start is empty, so a malformed table never reads or
+ * writes outside A / C; rows no group claims are not written.  Covers fp16 / bf16 A, 4- and 2-bit uint / int W in row-major
+ * compressed or interleaved-16 storage, K % 128 == 0, N % 16 == 0, group_size a multiple of 128 or -1; everything else is
+ * rejected.  total_rows == 0 validates and returns 0 without touching the device.  num_groups <= BB_GROUPED_MAX_GROUPS.
+ * Launched with programmatic stream serialization like the decode kernels, but offsets, A AND W are read only after the
+ * preceding kernel has completed (which weights to read depends on the offsets). */
+#define BB_GROUPED_MAX_GROUPS 256
+int bb_matmul_grouped(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                      const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream);
+
 /* Cross-rank barrier for the column-parallel path (no reference counterpart): rank `rank` of `n_peers` signals every peer and
  * waits for all of them, on `stream`, as ONE small kernel -- ordered after the preceding kernels' peer stores (it is launched as a
  * programmatic dependent and waits for them), so after it every rank may read what bb_matmul_scatter calls issued before it wrote.
