@@ -68,10 +68,11 @@ __device__ __forceinline__ T decode_value(uint32_t u, int fmt, int bits, const T
   return cvt_int<T>(0);
 }
 
+// the _rn forms are never contracted into an fma: w * s - z keeps its two roundings (a plain __hmul / __hsub pair is fused)
 template <typename T>
-__device__ __forceinline__ T t_sub(T a, T b) { return __hsub(a, b); }
+__device__ __forceinline__ T t_sub(T a, T b) { return __hsub_rn(a, b); }
 template <typename T>
-__device__ __forceinline__ T t_mul(T a, T b) { return __hmul(a, b); }
+__device__ __forceinline__ T t_mul(T a, T b) { return __hmul_rn(a, b); }
 template <typename T>
 __device__ __forceinline__ T t_fma(T a, T b, T c) { return __hfma(a, b, c); }
 
@@ -122,8 +123,11 @@ generic_float_kernel(const bb_matmul_desc d, const T* __restrict__ A, const uint
   const size_t row_bytes = size_t(K) * bits / 8;
   const int tiled = d.w_tile == BB_TILE_SLAB;
   const uint8_t* Wrow = W + (tiled ? tiled_byte_offset(n, 0, (long long)row_bytes) : size_t(n) * row_bytes);
+  // "rescale" w * s - z: the reference's LOP3 decode (fp16, interleaved integer weights) uses one fma for 4- and 1-bit weights
+  // (lop3.py:256,269; decode_i1b_to_f16_scale_zeros_rescale) but multiplies then subtracts for 2-bit ones (:633-635); every
+  // other case is its TE definition, two roundings (bf16 has no fast decode in the reference)
   const bool use_fma = d.w_layout != BB_LAYOUT_COMPRESSED && (d.w_fmt == BB_W_UINT || d.w_fmt == BB_W_INT) &&
-                       std::is_same<T, __half>::value;
+                       std::is_same<T, __half>::value && bits != 2;
   float acc[MT];
 #pragma unroll
   for (int i = 0; i < MT; ++i) acc[i] = 0.f;
