@@ -276,16 +276,16 @@ int bb_matmul_scatter(const bb_matmul_desc* desc, const void* A, const void* W, 
                      workspace_bytes, stream);
 }
 
-int bb_matmul_grouped(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
-                      const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream) {
-  if (validate(desc)) return 1;
-  if (!grouped_supported(*desc)) return 1;
+// the argument checks of both grouped entry points, after the configuration check: 0 = launch, -1 = nothing to do
+// (total_rows == 0), otherwise the error code to return
+static int check_grouped_args(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                              const void* scale, const void* zeros, const void* bias, void* C, int total_rows) {
   if (num_groups < 1 || num_groups > BB_GROUPED_MAX_GROUPS) {
     set_error("num_groups must be in [1, %d] (got %d)", BB_GROUPED_MAX_GROUPS, num_groups);
     return 1;
   }
   if (total_rows < 0) { set_error("total_rows must be >= 0 (got %d)", total_rows); return 1; }
-  if (total_rows == 0) return 0;
+  if (total_rows == 0) return -1;
   if (!offsets) { set_error("offsets must be a device pointer to num_groups + 1 int32 values"); return 1; }
   if (!A || !W || !C) { set_error("A, W and C must be non-null"); return 1; }
   if (desc->with_scaling && !scale) { set_error("with_scaling is set but scale is null"); return 1; }
@@ -295,7 +295,25 @@ int bb_matmul_grouped(const bb_matmul_desc* desc, int num_groups, const int32_t*
     set_error("grouped matmul: A and W must be 16-byte aligned, offsets 4-byte aligned");
     return 5;
   }
+  return 0;
+}
+
+int bb_matmul_grouped(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                      const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream) {
+  if (validate(desc)) return 1;
+  if (!grouped_supported(*desc)) return 1;
+  const int rc = check_grouped_args(desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows);
+  if (rc) return rc < 0 ? 0 : rc;
   return launch_grouped(*desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows, (cudaStream_t)stream);
+}
+
+int bb_matmul_grouped_gemm(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                           const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream) {
+  if (validate(desc)) return 1;
+  if (!grouped_gemm_supported(*desc)) return 1;
+  const int rc = check_grouped_args(desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows);
+  if (rc) return rc < 0 ? 0 : rc;
+  return launch_grouped_gemm(*desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows, (cudaStream_t)stream);
 }
 
 int bb_peer_barrier(void* const* peer_flags, int n_peers, int rank, void* stream) {

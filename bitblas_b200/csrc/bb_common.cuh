@@ -88,6 +88,10 @@ size_t gemm_ts_workspace_bytes(const bb_matmul_desc& d, int m);
 bool grouped_supported(const bb_matmul_desc& d);
 int launch_grouped(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
                    const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream);
+// grouped wgmma GEMM, bb_grouped_gemm.cu: the same operands and offset contract
+bool grouped_gemm_supported(const bb_matmul_desc& d);
+int launch_grouped_gemm(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                        const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream);
 
 // bit position of logical element `o` (0 .. 32/bits-1) inside its 32-bit storage word, for each weight
 // layout (restates bitblas/quantization/utils.py:73-110 + testing/cpp/lop3_type_conversion/fast_decoding.hpp:30-95,607-668)
@@ -348,6 +352,57 @@ __device__ __forceinline__ void decode_u4x8_to_u8(uint32_t w, uint32_t orv, uint
 // bytes (u | 0x80) -> signed (u - zp) without inter-byte borrows: ((u|0x80) - zp) ^ 0x80
 __device__ __forceinline__ uint32_t bytes_sub_zp(uint32_t v_or80, uint32_t zp4) {
   return (v_or80 - zp4) ^ 0x80808080u;
+}
+
+// Programmatic dependent launch (the design notes are in bb_gemv_mma.cuh)
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+// ---- work schedule of the grouped (mixture-of-experts) kernels over untrusted device offsets ---------------------------------
+// Run by the 32 lanes of one warp (lane = threadIdx.x) on the kernel's parameters g (g.offsets [g.E + 1], g.T rows; read from the
+// parameter space as the kernel would): clamps offsets[e], offsets[e + 1] to [0, T] (a group whose end is below its start is
+// empty) into row0_s[e] / rows_s[e], and gives group e the work items [item0_s[e], item0_s[e + 1]): per_chunk * ceil(rows / R)
+// of them, numbered by one warp prefix sum; item0_s[E] = all items.  The caller synchronises the CTA before it reads the arrays.
+template <typename GP>
+__device__ __forceinline__ void grouped_schedule(const GP& g, int R, int per_chunk, int* row0_s, int* rows_s, int* item0_s) {
+  const int lane = threadIdx.x;
+  const int per = (g.E + 31) / 32;   // consecutive groups per lane
+  const int e0 = lane * per;
+  int cnt = 0;
+  for (int i = 0; i < per; ++i) {
+    const int e = e0 + i;
+    if (e < g.E) {
+      const int b = min(max(g.offsets[e], 0), g.T);
+      const int m = max(min(max(g.offsets[e + 1], 0), g.T) - b, 0);
+      row0_s[e] = b;
+      rows_s[e] = m;
+      cnt += per_chunk * ((m + R - 1) / R);
+    }
+  }
+  int incl = cnt;   // inclusive prefix sum over the lanes
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, incl, d);
+    if (lane >= d) incl += v;
+  }
+  int run = incl - cnt;
+  for (int i = 0; i < per; ++i) {
+    const int e = e0 + i;
+    if (e < g.E) {
+      item0_s[e] = run;
+      run += per_chunk * ((rows_s[e] + R - 1) / R);
+    }
+  }
+  if (lane == 31) item0_s[g.E] = incl;
+}
+// the group of work item `item`: the last e with item0_s[e] <= item (an empty group shares its start with the next one)
+__device__ __forceinline__ int grouped_find(const int* item0_s, int E, int item) {
+  int lo = 0, hi = E - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (item0_s[mid] <= item) lo = mid; else hi = mid - 1;
+  }
+  return lo;
 }
 
 }  // namespace bb

@@ -60,9 +60,8 @@ __device__ __forceinline__ float raw_to_float(uint16_t b) {
 // executes pdl_wait -- which
 // returns once the preceding kernel has completed and flushed -- before the first activation load.  Launch latency and the
 // first DRAM round trip of kernel i+1 then overlap the tail of kernel i.  Both instructions are no-ops when the launch
-// carries no programmatic-serialization attribute or the predecessor never triggers.
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+// carries no programmatic-serialization attribute or the predecessor never triggers.  (pdl_launch_dependents / pdl_wait:
+// bb_common.cuh.)
 
 template <int BITS>
 __device__ __forceinline__ void load_w(const uint8_t* p, uint32_t (&w)[BITS]) {

@@ -48,48 +48,12 @@ gemv_grouped_kernel(const GroupedParams g) {
 
   pdl_wait();   // offsets and A are the preceding kernels' output; nothing is read before this (see the header)
   const int nb = g.p.N / 16;
-  if (threadIdx.x < 32) {
-    const int lane = threadIdx.x;
-    const int per = (g.E + 31) / 32;   // consecutive groups per lane
-    const int e0 = lane * per;
-    int cnt = 0;
-    for (int i = 0; i < per; ++i) {
-      const int e = e0 + i;
-      if (e < g.E) {
-        const int b = min(max(g.offsets[e], 0), g.T);
-        const int m = max(min(max(g.offsets[e + 1], 0), g.T) - b, 0);
-        row0_s[e] = b;
-        rows_s[e] = m;
-        cnt += nb * ((m + R - 1) / R);
-      }
-    }
-    int incl = cnt;   // inclusive prefix sum over the lanes
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const int v = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl += v;
-    }
-    int run = incl - cnt;
-    for (int i = 0; i < per; ++i) {
-      const int e = e0 + i;
-      if (e < g.E) {
-        item0_s[e] = run;
-        run += nb * ((rows_s[e] + R - 1) / R);
-      }
-    }
-    if (lane == 31) item0_s[g.E] = incl;
-  }
+  if (threadIdx.x < 32) grouped_schedule(g, R, nb, row0_s, rows_s, item0_s);
   __syncthreads();
   const int total = item0_s[g.E];
 
   for (int item = blockIdx.x; item < total; item += gridDim.x) {
-    // the group of this item: the last e with item0_s[e] <= item (an empty group shares its start with the next one)
-    int lo = 0, hi = g.E - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (item0_s[mid] <= item) lo = mid; else hi = mid - 1;
-    }
-    const int e = lo;
+    const int e = grouped_find(item0_s, g.E, item);
     const int local = item - item0_s[e];
     const int chunk = local / nb, rb = local - chunk * nb;
     const int r0 = row0_s[e] + chunk * R;

@@ -263,11 +263,13 @@ class GroupedLinear(nn.Module):
         if not bias:
             self.bias = None
 
-    def forward(self, A, offsets, output=None):
+    def forward(self, A, offsets, output=None, capturable=False):
+        """capturable=True: one graph-capturable launch at every token count (see Matmul.forward_grouped)"""
         op = self.bitblas_matmul
         cfg = op.config
         return op.forward_grouped(A, self.qweight, offsets, scale=self.scales if cfg.with_scaling else None,
-                                  zeros=self.zeros if cfg.with_zeros else None, bias=self.bias, output=output)
+                                  zeros=self.zeros if cfg.with_zeros else None, bias=self.bias, output=output,
+                                  capturable=capturable)
 
     def load_and_transform_weight(self, weight: torch.Tensor, scales: torch.Tensor = None, zeros: torch.Tensor = None,
                                   bias: torch.Tensor = None):

@@ -274,6 +274,7 @@ class Matmul(Operator):
         self._ws_need = {}
         self._checked_key = None
         self._grouped_checked_key = None
+        self._grouped_gemm_ok = False   # bb_matmul_grouped_gemm covers the checked parameter set (N % 128 == 0)
         self._torch_a_dtype = getattr(torch, config.A_dtype, None)
         self._desc_ref = None
         self.weight_executors = None
@@ -545,7 +546,7 @@ class Matmul(Operator):
         for name, t, dtype, shape, _ in specs:
             self._check_tensor(t, name, dtype)
 
-    def forward_grouped(self, A, W, offsets, scale=None, zeros=None, bias=None, output=None):
+    def forward_grouped(self, A, W, offsets, scale=None, zeros=None, bias=None, output=None, capturable=False):
         """Grouped matmul for mixture-of-experts layers (bb_matmul_grouped): E problems of this operator's config.  A [T, K] holds
         every group's rows, sorted so that group e owns rows [offsets[e], offsets[e+1]); `offsets` is an int32 CUDA tensor of
         E + 1 entries.  W, scale, zeros and bias are stacked over the groups (see _check_grouped_params).  For every group e:
@@ -555,7 +556,11 @@ class Matmul(Operator):
         Up to GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E rows this is ONE kernel launch that reads the offsets on the device: no host
         synchronisation, CUDA-graph capturable.  Above it (prefill) the offsets are copied to the host once and every non-empty
         group runs through bb_matmul on its row slice, where the dispatcher picks the wgmma GEMM; that path synchronises with the
-        device and cannot be captured in a graph."""
+        device and cannot be captured in a graph.
+
+        capturable=True (the meaning the flag has on torch's optimizers): the host never reads the offsets, so the call is one
+        launch and graph-capturable at every T.  Above the threshold it runs the grouped wgmma GEMM (bb_matmul_grouped_gemm, the
+        numerics of bb_matmul on the wgmma GEMM) where it covers the config (N % 128 == 0), and bb_matmul_grouped otherwise."""
         if self.consistent:
             raise NotImplementedError("forward_grouped needs a low-bit weight operator")
         c = self.config
@@ -570,6 +575,7 @@ class Matmul(Operator):
         if key != self._grouped_checked_key:
             self._check_grouped_params(E, W, scale, zeros, bias)
             self.check_grouped(E)
+            self._grouped_gemm_ok = self.lib._c.bb_matmul_grouped_gemm(self._desc_ref, E, 0, 0, 0, 0, 0, 0, 0, 0, 0) == 0
             self._grouped_checked_key = key
         if not isinstance(A, torch.Tensor) or A.dim() != 2 or A.shape[1] != c.K:
             raise ValueError(f"A must be [T, K={c.K}], got {tuple(A.shape) if isinstance(A, torch.Tensor) else type(A)}")
@@ -591,11 +597,16 @@ class Matmul(Operator):
         stream = torch.cuda.current_stream(dev).cuda_stream
         ptrs = key[1:]
         with torch.cuda.device(dev):   # the kernels launch on the calling thread's current device
-            if T <= GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E:
+            if T <= GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E or (capturable and not self._grouped_gemm_ok):
                 rc = self.lib._c.bb_matmul_grouped(self._desc_ref, E, offsets.data_ptr(), A.data_ptr(), *ptrs,
                                                    output.data_ptr(), T, stream)
                 if rc != 0:
                     raise RuntimeError(f"bb_matmul_grouped failed (code {rc}): {_lib.last_error()}")
+            elif capturable:
+                rc = self.lib._c.bb_matmul_grouped_gemm(self._desc_ref, E, offsets.data_ptr(), A.data_ptr(), *ptrs,
+                                                        output.data_ptr(), T, stream)
+                if rc != 0:
+                    raise RuntimeError(f"bb_matmul_grouped_gemm failed (code {rc}): {_lib.last_error()}")
             else:
                 self._forward_grouped_per_group(A, W, offsets, scale, zeros, bias, output, dev, stream)
         return output

@@ -151,6 +151,15 @@ int bb_matmul_scatter(const bb_matmul_desc* desc, const void* A, const void* W, 
 int bb_matmul_grouped(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
                       const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream);
 
+/* Grouped matmul on the wgmma GEMM, for mixture-of-experts prefill: the signature, operand layout and offset contract of
+ * bb_matmul_grouped, with the numerics of bb_matmul on the wgmma GEMM (gemm_ts, without split-K), in ONE CUDA-graph capturable
+ * launch at any number of rows per group.  Covers what bb_matmul_grouped covers with N % 128 == 0 (the CTA tile is 128 weight
+ * rows); everything else is rejected with a message.  Takes no workspace.  total_rows == 0 validates and returns 0 without
+ * touching the device; A and W must be 16-byte aligned.  Launched with programmatic stream serialization; offsets, A and W
+ * are read only after the preceding kernel has completed. */
+int bb_matmul_grouped_gemm(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                           const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream);
+
 /* Cross-rank barrier for the column-parallel path (no reference counterpart): rank `rank` of `n_peers` signals every peer and
  * waits for all of them, on `stream`, as ONE small kernel -- ordered after the preceding kernels' peer stores (it is launched as a
  * programmatic dependent and waits for them), so after it every rank may read what bb_matmul_scatter calls issued before it wrote.
