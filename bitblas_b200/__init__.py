@@ -26,3 +26,4 @@ from .utils import auto_detect_nvidia_target  # noqa: E402,F401
 from . import cache, quantization, testing  # noqa: E402,F401
 from .parallel import ColumnParallelLinear  # noqa: E402,F401
 from .graph import CapturedStep  # noqa: E402,F401
+from .moe import MoEExperts  # noqa: E402,F401

@@ -6,6 +6,7 @@
 //   m <= 8   : memory-bound streaming kernels (bb_gemv.cu)
 //   m  > 8   : wgmma tensor-core kernel (bb_gemm_ts.cu), split-K when the tile grid is smaller than the chip
 //   anything the fast kernels do not cover: the generic SIMT kernel (bb_generic.cu).
+#include <climits>
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
@@ -314,6 +315,82 @@ int bb_matmul_grouped_gemm(const bb_matmul_desc* desc, int num_groups, const int
   const int rc = check_grouped_args(desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows);
   if (rc) return rc < 0 ? 0 : rc;
   return launch_grouped_gemm(*desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows, (cudaStream_t)stream);
+}
+
+// the gate/up interleave pairs 8 gate rows with 8 up rows in every 16-row block of W: N = 2I with I % 8 == 0
+static bool swiglu_shape_ok(const bb_matmul_desc* desc) {
+  if (desc && desc->N % 16) {
+    set_error("SwiGLU: desc->N = 2I needs I %% 8 == 0 (gate/up interleave in blocks of 8 rows; N=%d)", desc->N);
+    return false;
+  }
+  return true;
+}
+
+int bb_matmul_grouped_swiglu(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                             const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream) {
+  if (validate(desc)) return 1;
+  if (!swiglu_shape_ok(desc) || !grouped_supported(*desc)) return 1;
+  const int rc = check_grouped_args(desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows);
+  if (rc) return rc < 0 ? 0 : rc;
+  return launch_grouped(*desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows, (cudaStream_t)stream, true);
+}
+
+int bb_matmul_grouped_gemm_swiglu(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                                  const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream) {
+  if (validate(desc)) return 1;
+  if (!swiglu_shape_ok(desc) || !grouped_gemm_supported(*desc)) return 1;
+  const int rc = check_grouped_args(desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows);
+  if (rc) return rc < 0 ? 0 : rc;
+  return launch_grouped_gemm(*desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows, (cudaStream_t)stream, true);
+}
+
+int bb_moe_route(const int32_t* topk_ids, int num_tokens, int top_k, int num_experts, const void* x, int a_dtype, int K,
+                 int32_t* offsets, int32_t* slot_rows, void* x_sorted, void* stream) {
+  if (num_experts < 1 || num_experts > BB_GROUPED_MAX_GROUPS) {
+    set_error("moe route: num_experts must be in [1, %d] (got %d)", BB_GROUPED_MAX_GROUPS, num_experts);
+    return 1;
+  }
+  if (top_k < 1) { set_error("moe route: top_k must be >= 1 (got %d)", top_k); return 1; }
+  if (num_tokens < 0) { set_error("moe route: num_tokens must be >= 0 (got %d)", num_tokens); return 1; }
+  if ((long long)num_tokens * top_k > INT_MAX) {
+    set_error("moe route: num_tokens * top_k must be below 2^31 (got %d x %d)", num_tokens, top_k);
+    return 1;
+  }
+  if (a_dtype != BB_F16 && a_dtype != BB_BF16) { set_error("moe route: x must be float16 or bfloat16 (a_dtype=%d)", a_dtype); return 1; }
+  if (K <= 0 || K % 8) { set_error("moe route: needs K > 0 and K %% 8 == 0 (K=%d)", K); return 1; }
+  if (num_tokens == 0) return 0;
+  if (!topk_ids || !x || !offsets || !slot_rows || !x_sorted) { set_error("moe route: every pointer must be non-null"); return 1; }
+  if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(x_sorted) & 15) ||
+      (reinterpret_cast<uintptr_t>(topk_ids) & 3) || (reinterpret_cast<uintptr_t>(offsets) & 3) ||
+      (reinterpret_cast<uintptr_t>(slot_rows) & 3)) {
+    set_error("moe route: x and x_sorted must be 16-byte aligned, the int32 arrays 4-byte aligned");
+    return 5;
+  }
+  return launch_moe_route(topk_ids, num_tokens * top_k, top_k, num_experts, x, K, offsets, slot_rows, x_sorted,
+                          (cudaStream_t)stream);
+}
+
+int bb_moe_combine(const int32_t* slot_rows, const float* topk_weights, const void* Y, int out_dtype, void* out, int num_tokens,
+                   int top_k, int N, void* stream) {
+  if (top_k < 1) { set_error("moe combine: top_k must be >= 1 (got %d)", top_k); return 1; }
+  if (num_tokens < 0) { set_error("moe combine: num_tokens must be >= 0 (got %d)", num_tokens); return 1; }
+  if ((long long)num_tokens * top_k > INT_MAX) {
+    set_error("moe combine: num_tokens * top_k must be below 2^31 (got %d x %d)", num_tokens, top_k);
+    return 1;
+  }
+  if (out_dtype != BB_F16 && out_dtype != BB_BF16 && out_dtype != BB_F32) {
+    set_error("moe combine: out_dtype must be float16, bfloat16 or float32 (got %d)", out_dtype);
+    return 1;
+  }
+  if (N <= 0 || N % 8) { set_error("moe combine: needs N > 0 and N %% 8 == 0 (N=%d)", N); return 1; }
+  if (num_tokens == 0) return 0;
+  if (!slot_rows || !topk_weights || !Y || !out) { set_error("moe combine: every pointer must be non-null"); return 1; }
+  if ((reinterpret_cast<uintptr_t>(Y) & 15) || (reinterpret_cast<uintptr_t>(out) & 15) ||
+      (reinterpret_cast<uintptr_t>(slot_rows) & 3) || (reinterpret_cast<uintptr_t>(topk_weights) & 3)) {
+    set_error("moe combine: Y and out must be 16-byte aligned, slot_rows and topk_weights 4-byte aligned");
+    return 5;
+  }
+  return launch_moe_combine(slot_rows, topk_weights, Y, out_dtype, out, num_tokens, top_k, N, (cudaStream_t)stream);
 }
 
 int bb_peer_barrier(void* const* peer_flags, int n_peers, int rank, void* stream) {

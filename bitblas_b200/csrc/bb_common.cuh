@@ -84,14 +84,22 @@ int launch_gemv_i8(const MatmulArgs& a);
 bool gemm_ts_supported(const bb_matmul_desc& d, int m);
 int launch_gemm_ts(const MatmulArgs& a);
 size_t gemm_ts_workspace_bytes(const bb_matmul_desc& d, int m);
-// grouped (mixture-of-experts) matmul, bb_grouped.cu: grouped_supported sets the error message when it returns false
+// grouped (mixture-of-experts) matmul, bb_grouped.cu: grouped_supported sets the error message when it returns false.
+// swiglu: W holds gate/up interleaved (2I = d.N rows), C is [total_rows, d.N / 2] = silu(gate) * up (store_swiglu below)
 bool grouped_supported(const bb_matmul_desc& d);
 int launch_grouped(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
-                   const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream);
+                   const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream,
+                   bool swiglu = false);
 // grouped wgmma GEMM, bb_grouped_gemm.cu: the same operands and offset contract
 bool grouped_gemm_supported(const bb_matmul_desc& d);
 int launch_grouped_gemm(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
-                        const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream);
+                        const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream,
+                        bool swiglu = false);
+// mixture-of-experts routing and top-k combine, bb_moe.cu (arguments validated by the callers in bb_api.cu)
+int launch_moe_route(const int32_t* topk_ids, int n_slots, int top_k, int num_experts, const void* x, int K, int32_t* offsets,
+                     int32_t* slot_rows, void* x_sorted, cudaStream_t stream);
+int launch_moe_combine(const int32_t* slot_rows, const float* topk_weights, const void* Y, int out_dtype, void* out,
+                       int num_tokens, int top_k, int N, cudaStream_t stream);
 
 // bit position of logical element `o` (0 .. 32/bits-1) inside its 32-bit storage word, for each weight
 // layout (restates bitblas/quantization/utils.py:73-110 + testing/cpp/lop3_type_conversion/fast_decoding.hpp:30-95,607-668)
@@ -395,6 +403,31 @@ __device__ __forceinline__ void grouped_schedule(const GP& g, int R, int per_chu
   }
   if (lane == 31) item0_s[g.E] = incl;
 }
+// ---- SwiGLU epilogue of the grouped kernels (gate/up interleave: weight row 16b + i is gate row 8b + i for i < 8, up row 8b + i - 8
+// for i >= 8; both halves of a 16-row block are owned by the same thread) ----------------------------------------------------------
+// one pre-activation as the plain grouped epilogue stores it: cast to out_dtype, then the bias (already a float of A_dtype) added in
+// out_dtype; fp32 output: one fp32 sum (bias = 0 without one)
+__device__ __forceinline__ float swiglu_operand(float v, bool has_bias, float bias, int out_dtype) {
+  if (out_dtype == BB_F16) {
+    __half h = __float2half_rn(v);
+    if (has_bias) h = __hadd(h, __float2half_rn(bias));
+    return __half2float(h);
+  }
+  if (out_dtype == BB_BF16) {
+    __nv_bfloat16 h = __float2bfloat16_rn(v);
+    if (has_bias) h = __hadd(h, __float2bfloat16_rn(bias));
+    return __bfloat162float(h);
+  }
+  return v + bias;
+}
+// C[o] = silu(g) * u = g / (1 + exp(-g)) * u in fp32, rounded once to out_dtype
+__device__ __forceinline__ void store_swiglu(void* C, size_t o, float g, float u, int out_dtype) {
+  const float y = g / (1.f + expf(-g)) * u;
+  if (out_dtype == BB_F16) reinterpret_cast<__half*>(C)[o] = __float2half_rn(y);
+  else if (out_dtype == BB_BF16) reinterpret_cast<__nv_bfloat16*>(C)[o] = __float2bfloat16_rn(y);
+  else reinterpret_cast<float*>(C)[o] = y;
+}
+
 // the group of work item `item`: the last e with item0_s[e] <= item (an empty group shares its start with the next one)
 __device__ __forceinline__ int grouped_find(const int* item0_s, int E, int item) {
   int lo = 0, hi = E - 1;

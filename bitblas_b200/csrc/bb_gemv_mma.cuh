@@ -95,8 +95,9 @@ constexpr int gemv_mma_maxnreg(int nt, int zk) {
 // short-lived CTA costs more than the in-order load stalls it removes.)
 // One 16-row block `rb` of W against rows [0, p.M) of p.A (p.M <= 8 * NT), K split over the p.ks warps of the CTA and reduced
 // through `red`.  PDL: the tile issues griddepcontrol.wait after its weight prologue and launch_dependents after its weight
-// stream (gemv_mma_kernel); with PDL = false the caller owns both instructions.
-template <typename T, int BITS, bool IL, int NT, int ZK, bool SC, bool PDL>
+// stream (gemv_mma_kernel); with PDL = false the caller owns both instructions.  SWIGLU: W holds gate/up interleaved (bb_common.cuh),
+// and rows r and r + 8 of the block become column rb * 8 + r of p.out (row stride p.out.ld = N / 2), one destination only.
+template <typename T, int BITS, bool IL, int NT, int ZK, bool SC, bool PDL, bool SWIGLU = false>
 __device__ __forceinline__ void gemv_mma_tile(const GemvParams& p, const int rb, float (&red)[MAX_KS][16][8 * NT]) {
   constexpr bool RS = ZK == 2;
   constexpr int NP = 32 / BITS / 2;     // pairs per 32-bit word: 4 (4-bit) or 8 (2-bit)
@@ -355,24 +356,41 @@ __device__ __forceinline__ void gemv_mma_tile(const GemvParams& p, const int rb,
     red[warp][r + 8][8 * t + 2 * q + 1] = acc_t[t][3];
   }
   __syncthreads();
-  for (int idx = threadIdx.x; idx < 16 * 8 * NT; idx += blockDim.x) {
-    const int row = idx & 15, m = idx >> 4;
-    if (m >= p.M) continue;
-    float v = 0.f;
-    for (int w = 0; w < p.ks; ++w) v += red[w][row][m];
-    const int n = rb * 16 + row;
-    const size_t o = size_t(m) * size_t(p.out.ld) + size_t(p.out.col0) + n;
-    const float bf = p.bias ? TypeTraits<T>::to_float(reinterpret_cast<const T*>(p.bias)[n]) : 0.f;
-    if (p.out_dtype == BB_F16) {
-      __half h = __float2half_rn(v);
-      if (p.bias) h = __hadd(h, __float2half_rn(bf));
-      for (int d = 0; d < p.out.n; ++d) reinterpret_cast<__half*>(p.out.ptr[d])[o] = h;
-    } else if (p.out_dtype == BB_BF16) {
-      __nv_bfloat16 h = __float2bfloat16_rn(v);
-      if (p.bias) h = __hadd(h, __float2bfloat16_rn(bf));
-      for (int d = 0; d < p.out.n; ++d) reinterpret_cast<__nv_bfloat16*>(p.out.ptr[d])[o] = h;
-    } else {
-      for (int d = 0; d < p.out.n; ++d) reinterpret_cast<float*>(p.out.ptr[d])[o] = v + bf;
+  if constexpr (SWIGLU) {
+    for (int idx = threadIdx.x; idx < 8 * 8 * NT; idx += blockDim.x) {
+      const int row = idx & 7, m = idx >> 3;
+      if (m >= p.M) continue;
+      float vg = 0.f, vu = 0.f;
+      for (int w = 0; w < p.ks; ++w) {
+        vg += red[w][row][m];
+        vu += red[w][row + 8][m];
+      }
+      const int n = rb * 16 + row;
+      const T* bias = reinterpret_cast<const T*>(p.bias);
+      const float g = swiglu_operand(vg, bias != nullptr, bias ? TypeTraits<T>::to_float(bias[n]) : 0.f, p.out_dtype);
+      const float u = swiglu_operand(vu, bias != nullptr, bias ? TypeTraits<T>::to_float(bias[n + 8]) : 0.f, p.out_dtype);
+      store_swiglu(p.out.ptr[0], size_t(m) * size_t(p.out.ld) + size_t(rb * 8 + row), g, u, p.out_dtype);
+    }
+  } else {
+    for (int idx = threadIdx.x; idx < 16 * 8 * NT; idx += blockDim.x) {
+      const int row = idx & 15, m = idx >> 4;
+      if (m >= p.M) continue;
+      float v = 0.f;
+      for (int w = 0; w < p.ks; ++w) v += red[w][row][m];
+      const int n = rb * 16 + row;
+      const size_t o = size_t(m) * size_t(p.out.ld) + size_t(p.out.col0) + n;
+      const float bf = p.bias ? TypeTraits<T>::to_float(reinterpret_cast<const T*>(p.bias)[n]) : 0.f;
+      if (p.out_dtype == BB_F16) {
+        __half h = __float2half_rn(v);
+        if (p.bias) h = __hadd(h, __float2half_rn(bf));
+        for (int d = 0; d < p.out.n; ++d) reinterpret_cast<__half*>(p.out.ptr[d])[o] = h;
+      } else if (p.out_dtype == BB_BF16) {
+        __nv_bfloat16 h = __float2bfloat16_rn(v);
+        if (p.bias) h = __hadd(h, __float2bfloat16_rn(bf));
+        for (int d = 0; d < p.out.n; ++d) reinterpret_cast<__nv_bfloat16*>(p.out.ptr[d])[o] = h;
+      } else {
+        for (int d = 0; d < p.out.n; ++d) reinterpret_cast<float*>(p.out.ptr[d])[o] = v + bf;
+      }
     }
   }
 }

@@ -18,6 +18,8 @@
 //     instruction; unlike the single-matrix GEMV no weight is prefetched before it.  launch_dependents follows the CTA's last item.
 //   * the offsets are untrusted: each is clamped to [0, T] and a group whose end is below its start is empty, so a malformed
 //     table never reads or writes outside A[0:T] / C[0:T]; rows that no group claims are not written.
+//   * SWIGLU instances (bb_matmul_grouped_swiglu): W holds gate/up interleaved and the tile epilogue writes silu(gate) * up into
+//     C [T, N / 2] (gemv_mma_tile, bb_gemv_mma.cuh; DESIGN.md §3.2.1).
 #include <algorithm>
 #include <climits>
 
@@ -37,7 +39,7 @@ struct GroupedParams {
   int out_bytes;              // bytes per element of C
 };
 
-template <typename T, int BITS, bool IL, int NT, int ZK, bool SC>
+template <typename T, int BITS, bool IL, int NT, int ZK, bool SC, bool SWIGLU = false>
 __global__ void __launch_bounds__(NT == 1 ? 128 : MAX_KS * 32) __maxnreg__(gemv_mma_maxnreg(NT, ZK))
 gemv_grouped_kernel(const GroupedParams g) {
   constexpr int R = 8 * NT;   // rows of A per pass over a 16-row block of W
@@ -65,9 +67,9 @@ gemv_grouped_kernel(const GroupedParams g) {
     if (SC) p.scale = reinterpret_cast<const uint8_t*>(g.p.scale) + size_t(e) * size_t(g.s_stride);
     if (ZK) p.zeros = reinterpret_cast<const uint8_t*>(g.p.zeros) + size_t(e) * size_t(g.z_stride);
     if (g.p.bias) p.bias = reinterpret_cast<const uint8_t*>(g.p.bias) + size_t(e) * size_t(g.b_stride);
-    p.out.ptr[0] = reinterpret_cast<uint8_t*>(g.p.out.ptr[0]) + size_t(r0) * size_t(p.N) * size_t(g.out_bytes);
+    p.out.ptr[0] = reinterpret_cast<uint8_t*>(g.p.out.ptr[0]) + size_t(r0) * size_t(SWIGLU ? p.N / 2 : p.N) * size_t(g.out_bytes);
     if (item != int(blockIdx.x)) __syncthreads();   // the previous item's epilogue has finished reading `red`
-    gemv_mma_tile<T, BITS, IL, NT, ZK, SC, false>(p, rb, red);
+    gemv_mma_tile<T, BITS, IL, NT, ZK, SC, false, SWIGLU>(p, rb, red);
   }
   pdl_launch_dependents();
 }
@@ -111,12 +113,12 @@ int launch_grouped_kernel(KernelT kernel, int (&occ_cache)[MAX_KS + 1], GroupedP
   return 0;
 }
 
-template <typename T, int BITS, bool IL>
+template <typename T, int BITS, bool IL, bool SWIGLU>
 int launch_grouped_nt(const GroupedParams& g, int nt, const int (&max_items)[3], cudaStream_t s) {
 #define BB_GROUPED_GO(NTV, ZKV, SCV, MAXKS)                                                                   \
   {                                                                                                          \
     static int occ_cache[MAX_KS + 1] = {-1, -1, -1, -1, -1, -1, -1, -1, -1};                                 \
-    return launch_grouped_kernel(gemv_grouped_kernel<T, BITS, IL, NTV, ZKV, SCV>, occ_cache, g,             \
+    return launch_grouped_kernel(gemv_grouped_kernel<T, BITS, IL, NTV, ZKV, SCV, SWIGLU>, occ_cache, g,     \
                                  max_items[NTV == 1 ? 0 : (NTV == 2 ? 1 : 2)], MAXKS, s);                    \
   }
 #define BB_GROUPED_NT(ZKV, SCV)                     \
@@ -133,6 +135,17 @@ int launch_grouped_nt(const GroupedParams& g, int nt, const int (&max_items)[3],
 }
 
 size_t elem_bytes(int dtype) { return dtype == BB_F32 ? 4 : 2; }
+
+template <bool SWIGLU>
+int launch_grouped_typed(const bb_matmul_desc& d, bool il, const GroupedParams& g, int nt, const int (&max_items)[3], cudaStream_t s) {
+  if (d.a_dtype == BB_F16) {
+    if (d.w_bits == 4) return il ? launch_grouped_nt<__half, 4, true, SWIGLU>(g, nt, max_items, s) : launch_grouped_nt<__half, 4, false, SWIGLU>(g, nt, max_items, s);
+    return il ? launch_grouped_nt<__half, 2, true, SWIGLU>(g, nt, max_items, s) : launch_grouped_nt<__half, 2, false, SWIGLU>(g, nt, max_items, s);
+  }
+  if (d.w_bits == 4) return il ? launch_grouped_nt<__nv_bfloat16, 4, true, SWIGLU>(g, nt, max_items, s) : launch_grouped_nt<__nv_bfloat16, 4, false, SWIGLU>(g, nt, max_items, s);
+  return il ? launch_grouped_nt<__nv_bfloat16, 2, true, SWIGLU>(g, nt, max_items, s) : launch_grouped_nt<__nv_bfloat16, 2, false, SWIGLU>(g, nt, max_items, s);
+}
+
 
 }  // namespace
 
@@ -157,7 +170,8 @@ bool grouped_supported(const bb_matmul_desc& d) {
 }
 
 int launch_grouped(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
-                   const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream) {
+                   const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream,
+                   bool swiglu) {
   MatmulArgs a = {};
   a.d = d; a.A = A; a.W = W; a.scale = scale; a.zeros = zeros; a.bias = bias; a.C = C; a.m = total_rows; a.n_peers = 0;
   GroupedParams g;
@@ -167,6 +181,7 @@ int launch_grouped(const bb_matmul_desc& d, int num_groups, const int32_t* offse
   p.zeros = d.with_zeros ? zeros : nullptr;
   p.bias = d.with_bias ? bias : nullptr;
   p.out = make_outspec(a);
+  if (swiglu) p.out.ld = d.N / 2;
   p.M = 0; p.N = d.N; p.K = d.K;
   p.g = a.gsize(); p.G = a.groups();
   p.with_scaling = d.with_scaling;
@@ -195,12 +210,7 @@ int launch_grouped(const bb_matmul_desc& d, int num_groups, const int32_t* offse
     max_items[i] = int(items);
   }
   const bool il = d.w_layout == BB_LAYOUT_INTERLEAVED_16;
-  if (d.a_dtype == BB_F16) {
-    if (d.w_bits == 4) return il ? launch_grouped_nt<__half, 4, true>(g, nt, max_items, stream) : launch_grouped_nt<__half, 4, false>(g, nt, max_items, stream);
-    return il ? launch_grouped_nt<__half, 2, true>(g, nt, max_items, stream) : launch_grouped_nt<__half, 2, false>(g, nt, max_items, stream);
-  }
-  if (d.w_bits == 4) return il ? launch_grouped_nt<__nv_bfloat16, 4, true>(g, nt, max_items, stream) : launch_grouped_nt<__nv_bfloat16, 4, false>(g, nt, max_items, stream);
-  return il ? launch_grouped_nt<__nv_bfloat16, 2, true>(g, nt, max_items, stream) : launch_grouped_nt<__nv_bfloat16, 2, false>(g, nt, max_items, stream);
+  return swiglu ? launch_grouped_typed<true>(d, il, g, nt, max_items, stream) : launch_grouped_typed<false>(d, il, g, nt, max_items, stream);
 }
 
 }  // namespace bb

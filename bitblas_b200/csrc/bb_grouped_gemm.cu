@@ -21,6 +21,7 @@
 //     the offsets are read); launch_dependents follows the CTA's last tile.
 //   * the offsets are untrusted, with bb_matmul_grouped's contract: clamped to [0, T], a group whose end is below its start is
 //     empty, and rows no group claims are not written.
+//   * SWIGLU instances (bb_matmul_grouped_gemm_swiglu): gate/up interleaved W, C [T, N / 2] = silu(gate) * up (store_tile).
 #include <algorithm>
 #include <climits>
 
@@ -39,43 +40,60 @@ struct GroupedTsParams {
 };
 
 // gemm_ts_kernel's epilogue for one destination and no split-K: acc[4i + 2h + j] = C^T[row rA + 8h][column 8i + 2t + j] ->
-// C[m, n] for the rows m < m_end, cast to out_dtype, then bias[e][n] added in out_dtype (fp32: in one sum), as bb_matmul rounds
-template <typename T, int BM>
+// C[m, n] for the rows m < m_end, cast to out_dtype, then bias[e][n] added in out_dtype (fp32: in one sum), as bb_matmul rounds.
+// SWIGLU: rows nA = 16b + i and nB = nA + 8 (i < 8) are gate and up of C[m, 8b + i] = silu(gate) * up, row stride N / 2
+template <typename T, int BM, bool SWIGLU>
 __device__ __forceinline__ void store_tile(const float (&acc)[BM / 2], const TsParams& p, const T* bias, int m0, int m_end,
                                            int nA, int nB, int t) {
-  float bias_f[2] = {0.f, 0.f};
-  if (bias) {
-    bias_f[0] = TypeTraits<T>::to_float(bias[nA]);
-    bias_f[1] = TypeTraits<T>::to_float(bias[nB]);
-  }
-  void* const C = p.out.ptr[0];
+  if constexpr (SWIGLU) {
+    const float bg = bias ? TypeTraits<T>::to_float(bias[nA]) : 0.f, bu = bias ? TypeTraits<T>::to_float(bias[nB]) : 0.f;
+    const size_t col = size_t(nA >> 4) * 8 + size_t(nA & 7);
 #pragma unroll
-  for (int i = 0; i < BM / 8; ++i) {
+    for (int i = 0; i < BM / 8; ++i) {
 #pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      const int m = m0 + 8 * i + 2 * t + j;
-      if (m >= m_end) continue;
+      for (int j = 0; j < 2; ++j) {
+        const int m = m0 + 8 * i + 2 * t + j;
+        if (m >= m_end) continue;
+        const float g = swiglu_operand(acc[4 * i + j], bias != nullptr, bg, p.out_dtype);
+        const float u = swiglu_operand(acc[4 * i + 2 + j], bias != nullptr, bu, p.out_dtype);
+        store_swiglu(p.out.ptr[0], size_t(m) * size_t(p.N / 2) + col, g, u, p.out_dtype);
+      }
+    }
+  } else {
+    float bias_f[2] = {0.f, 0.f};
+    if (bias) {
+      bias_f[0] = TypeTraits<T>::to_float(bias[nA]);
+      bias_f[1] = TypeTraits<T>::to_float(bias[nB]);
+    }
+    void* const C = p.out.ptr[0];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const float v = acc[4 * i + 2 * h + j];
-        const size_t o = size_t(m) * size_t(p.N) + size_t(h ? nB : nA);
-        if (p.out_dtype == BB_F16) {
-          __half r = __float2half_rn(v);
-          if (bias) r = __hadd(r, __float2half_rn(bias_f[h]));
-          reinterpret_cast<__half*>(C)[o] = r;
-        } else if (p.out_dtype == BB_BF16) {
-          __nv_bfloat16 r = __float2bfloat16_rn(v);
-          if (bias) r = __hadd(r, __float2bfloat16_rn(bias_f[h]));
-          reinterpret_cast<__nv_bfloat16*>(C)[o] = r;
-        } else {
-          reinterpret_cast<float*>(C)[o] = v + (bias ? bias_f[h] : 0.f);
+    for (int i = 0; i < BM / 8; ++i) {
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int m = m0 + 8 * i + 2 * t + j;
+        if (m >= m_end) continue;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float v = acc[4 * i + 2 * h + j];
+          const size_t o = size_t(m) * size_t(p.N) + size_t(h ? nB : nA);
+          if (p.out_dtype == BB_F16) {
+            __half r = __float2half_rn(v);
+            if (bias) r = __hadd(r, __float2half_rn(bias_f[h]));
+            reinterpret_cast<__half*>(C)[o] = r;
+          } else if (p.out_dtype == BB_BF16) {
+            __nv_bfloat16 r = __float2bfloat16_rn(v);
+            if (bias) r = __hadd(r, __float2bfloat16_rn(bias_f[h]));
+            reinterpret_cast<__nv_bfloat16*>(C)[o] = r;
+          } else {
+            reinterpret_cast<float*>(C)[o] = v + (bias ? bias_f[h] : 0.f);
+          }
         }
       }
     }
   }
 }
 
-template <typename T, int BITS, int BM, bool IL>
+template <typename T, int BITS, int BM, bool IL, bool SWIGLU = false>
 __global__ void __launch_bounds__(TS_THREADS, 1)
 gemm_ts_grouped_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                        const GroupedTsParams g) {
@@ -225,7 +243,7 @@ gemm_ts_grouped_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       if (lane == 0) mbar_arrive(&empty[prev_st]);
       const T* bias = p.bias ? reinterpret_cast<const T*>(reinterpret_cast<const uint8_t*>(p.bias) + size_t(e) * size_t(g.b_stride))
                              : nullptr;
-      store_tile<T, BM>(acc, p, bias, m0, m_end, nA, nB, t);
+      store_tile<T, BM, SWIGLU>(acc, p, bias, m0, m_end, nA, nB, t);
     }
   };
   switch (p.mode) {
@@ -238,10 +256,10 @@ gemm_ts_grouped_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   pdl_launch_dependents();
 }
 
-template <typename T, int BITS, int BM, bool IL>
+template <typename T, int BITS, int BM, bool IL, bool SWIGLU>
 int launch_grouped_gemm_inst(const GroupedTsParams& g, const void* A, const void* W, long long max_tiles, cudaStream_t stream) {
   using SM = TsSmem<T, BITS, BM>;
-  auto kernel = gemm_ts_grouped_kernel<T, BITS, BM, IL>;
+  auto kernel = gemm_ts_grouped_kernel<T, BITS, BM, IL, SWIGLU>;
   static int resident_per_sm[BB_MAX_DEVICES] = {};   // 0 until queried (cudaFuncSetAttribute is per device)
   const int dev = current_device();
   if (!resident_per_sm[dev]) {
@@ -276,7 +294,7 @@ int launch_grouped_gemm_inst(const GroupedTsParams& g, const void* A, const void
   return 0;
 }
 
-template <typename T, int BITS, bool IL>
+template <typename T, int BITS, bool IL, bool SWIGLU>
 int launch_grouped_gemm_bm(const GroupedTsParams& g, const void* A, const void* W, cudaStream_t stream) {
   // rows of A per tile from the mean rows per active group (T rows over at most min(E, T) groups), as launch_ts_bm picks BM
   // from m; tiles: sum_e ceil(m_e / BM) per n-tile <= ceil(T / BM) + (groups with rows)
@@ -284,9 +302,20 @@ int launch_grouped_gemm_bm(const GroupedTsParams& g, const void* A, const void* 
   const int mean_rows = (g.T + active - 1) / active;
   const int bm = mean_rows <= 32 ? 32 : (mean_rows <= 64 ? 64 : 128);
   const long long max_tiles = (long long)(g.p.N / TS_ROWS) * ((g.T + bm - 1) / bm + active);
-  if (bm == 32) return launch_grouped_gemm_inst<T, BITS, 32, IL>(g, A, W, max_tiles, stream);
-  if (bm == 64) return launch_grouped_gemm_inst<T, BITS, 64, IL>(g, A, W, max_tiles, stream);
-  return launch_grouped_gemm_inst<T, BITS, 128, IL>(g, A, W, max_tiles, stream);
+  if (bm == 32) return launch_grouped_gemm_inst<T, BITS, 32, IL, SWIGLU>(g, A, W, max_tiles, stream);
+  if (bm == 64) return launch_grouped_gemm_inst<T, BITS, 64, IL, SWIGLU>(g, A, W, max_tiles, stream);
+  return launch_grouped_gemm_inst<T, BITS, 128, IL, SWIGLU>(g, A, W, max_tiles, stream);
+}
+
+template <bool SWIGLU>
+int launch_grouped_gemm_typed(const bb_matmul_desc& d, bool il, const GroupedTsParams& g, const void* A, const void* W,
+                              cudaStream_t s) {
+  if (d.a_dtype == BB_F16) {
+    if (d.w_bits == 4) return il ? launch_grouped_gemm_bm<__half, 4, true, SWIGLU>(g, A, W, s) : launch_grouped_gemm_bm<__half, 4, false, SWIGLU>(g, A, W, s);
+    return il ? launch_grouped_gemm_bm<__half, 2, true, SWIGLU>(g, A, W, s) : launch_grouped_gemm_bm<__half, 2, false, SWIGLU>(g, A, W, s);
+  }
+  if (d.w_bits == 4) return il ? launch_grouped_gemm_bm<__nv_bfloat16, 4, true, SWIGLU>(g, A, W, s) : launch_grouped_gemm_bm<__nv_bfloat16, 4, false, SWIGLU>(g, A, W, s);
+  return il ? launch_grouped_gemm_bm<__nv_bfloat16, 2, true, SWIGLU>(g, A, W, s) : launch_grouped_gemm_bm<__nv_bfloat16, 2, false, SWIGLU>(g, A, W, s);
 }
 
 }  // namespace
@@ -302,7 +331,8 @@ bool grouped_gemm_supported(const bb_matmul_desc& d) {
 }
 
 int launch_grouped_gemm(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
-                        const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream) {
+                        const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream,
+                        bool swiglu) {
   MatmulArgs a = {};
   a.d = d; a.A = A; a.W = W; a.scale = scale; a.zeros = zeros; a.bias = bias; a.C = C; a.m = total_rows; a.n_peers = 0;
   GroupedTsParams g;
@@ -326,12 +356,7 @@ int launch_grouped_gemm(const bb_matmul_desc& d, int num_groups, const int32_t* 
     return 1;
   }
   const bool il = d.w_layout == BB_LAYOUT_INTERLEAVED_16;
-  if (d.a_dtype == BB_F16) {
-    if (d.w_bits == 4) return il ? launch_grouped_gemm_bm<__half, 4, true>(g, A, W, stream) : launch_grouped_gemm_bm<__half, 4, false>(g, A, W, stream);
-    return il ? launch_grouped_gemm_bm<__half, 2, true>(g, A, W, stream) : launch_grouped_gemm_bm<__half, 2, false>(g, A, W, stream);
-  }
-  if (d.w_bits == 4) return il ? launch_grouped_gemm_bm<__nv_bfloat16, 4, true>(g, A, W, stream) : launch_grouped_gemm_bm<__nv_bfloat16, 4, false>(g, A, W, stream);
-  return il ? launch_grouped_gemm_bm<__nv_bfloat16, 2, true>(g, A, W, stream) : launch_grouped_gemm_bm<__nv_bfloat16, 2, false>(g, A, W, stream);
+  return swiglu ? launch_grouped_gemm_typed<true>(d, il, g, A, W, stream) : launch_grouped_gemm_typed<false>(d, il, g, A, W, stream);
 }
 
 }  // namespace bb

@@ -1,0 +1,259 @@
+// bb_moe.cu -- the two ends of a mixture-of-experts expert block around the grouped matmuls (bb_moe_route, bb_moe_combine).
+//
+// Routing (moe_route_kernel): slot s = t * k + j of a [T, k] top-k id table goes to expert ids[s]; rows are sorted by expert and,
+// within an expert, by slot, so the order is stable and independent of the grid.  One persistent launch, no workspace:
+//   * every CTA owns a contiguous slot range [s0, s1) and histograms ALL n = T * k ids in shared memory (E <= 256 counters; warp
+//     aggregation with match.any keeps a routing that sends every slot to one expert from serialising on one shared atomic).  It
+//     counts the ids before s0 separately, so it knows each expert's first sorted row and how many of its rows precede the range.
+//   * it then walks its range in chunks of one slot per thread: match.any ranks the slots of an expert inside a warp, per-warp
+//     counts in shared memory rank them across the warps of the chunk, and a running count per expert carries on to the next
+//     chunk.  The chunk's rows of x are copied with 16-byte vectors.
+//   * ids outside [0, E) are dropped (slot_rows[s] = -1); sorted rows offsets[E] .. n - 1 are not written.
+//   * PDL: griddepcontrol.wait before the first read of ids and x; launch_dependents after the copy.
+//
+// Combine (moe_combine_kernel): out[t, :] = sum_j w[t, j] * Y[slot_rows[t * k + j], :], accumulated in fp32 in j order and rounded
+// once; slots whose row is outside [0, T * k) add nothing.  One thread per 8 output elements, no atomics: deterministic.
+#include <algorithm>
+#include <type_traits>
+
+#include "bb_common.cuh"
+
+namespace bb {
+
+namespace {
+
+constexpr int ROUTE_THREADS = 256;
+constexpr int ROUTE_WARPS = ROUTE_THREADS / 32;
+constexpr int ROUTE_MIN_SLOTS = 8;   // slots per CTA below which more CTAs only repeat the histogram
+constexpr int ROUTE_CTAS_PER_SM = 2;  // every CTA reads all T * k ids: more CTAs than this per SM cost more than their copy gains
+
+struct RouteParams {
+  const int32_t* ids;
+  const uint4* x;       // [T, K / 8] 16-byte vectors
+  int32_t* offsets;     // [E + 1]
+  int32_t* slot_rows;   // [n]
+  uint4* x_sorted;      // [n, K / 8]
+  int n, k, E, vecs;    // slots, top-k, experts, 16-byte vectors per row
+};
+
+__device__ __forceinline__ int route_expert(const RouteParams& r, long long s) {
+  if (s >= r.n) return -1;
+  const int e = r.ids[s];
+  return (e >= 0 && e < r.E) ? e : -1;
+}
+
+__global__ void __launch_bounds__(ROUTE_THREADS) moe_route_kernel(const RouteParams r) {
+  __shared__ int cnt_s[BB_GROUPED_MAX_GROUPS];      // slots of each expert (all n)
+  __shared__ int run_s[BB_GROUPED_MAX_GROUPS];      // first sorted row of each expert's next slot in this CTA
+  __shared__ int warp_s[ROUTE_WARPS][BB_GROUPED_MAX_GROUPS];   // slots of each expert per warp of the current chunk
+  __shared__ int dst_s[ROUTE_THREADS];              // sorted row of each slot of the chunk (-1: dropped)
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const unsigned lt = (1u << lane) - 1u;
+  int s0, s1;
+  {
+    const int base = r.n / gridDim.x, rem = r.n % gridDim.x, b = blockIdx.x;
+    s0 = b * base + min(b, rem);
+    s1 = s0 + base + (b < rem ? 1 : 0);
+  }
+  for (int e = tid; e < BB_GROUPED_MAX_GROUPS; e += ROUTE_THREADS) {
+    cnt_s[e] = 0;
+    run_s[e] = 0;
+    for (int w = 0; w < ROUTE_WARPS; ++w) warp_s[w][e] = 0;
+  }
+  __syncthreads();
+  pdl_wait();   // ids and x are the preceding kernels' output
+
+  // histogram: all slots into cnt_s, the slots before s0 into run_s
+  for (long long base = 0; base < r.n; base += ROUTE_THREADS) {
+    const long long s = base + tid;
+    const int e = route_expert(r, s);
+    const unsigned peers = __match_any_sync(0xffffffffu, e);
+    if (e >= 0 && (peers & lt) == 0) atomicAdd(&cnt_s[e], __popc(peers));
+    if (base < s0) {
+      const int eb = s < s0 ? e : -1;
+      const unsigned pb = __match_any_sync(0xffffffffu, eb);
+      if (eb >= 0 && (pb & lt) == 0) atomicAdd(&run_s[eb], __popc(pb));
+    }
+  }
+  __syncthreads();
+  // exclusive prefix sum of the counts by warp 0 (8 consecutive experts per lane): offsets, and run_s += each expert's start
+  if (warp == 0) {
+    constexpr int PER = BB_GROUPED_MAX_GROUPS / 32;
+    int c[PER], sum = 0;
+#pragma unroll
+    for (int i = 0; i < PER; ++i) {
+      const int e = lane * PER + i;
+      c[i] = e < r.E ? cnt_s[e] : 0;
+      sum += c[i];
+    }
+    int incl = sum;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= d) incl += v;
+    }
+    int start = incl - sum;
+#pragma unroll
+    for (int i = 0; i < PER; ++i) {
+      const int e = lane * PER + i;
+      if (e < r.E) {
+        if (blockIdx.x == 0) r.offsets[e] = start;
+        run_s[e] += start;
+      }
+      start += c[i];
+    }
+    if (blockIdx.x == 0 && lane == 31) r.offsets[r.E] = incl;
+  }
+  __syncthreads();
+
+  for (long long c0 = s0; c0 < s1; c0 += ROUTE_THREADS) {
+    const long long s = c0 + tid;
+    const int e = s < s1 ? route_expert(r, s) : -1;
+    const unsigned peers = __match_any_sync(0xffffffffu, e);
+    const bool leader = e >= 0 && (peers & lt) == 0;
+    if (leader) warp_s[warp][e] = __popc(peers);
+    __syncthreads();
+    int row = -1;
+    if (e >= 0) {
+      row = run_s[e] + __popc(peers & lt);
+      for (int w = 0; w < warp; ++w) row += warp_s[w][e];
+    }
+    if (s < s1) r.slot_rows[s] = row;
+    dst_s[tid] = row;
+    __syncthreads();
+    if (leader) {
+      atomicAdd(&run_s[e], __popc(peers));
+      warp_s[warp][e] = 0;
+    }
+    // copy the chunk's rows: x[s / k] -> x_sorted[row]
+    const int len = int(min((long long)ROUTE_THREADS, s1 - c0));
+    const long long total = (long long)len * r.vecs;
+    for (long long idx = tid; idx < total; idx += ROUTE_THREADS) {
+      const int i = int(idx / r.vecs), v = int(idx - (long long)i * r.vecs);
+      const int dst = dst_s[i];
+      if (dst >= 0) r.x_sorted[size_t(dst) * r.vecs + v] = r.x[size_t((c0 + i) / r.k) * r.vecs + v];
+    }
+    __syncthreads();   // run_s, warp_s and dst_s are final for the next chunk
+  }
+  pdl_launch_dependents();
+}
+
+struct CombineParams {
+  const int32_t* slot_rows;   // [T * k]
+  const float* w;             // [T * k]
+  const void* Y;              // [T * k, N]
+  void* out;                  // [T, N]
+  int k, cols8;               // top-k, N / 8
+  long long T, n;             // tokens, slots = T * k
+  int out_dtype;
+};
+
+template <typename OT>
+__device__ __forceinline__ void load8(const void* base, size_t elem, float (&v)[8]) {
+  if constexpr (std::is_same<OT, float>::value) {
+    const float4* p = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(base) + elem);
+    const float4 a = p[0], b = p[1];
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+  } else {
+    const uint4 q = *reinterpret_cast<const uint4*>(reinterpret_cast<const OT*>(base) + elem);
+    const OT* h = reinterpret_cast<const OT*>(&q);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) v[i] = TypeTraits<OT>::to_float(h[i]);
+  }
+}
+
+template <typename OT>
+__device__ __forceinline__ void store8(void* base, size_t elem, const float (&v)[8]) {
+  if constexpr (std::is_same<OT, float>::value) {
+    float4* p = reinterpret_cast<float4*>(reinterpret_cast<float*>(base) + elem);
+    p[0] = make_float4(v[0], v[1], v[2], v[3]);
+    p[1] = make_float4(v[4], v[5], v[6], v[7]);
+  } else {
+    uint4 q;
+    OT* h = reinterpret_cast<OT*>(&q);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) h[i] = TypeTraits<OT>::from_float(v[i]);
+    *reinterpret_cast<uint4*>(reinterpret_cast<OT*>(base) + elem) = q;
+  }
+}
+
+template <typename OT>
+__global__ void __launch_bounds__(256) moe_combine_kernel(const CombineParams c) {
+  pdl_wait();   // Y is the preceding kernel's output
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx < c.T * c.cols8) {
+    const long long t = idx / c.cols8;
+    const int col = int(idx - t * c.cols8) * 8;
+    const size_t N = size_t(c.cols8) * 8;
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int j = 0; j < c.k; ++j) {
+      const long long s = t * c.k + j;
+      const int row = c.slot_rows[s];
+      if (row < 0 || row >= c.n) continue;
+      const float w = c.w[s];
+      float y[8];
+      load8<OT>(c.Y, size_t(row) * N + col, y);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[i] = fmaf(w, y[i], acc[i]);
+    }
+    store8<OT>(c.out, size_t(t) * N + col, acc);
+  }
+  pdl_launch_dependents();
+}
+
+cudaLaunchAttribute pdl_attr() {
+  cudaLaunchAttribute a;
+  a.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  a.val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+  return a;
+}
+
+}  // namespace
+
+int launch_moe_route(const int32_t* topk_ids, int n_slots, int top_k, int num_experts, const void* x, int K, int32_t* offsets,
+                     int32_t* slot_rows, void* x_sorted, cudaStream_t stream) {
+  static int resident_per_sm[BB_MAX_DEVICES] = {};
+  const int dev = current_device();
+  if (!resident_per_sm[dev]) {
+    int occ = 0;
+    BB_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, moe_route_kernel, ROUTE_THREADS, 0));
+    if (occ <= 0) { set_error("moe route: the kernel cannot be resident on this device"); return 2; }
+    resident_per_sm[dev] = std::min(occ, ROUTE_CTAS_PER_SM);
+  }
+  RouteParams r;
+  r.ids = topk_ids; r.x = reinterpret_cast<const uint4*>(x); r.offsets = offsets; r.slot_rows = slot_rows;
+  r.x_sorted = reinterpret_cast<uint4*>(x_sorted); r.n = n_slots; r.k = top_k; r.E = num_experts; r.vecs = K / 8;
+  const int resident = resident_per_sm[dev] * device_sm_count();
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(std::max(1, std::min((n_slots + ROUTE_MIN_SLOTS - 1) / ROUTE_MIN_SLOTS, resident)));
+  cfg.blockDim = dim3(ROUTE_THREADS);
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1] = {pdl_attr()};
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, moe_route_kernel, r));
+  BB_LAUNCH_CHECK();
+  return 0;
+}
+
+int launch_moe_combine(const int32_t* slot_rows, const float* topk_weights, const void* Y, int out_dtype, void* out,
+                       int num_tokens, int top_k, int N, cudaStream_t stream) {
+  CombineParams c;
+  c.slot_rows = slot_rows; c.w = topk_weights; c.Y = Y; c.out = out; c.k = top_k; c.cols8 = N / 8;
+  c.T = num_tokens; c.n = (long long)num_tokens * top_k; c.out_dtype = out_dtype;
+  const long long threads = c.T * c.cols8;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(unsigned((threads + 255) / 256));
+  cfg.blockDim = dim3(256);
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1] = {pdl_attr()};
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  if (out_dtype == BB_F16) BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, moe_combine_kernel<__half>, c));
+  else if (out_dtype == BB_BF16) BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, moe_combine_kernel<__nv_bfloat16>, c));
+  else BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, moe_combine_kernel<float>, c));
+  BB_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // namespace bb

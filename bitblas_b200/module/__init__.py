@@ -240,7 +240,8 @@ class GroupedLinear(nn.Module):
     (``Matmul.forward_grouped``).  Constructor arguments after ``num_groups`` are those of ``Linear``; the buffers are
     ``Linear``'s stacked over the experts: ``qweight`` [E, N, K*bits/8], ``scales`` [E, N, K/g], ``zeros`` [E, N, K/g] (or
     [E, K/g, N*bits/8] for ``zeros_mode="quantized"``) and ``bias`` [E, N].  ``forward(A, offsets)`` takes the activations sorted
-    by expert and the int32 device row offsets [E + 1]; routing, top-k weighting and combining stay with the caller."""
+    by expert and the int32 device row offsets [E + 1]; routing, top-k weighting and combining stay with the caller (``MoEExperts``
+    runs the whole SwiGLU expert block)."""
 
     def __init__(self, num_groups: int, in_features: int, out_features: int, bias: bool = False, **linear_kwargs):
         super().__init__()

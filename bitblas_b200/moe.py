@@ -1,0 +1,209 @@
+"""Mixture-of-experts expert block: device routing (bb_moe_route), the gate/up interleave that the SwiGLU grouped calls read, the
+weighted top-k combine (bb_moe_combine), and ``MoEExperts``, which runs router output to layer output in four library launches.
+
+Gate/up interleave (include/bitblas_b200.h): the fused gate/up projection of I rows each is stored as 2I rows in which stored row
+16b + i is gate row 8b + i for i < 8 and up row 8b + i - 8 for i >= 8.  Every per-row buffer follows the same permutation:
+the weight, scales and zeros ([.., 2I, *]) and the bias ([.., 2I]) along their row axis; quantized zeros ([.., G, 2I*bits/8],
+packed along the rows) in whole bytes, 8 rows being `bits` bytes.
+"""
+from __future__ import annotations
+
+import torch
+import torch.nn as nn
+
+from . import _lib
+
+INTERLEAVE_ROWS = 8
+# kind -> (axis holding the rows, rows per element along it: None = 1, "bits" = 8 / bits packed rows per byte)
+_KINDS = {"weight": (-2, None), "scale": (-2, None), "zeros": (-2, None), "bias": (-1, None), "qzeros": (-1, "bits")}
+
+
+def _block(kind, bits):
+    if kind not in _KINDS:
+        raise ValueError(f"kind must be one of {sorted(_KINDS)} (got {kind!r})")
+    dim, packed = _KINDS[kind]
+    if packed is None:
+        return dim, INTERLEAVE_ROWS
+    if bits not in (2, 4):
+        raise ValueError("quantized zeros need bits = 4 or 2 (8 rows are `bits` whole bytes)")
+    return dim, INTERLEAVE_ROWS * bits // 8
+
+
+def interleave_gate_up(gate: torch.Tensor, up: torch.Tensor, kind: str, bits: int = None) -> torch.Tensor:
+    """gate, up [.., I, ..] (the rows on the axis of `kind`) -> the stored [.., 2I, ..] of the gate/up interleave.  kind: "weight",
+    "scale", "zeros", "bias", or "qzeros" (quantized zeros packed along the rows; needs `bits`).  CPU or CUDA tensors."""
+    dim, blk = _block(kind, bits)
+    if gate.shape != up.shape:
+        raise ValueError(f"gate and up must have the same shape (got {tuple(gate.shape)} and {tuple(up.shape)})")
+    n = gate.shape[dim]
+    if n % blk:
+        raise ValueError(f"the {kind} row axis ({n}) must be a multiple of {blk}: the interleave moves blocks of 8 rows")
+    g, u = gate.movedim(dim, -1), up.movedim(dim, -1)
+    lead = g.shape[:-1]
+    out = torch.stack([g.reshape(*lead, n // blk, blk), u.reshape(*lead, n // blk, blk)], dim=-2).reshape(*lead, 2 * n)
+    return out.movedim(-1, dim).contiguous()
+
+
+def deinterleave_gate_up(fused: torch.Tensor, kind: str, bits: int = None):
+    """the inverse of interleave_gate_up: stored [.., 2I, ..] -> (gate, up)"""
+    dim, blk = _block(kind, bits)
+    n2 = fused.shape[dim]
+    if n2 % (2 * blk):
+        raise ValueError(f"the {kind} row axis ({n2}) must be a multiple of {2 * blk}")
+    f = fused.movedim(dim, -1)
+    lead = f.shape[:-1]
+    pairs = f.reshape(*lead, n2 // (2 * blk), 2, blk)
+    gate = pairs[..., 0, :].reshape(*lead, n2 // 2).movedim(-1, dim).contiguous()
+    up = pairs[..., 1, :].reshape(*lead, n2 // 2).movedim(-1, dim).contiguous()
+    return gate, up
+
+
+def _device_ready(t: torch.Tensor):
+    dev = t.device
+    idx = dev.index if dev.index is not None else torch.cuda.current_device()
+    if idx not in _lib._inited:
+        _lib.ensure_init(idx)
+    return dev, torch.cuda.current_stream(dev).cuda_stream
+
+
+def _check(t, name, dtype, dim):
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"{name} must be a torch.Tensor")
+    if t.dtype != dtype or t.dim() != dim:
+        raise TypeError(f"{name} must be a {dim}-D {dtype} tensor (got {t.dim()}-D {t.dtype})")
+    if not t.is_cuda:
+        raise RuntimeError(f"{name} must be a CUDA tensor: bitblas_b200 has no CPU path")
+    if not t.is_contiguous():
+        raise ValueError(f"{name} must be contiguous")
+
+
+def moe_route(topk_ids: torch.Tensor, x: torch.Tensor, num_experts: int):
+    """Route the tokens of x [T, K] (fp16 / bf16) by topk_ids (int32 [T, k]) on the device, in one launch (bb_moe_route).
+    Returns (offsets int32 [E + 1], slot_rows int32 [T*k], x_sorted [T*k, K]): slot t*k + j goes to sorted row slot_rows[t*k + j]
+    of expert topk_ids[t, j]; rows are ordered by expert, then by slot.  Ids outside [0, E) are dropped (slot_rows = -1) and
+    x_sorted rows offsets[E] .. T*k - 1 are left unwritten."""
+    _check(topk_ids, "topk_ids", torch.int32, 2)
+    if not isinstance(x, torch.Tensor) or x.dtype not in (torch.float16, torch.bfloat16):
+        raise TypeError("x must be a float16 or bfloat16 torch.Tensor")
+    _check(x, "x", x.dtype, 2)
+    T, k = topk_ids.shape
+    if x.shape[0] != T:
+        raise ValueError(f"x has {x.shape[0]} rows, topk_ids {T}")
+    if x.device != topk_ids.device:
+        raise ValueError("x and topk_ids must be on the same device")
+    dev, stream = _device_ready(x)
+    E, K = int(num_experts), x.shape[1]
+    offsets = torch.empty(max(E, 0) + 1, dtype=torch.int32, device=dev)
+    slot_rows = torch.empty(T * k, dtype=torch.int32, device=dev)
+    x_sorted = torch.empty((T * k, K), dtype=x.dtype, device=dev)
+    with torch.cuda.device(dev):
+        rc = _lib.load().bb_moe_route(topk_ids.data_ptr(), T, k, E, x.data_ptr(), _lib.DTYPE_IDS[str(x.dtype)[6:]], K,
+                                      offsets.data_ptr(), slot_rows.data_ptr(), x_sorted.data_ptr(), stream)
+    _lib.check(rc, "bb_moe_route")
+    return offsets, slot_rows, x_sorted
+
+
+def moe_combine(y_sorted: torch.Tensor, slot_rows: torch.Tensor, topk_weights: torch.Tensor, output: torch.Tensor = None):
+    """out[t] = sum_j topk_weights[t, j] * y_sorted[slot_rows[t*k + j]] in one launch (bb_moe_combine): fp32 accumulation in j
+    order, one rounding to y_sorted's dtype (fp16 / bf16 / fp32); dropped slots add nothing.  y_sorted [T*k, N], slot_rows
+    int32 [T*k], topk_weights float32 [T, k]; returns [T, N]."""
+    if not isinstance(y_sorted, torch.Tensor) or y_sorted.dtype not in (torch.float16, torch.bfloat16, torch.float32):
+        raise TypeError("y_sorted must be a float16, bfloat16 or float32 torch.Tensor")
+    _check(y_sorted, "y_sorted", y_sorted.dtype, 2)
+    _check(topk_weights, "topk_weights", torch.float32, 2)
+    _check(slot_rows, "slot_rows", torch.int32, 1)
+    T, k = topk_weights.shape
+    N = y_sorted.shape[1]
+    if slot_rows.numel() != T * k or y_sorted.shape[0] != T * k:
+        raise ValueError(f"slot_rows and y_sorted need T*k = {T * k} rows (got {slot_rows.numel()} and {y_sorted.shape[0]})")
+    if not (y_sorted.device == slot_rows.device == topk_weights.device):
+        raise ValueError("y_sorted, slot_rows and topk_weights must be on the same device")
+    dev, stream = _device_ready(y_sorted)
+    if output is None:
+        output = torch.empty((T, N), dtype=y_sorted.dtype, device=dev)
+    else:
+        _check(output, "output", y_sorted.dtype, 2)
+        if tuple(output.shape) != (T, N) or output.device != dev:
+            raise ValueError(f"output must be [T={T}, N={N}] on {dev}")
+    with torch.cuda.device(dev):
+        rc = _lib.load().bb_moe_combine(slot_rows.data_ptr(), topk_weights.data_ptr(), y_sorted.data_ptr(),
+                                        _lib.DTYPE_IDS[str(y_sorted.dtype)[6:]], output.data_ptr(), T, k, N, stream)
+    _lib.check(rc, "bb_moe_combine")
+    return output
+
+
+class MoEExperts(nn.Module):
+    """The expert block of a SwiGLU mixture-of-experts layer, from router output to layer output:
+    ``y[t] = sum_j w[t, j] * down_e(silu(gate_e(x[t])) * up_e(x[t]))`` with e = topk_ids[t, j], as four library launches with no
+    host synchronisation (CUDA-graph capturable): moe_route -> grouped gate/up with SwiGLU in the epilogue -> grouped down ->
+    moe_combine.  ``gate_up`` (H -> 2I, gate/up interleaved) and ``down`` (I -> H) are ``GroupedLinear``s built from the
+    ``Linear`` keyword arguments; ``out_dtype`` must equal ``A_dtype`` (the gate/up output is the down projection's input)."""
+
+    def __init__(self, num_experts: int, hidden_size: int, intermediate_size: int, bias: bool = False, **linear_kwargs):
+        super().__init__()
+        from .module import GroupedLinear
+        if intermediate_size % INTERLEAVE_ROWS:
+            raise ValueError(f"intermediate_size must be a multiple of {INTERLEAVE_ROWS} (gate/up interleave; got {intermediate_size})")
+        a_dtype = linear_kwargs.get("A_dtype", "float16")
+        if linear_kwargs.get("out_dtype", "float16") != a_dtype:
+            raise ValueError("MoEExperts needs out_dtype == A_dtype: the gate/up output is the down projection's input")
+        self.num_experts, self.hidden_size, self.intermediate_size = int(num_experts), hidden_size, intermediate_size
+        self.gate_up = GroupedLinear(num_experts, hidden_size, 2 * intermediate_size, bias=bias, **linear_kwargs)
+        self.down = GroupedLinear(num_experts, intermediate_size, hidden_size, bias=bias, **linear_kwargs)
+        self.gate_up.bitblas_matmul.check_grouped(self.num_experts, swiglu=True)
+        self._linear_kwargs = dict(linear_kwargs, bias=bias)
+
+    def forward(self, x: torch.Tensor, topk_ids: torch.Tensor, topk_weights: torch.Tensor, output: torch.Tensor = None):
+        """x [T, H], topk_ids int32 [T, k], topk_weights float32 [T, k] -> [T, H]"""
+        if x.dim() != 2 or x.shape[1] != self.hidden_size:
+            raise ValueError(f"x must be [T, H={self.hidden_size}], got {tuple(x.shape)}")
+        if tuple(topk_weights.shape) != tuple(topk_ids.shape):
+            raise ValueError("topk_ids and topk_weights must have the same [T, k] shape")
+        offsets, slot_rows, x_sorted = moe_route(topk_ids, x, self.num_experts)
+        gu, cfg = self.gate_up, self.gate_up.bitblas_matmul.config
+        h = gu.bitblas_matmul.forward_grouped_swiglu(x_sorted, gu.qweight, offsets, gu.scales if cfg.with_scaling else None,
+                                                     gu.zeros if cfg.with_zeros else None, gu.bias)
+        y = self.down(h, offsets, capturable=True)
+        return moe_combine(y, slot_rows, topk_weights, output)
+
+    # ---- loading -----------------------------------------------------------------------------------------------------------
+    def _zeros_kind(self):
+        return "qzeros" if self.gate_up.bitblas_matmul.config.zeros_mode == "quantized" else "zeros"
+
+    def load_and_transform_weight(self, gate, up, down):
+        """gate, up, down: (weight, scales, zeros, bias) per projection, each stacked over the experts as
+        GroupedLinear.load_and_transform_weight takes it (None where the config has none; missing trailing entries are None).
+        gate / up are interleaved into gate_up before the storage transform (which works row by row)."""
+        g, u = (tuple(gate) + (None,) * 4)[:4], (tuple(up) + (None,) * 4)[:4]
+        kinds = ("weight", "scale", self._zeros_kind(), "bias")
+        fused = [None if a is None else interleave_gate_up(a, b, kind, self.gate_up.bits) for a, b, kind in zip(g, u, kinds)]
+        self.gate_up.load_and_transform_weight(*fused)
+        self.down.load_and_transform_weight(*down)
+
+    def _repack(self, gate_modules, up_modules, down_modules, device, v2):
+        from .module import GroupedLinear
+        kw = dict(self._linear_kwargs)
+        bias = kw.pop("bias")
+        halves = []
+        for mods in (gate_modules, up_modules):
+            half = GroupedLinear(self.num_experts, self.hidden_size, self.intermediate_size, bias=bias, **kw)
+            half._repack(mods, device, v2)
+            halves.append(half)
+        g, u = halves
+        gu = self.gate_up
+        gu.qweight = interleave_gate_up(g.qweight, u.qweight, "weight")
+        gu.scales = interleave_gate_up(g.scales, u.scales, "scale")
+        gu.zeros = interleave_gate_up(g.zeros, u.zeros, self._zeros_kind(), gu.bits)
+        if gu.bias is not None:
+            gu.bias = interleave_gate_up(g.bias, u.bias, "bias")
+        self.down._repack(down_modules, device, v2)
+
+    def repack_from_gptq(self, gate_modules, up_modules, down_modules, device="cuda"):
+        """one GPTQ QuantLinear per expert and projection: GroupedLinear's repack of gate and up, then the interleave"""
+        self._repack(gate_modules, up_modules, down_modules, device, v2=False)
+
+    def repack_from_gptq_v2(self, gate_modules, up_modules, down_modules, device="cuda"):
+        self._repack(gate_modules, up_modules, down_modules, device, v2=True)
+
+
+__all__ = ["MoEExperts", "moe_route", "moe_combine", "interleave_gate_up", "deinterleave_gate_up"]

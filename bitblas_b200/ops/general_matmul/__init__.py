@@ -515,14 +515,15 @@ class Matmul(Operator):
             raise RuntimeError(f"bb_matmul_scatter failed (code {rc}): {_lib.last_error()}")
 
     # ---- grouped (mixture-of-experts) forward -----------------------------------------------------------------------------
-    def check_grouped(self, num_groups: int) -> None:
-        """raise ValueError unless bb_matmul_grouped covers this operator's config with `num_groups` groups (validated by the
-        library with total_rows = 0: nothing touches the device)."""
+    def check_grouped(self, num_groups: int, swiglu: bool = False) -> None:
+        """raise ValueError unless bb_matmul_grouped (swiglu: bb_matmul_grouped_swiglu) covers this operator's config with
+        `num_groups` groups (validated by the library with total_rows = 0: nothing touches the device)."""
         if self.consistent:
             raise ValueError("the grouped matmul needs a low-bit weight operator (A_dtype != W_dtype)")
-        rc = self.lib._c.bb_matmul_grouped(self._desc_ref, int(num_groups), 0, 0, 0, 0, 0, 0, 0, 0, 0)
+        name = "bb_matmul_grouped_swiglu" if swiglu else "bb_matmul_grouped"
+        rc = getattr(self.lib._c, name)(self._desc_ref, int(num_groups), 0, 0, 0, 0, 0, 0, 0, 0, 0)
         if rc != 0:
-            raise ValueError(f"bb_matmul_grouped does not cover this configuration: {_lib.last_error()}")
+            raise ValueError(f"{name} does not cover this configuration: {_lib.last_error()}")
 
     def _check_grouped_params(self, E, W, scale, zeros, bias):
         """stacked parameter tensors: W [E, N, K*bits/8], scale [E, N, K/g], zeros [E, N, K/g] ([E, K/g, N*bits/8] quantized),
@@ -563,6 +564,45 @@ class Matmul(Operator):
         numerics of bb_matmul on the wgmma GEMM) where it covers the config (N % 128 == 0), and bb_matmul_grouped otherwise."""
         if self.consistent:
             raise NotImplementedError("forward_grouped needs a low-bit weight operator")
+        E, T, ptrs, output, dev, stream = self._grouped_prepare(A, W, offsets, scale, zeros, bias, output, self.config.N)
+        with torch.cuda.device(dev):   # the kernels launch on the calling thread's current device
+            if T <= GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E or capturable:
+                name = "bb_matmul_grouped" if self._grouped_single_launch(T, E) == "gemv" else "bb_matmul_grouped_gemm"
+                rc = getattr(self.lib._c, name)(self._desc_ref, E, offsets.data_ptr(), A.data_ptr(), *ptrs, output.data_ptr(),
+                                                T, stream)
+                if rc != 0:
+                    raise RuntimeError(f"{name} failed (code {rc}): {_lib.last_error()}")
+            else:
+                self._forward_grouped_per_group(A, W, offsets, scale, zeros, bias, output, dev, stream)
+        return output
+
+    def forward_grouped_swiglu(self, A, W, offsets, scale=None, zeros=None, bias=None, output=None):
+        """The gate/up projection of a SwiGLU mixture-of-experts block in ONE graph-capturable launch: this operator's N = 2I rows
+        hold gate and up in the gate/up interleave (bitblas_b200.moe.interleave_gate_up), and the output [T, I] is
+        silu(gate) * up, formed in the kernel epilogue from exactly the values forward_grouped(capturable=True) would store
+        (bb_matmul_grouped_swiglu / bb_matmul_grouped_gemm_swiglu, picked by the same rule).  Operands and offsets as in
+        forward_grouped."""
+        if self.consistent:
+            raise NotImplementedError("forward_grouped_swiglu needs a low-bit weight operator")
+        E, T, ptrs, output, dev, stream = self._grouped_prepare(A, W, offsets, scale, zeros, bias, output, self.config.N // 2,
+                                                                swiglu=True)
+        name = "bb_matmul_grouped_swiglu" if self._grouped_single_launch(T, E) == "gemv" else "bb_matmul_grouped_gemm_swiglu"
+        with torch.cuda.device(dev):
+            rc = getattr(self.lib._c, name)(self._desc_ref, E, offsets.data_ptr(), A.data_ptr(), *ptrs, output.data_ptr(), T,
+                                            stream)
+        if rc != 0:
+            raise RuntimeError(f"{name} failed (code {rc}): {_lib.last_error()}")
+        return output
+
+    def _grouped_single_launch(self, T: int, E: int) -> str:
+        """the kernel of the one capturable grouped launch for T rows over E groups: the grouped GEMV ("gemv") up to
+        GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E rows and where the grouped GEMM does not cover the config (N % 128 != 0),
+        the grouped wgmma GEMM ("gemm") above"""
+        return "gemm" if T > GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E and self._grouped_gemm_ok else "gemv"
+
+    def _grouped_prepare(self, A, W, offsets, scale, zeros, bias, output, out_cols, swiglu=False):
+        """argument checks of the grouped forwards (parameters once per distinct set); returns (E, T, parameter pointers, output
+        [T, out_cols], device, stream)"""
         c = self.config
         if not isinstance(offsets, torch.Tensor) or offsets.dtype != torch.int32:
             raise TypeError("offsets must be an int32 torch.Tensor of num_groups + 1 row offsets")
@@ -571,45 +611,30 @@ class Matmul(Operator):
                              f"(got shape {tuple(offsets.shape)})")
         E = offsets.numel() - 1
         key = (E, W.data_ptr(), scale.data_ptr() if scale is not None else 0, zeros.data_ptr() if zeros is not None else 0,
-               bias.data_ptr() if bias is not None else 0)
+               bias.data_ptr() if bias is not None else 0, swiglu)
         if key != self._grouped_checked_key:
             self._check_grouped_params(E, W, scale, zeros, bias)
-            self.check_grouped(E)
+            self.check_grouped(E, swiglu)
             self._grouped_gemm_ok = self.lib._c.bb_matmul_grouped_gemm(self._desc_ref, E, 0, 0, 0, 0, 0, 0, 0, 0, 0) == 0
             self._grouped_checked_key = key
         if not isinstance(A, torch.Tensor) or A.dim() != 2 or A.shape[1] != c.K:
             raise ValueError(f"A must be [T, K={c.K}], got {tuple(A.shape) if isinstance(A, torch.Tensor) else type(A)}")
         T = A.shape[0]
-        if output is not None and (not isinstance(output, torch.Tensor) or tuple(output.shape) != (T, c.N)):
-            raise ValueError(f"output must be [T={T}, N={c.N}]")
+        if output is not None and (not isinstance(output, torch.Tensor) or tuple(output.shape) != (T, out_cols)):
+            raise ValueError(f"output must be [T={T}, {out_cols}]")
         self._check_tensor(A, "A", self._torch_a_dtype)
         self._check_tensor(offsets, "offsets", torch.int32)
         if offsets.device != A.device or W.device != A.device:
             raise ValueError("A, W and offsets must be on the same device")
         dev = A.device
         if output is None:
-            output = torch.empty((T, c.N), dtype=self.torch_output_dtype, device=dev)
+            output = torch.empty((T, out_cols), dtype=self.torch_output_dtype, device=dev)
         else:
             self._check_tensor(output, "output", self.torch_output_dtype)
         idx = dev.index if dev.index is not None else torch.cuda.current_device()
         if idx not in _lib._inited:
             _lib.ensure_init(idx)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        ptrs = key[1:]
-        with torch.cuda.device(dev):   # the kernels launch on the calling thread's current device
-            if T <= GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E or (capturable and not self._grouped_gemm_ok):
-                rc = self.lib._c.bb_matmul_grouped(self._desc_ref, E, offsets.data_ptr(), A.data_ptr(), *ptrs,
-                                                   output.data_ptr(), T, stream)
-                if rc != 0:
-                    raise RuntimeError(f"bb_matmul_grouped failed (code {rc}): {_lib.last_error()}")
-            elif capturable:
-                rc = self.lib._c.bb_matmul_grouped_gemm(self._desc_ref, E, offsets.data_ptr(), A.data_ptr(), *ptrs,
-                                                        output.data_ptr(), T, stream)
-                if rc != 0:
-                    raise RuntimeError(f"bb_matmul_grouped_gemm failed (code {rc}): {_lib.last_error()}")
-            else:
-                self._forward_grouped_per_group(A, W, offsets, scale, zeros, bias, output, dev, stream)
-        return output
+        return E, T, key[1:5], output, dev, torch.cuda.current_stream(dev).cuda_stream
 
     def _forward_grouped_per_group(self, A, W, offsets, scale, zeros, bias, output, dev, stream):
         """prefill side of forward_grouped: one bb_matmul per non-empty group on its row slice, with the offsets clamped exactly as

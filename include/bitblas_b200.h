@@ -160,6 +160,38 @@ int bb_matmul_grouped(const bb_matmul_desc* desc, int num_groups, const int32_t*
 int bb_matmul_grouped_gemm(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
                            const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream);
 
+/* SwiGLU forms of the two grouped calls, for the gate/up projection of a mixture-of-experts expert block: the operands, offset
+ * contract, coverage and rejections of bb_matmul_grouped / bb_matmul_grouped_gemm, with desc->N = 2I fused gate/up rows stored in
+ * the "gate/up interleave": stored row 16b + i is gate row 8b + i for i < 8 and up row 8b + i - 8 for i >= 8 (so I % 8 == 0; the
+ * GEMM form also needs 2I % 128 == 0).  Scale, zeros and bias rows follow the same permutation (quantized zeros, packed along N,
+ * move in whole bytes: 8 rows are 4 bytes at 4 bits, 2 at 2 bits).  C is [total_rows, I]:
+ *     C[r, 8b + i] = round_out(silu(g) * u),   silu(g) = g / (1 + exp(-g)) in fp32, one rounding,
+ * where g and u are exactly what the plain call stores for the two rows (cast to out_dtype, bias added in out_dtype; fp32 output
+ * stays fp32).  The kernel instance is chosen from total_rows and num_groups exactly as in the plain calls. */
+int bb_matmul_grouped_swiglu(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                             const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream);
+int bb_matmul_grouped_gemm_swiglu(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                                  const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream);
+
+/* Mixture-of-experts routing on the device: slot s = t * top_k + j of the DEVICE int32 table topk_ids [num_tokens, top_k] goes to
+ * expert topk_ids[s].  Writes offsets [num_experts + 1] (the offsets of bb_matmul_grouped), slot_rows [T * top_k] (the sorted row
+ * of each slot) and x_sorted [T * top_k, K] with x_sorted[slot_rows[s]] = x[s / top_k].  Rows are ordered by expert and, within
+ * an expert, by slot: stable and deterministic.  Ids outside [0, num_experts) are dropped: slot_rows[s] = -1, and sorted rows
+ * offsets[num_experts] .. T * top_k - 1 are not written (the grouped calls, given total_rows = T * top_k, leave them unwritten
+ * too).  x is [num_tokens, K] of a_dtype (float16 | bfloat16), K % 8 == 0; 1 <= num_experts <= BB_GROUPED_MAX_GROUPS, top_k >= 1,
+ * T * top_k < 2^31.  ONE launch, no workspace, no host synchronisation (CUDA-graph capturable); programmatic stream serialization,
+ * nothing read before the preceding kernel has completed.  num_tokens == 0 validates and returns 0 without touching the device. */
+int bb_moe_route(const int32_t* topk_ids, int num_tokens, int top_k, int num_experts, const void* x, int a_dtype, int K,
+                 int32_t* offsets, int32_t* slot_rows, void* x_sorted, void* stream);
+
+/* Weighted top-k combine: out[t, :] = sum_j topk_weights[t, j] * Y[slot_rows[t * top_k + j], :], accumulated in fp32 over
+ * j = 0 .. top_k - 1 in that order and rounded once to out_dtype (float16 | bfloat16 | float32, also the type of Y [T * top_k, N]).
+ * Slots whose row is -1 or outside [0, T * top_k) add nothing; a token with no valid slot gets zeros.  No atomics: two runs are
+ * bit-identical.  N % 8 == 0; Y and out 16-byte aligned.  ONE launch with programmatic stream serialization, waiting for the
+ * preceding kernel first.  num_tokens == 0 validates and returns 0 without touching the device. */
+int bb_moe_combine(const int32_t* slot_rows, const float* topk_weights, const void* Y, int out_dtype, void* out, int num_tokens,
+                   int top_k, int N, void* stream);
+
 /* Cross-rank barrier for the column-parallel path (no reference counterpart): rank `rank` of `n_peers` signals every peer and
  * waits for all of them, on `stream`, as ONE small kernel -- ordered after the preceding kernels' peer stores (it is launched as a
  * programmatic dependent and waits for them), so after it every rank may read what bb_matmul_scatter calls issued before it wrote.

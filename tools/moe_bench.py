@@ -12,8 +12,10 @@ experts' weights and the active weight set does not stay in the 50 MB L2.  Devic
 Bytes: the active experts' weights, scales and zeros, plus activations and outputs; FLOP: 2 T N K.  The sweep times, for every
 shape up to a few thousand tokens, forward_grouped(capturable=True) (the grouped GEMV up to
 GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP rows per expert, the grouped wgmma GEMM above it) against both sides of the default
-forward_grouped: the single grouped GEMV launch and the per-group bb_matmul path.  The layer section times one prefill MoE layer
-(device routing, gate/up, SiLU gating, down) eager and replayed from one CUDA graph.
+forward_grouped: the single grouped GEMV launch and the per-group bb_matmul path.  The layer section times one MoE expert block
+from router output to layer output, MoEExperts.forward against the torch glue around the two grouped calls (both with the top-k
+weighted combine), eager and replayed from one CUDA graph, with the share of the device routing (bb_moe_route, which copies the
+x rows by expert) in the replayed block.
 """
 from __future__ import annotations
 
@@ -150,44 +152,71 @@ def point(layer, routes, iters, paths):
 
 
 def moe_layer(name, tokens, iters):
-    """one prefill MoE layer: routing on the device (top-k ids -> counts -> offsets, rows gathered by expert), gate/up, SiLU
-    gating, down; eager (default forward_grouped, and capturable=True) and as one CapturedStep replay (capturable=True)"""
+    """one MoE expert block, router output (top-k ids and weights) in, [T, H] layer output out: MoEExperts.forward (device routing,
+    gate/up with SwiGLU in the epilogue, down, weighted combine: 4 library launches) against the torch glue around the two grouped
+    calls (counts, cumsum, argsort, gather, slice + silu + mul, scatter of the slot rows, weighted sum), eager and as one CapturedStep
+    replay each"""
     m = MODELS[name]
     E, topk = m["E"], m["topk"]
-    (N1, K1), (N2, K2) = m["gate_up"], m["down"]
-    up, down = Layer(E, N1, K1, seed=3).gl, Layer(E, N2, K2, seed=4).gl
+    (N1, H), (_, I) = m["gate_up"], m["down"]
+    moe = bitblas.MoEExperts(E, H, I, **CFG).cuda()
+    for gl, seed in ((moe.gate_up, 3), (moe.down, 4)):
+        src = Layer(E, gl.out_features, gl.in_features, seed=seed).gl
+        gl.qweight, gl.scales, gl.zeros = src.qweight, src.scales, src.zeros
     g = torch.Generator(device="cuda").manual_seed(tokens)
-    x = (torch.rand((tokens, K1), device="cuda", generator=g) - 0.5).half()
-    ids = torch.rand((tokens, E), device="cuda", generator=g).argsort(dim=1)[:, :topk].reshape(-1)
+    x = (torch.rand((tokens, H), device="cuda", generator=g) - 0.5).half()
+    ids = torch.rand((tokens, E), device="cuda", generator=g).argsort(dim=1)[:, :topk].to(torch.int32).contiguous()
+    w = torch.softmax(torch.randn((tokens, topk), device="cuda", generator=g), dim=1)
     off = torch.zeros(E + 1, dtype=torch.int32, device="cuda")
+    out = torch.empty((tokens, H), dtype=torch.float16, device="cuda")
 
-    def fwd(capturable):
-        counts = torch.zeros(E, dtype=torch.int64, device="cuda").scatter_add_(0, ids, torch.ones_like(ids))
+    def glue():
+        flat = ids.reshape(-1).long()
+        counts = torch.zeros(E, dtype=torch.int64, device="cuda").scatter_add_(0, flat, torch.ones_like(flat))
         off[1:] = torch.cumsum(counts, 0).to(torch.int32)
-        rows = x[torch.argsort(ids, stable=True) // topk]
-        h = up(rows, off, capturable=capturable)
-        a = torch.nn.functional.silu(h[:, :K2]) * h[:, K2:]
-        return down(a.contiguous(), off, capturable=capturable)
+        order = torch.argsort(flat, stable=True)
+        h = moe.gate_up(x[order // topk], off, capturable=True).view(-1, I // 8, 2, 8)   # gate/up interleave
+        a = (torch.nn.functional.silu(h[:, :, 0]) * h[:, :, 1]).reshape(-1, I)
+        y = moe.down(a, off, capturable=True)
+        rows = torch.empty_like(order).scatter_(0, order, torch.arange(order.numel(), device="cuda"))
+        out.copy_((w[..., None] * y[rows].view(tokens, topk, H).float()).sum(1))
+        return out
 
-    def host_time(run, sync):
+    def fused():
+        return moe(x, ids, w, output=out)
+
+    def host_time(run, sync, n):
         for _ in range(3):
             run()
         sync()
         t0 = time.perf_counter()
-        for _ in range(iters):
+        for _ in range(n):
             run()
         sync()
-        return (time.perf_counter() - t0) / iters * 1e6
+        return (time.perf_counter() - t0) / n * 1e6
 
-    ref = fwd(False).clone()
-    step = bitblas.CapturedStep(lambda: fwd(True))
-    step()
-    res = dict(model=name, tokens=tokens, rows=tokens * topk,
-               eager_default_us=host_time(lambda: fwd(False), torch.cuda.synchronize),
-               eager_capturable_us=host_time(lambda: fwd(True), torch.cuda.synchronize),
-               graph_us=host_time(step.run, step.wait))
-    out = fwd(True)
-    res["max_abs_diff_vs_default"] = float((out.float() - ref.float()).abs().max())
+    def device_ops(fn):
+        try:
+            with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+                fn()
+                torch.cuda.synchronize()
+            return sum(1 for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA)
+        except Exception:   # the count is informative only
+            return -1
+
+    ref = glue().float().clone()
+    got = fused().float()
+    lib_launches = launches(lambda i: fused())
+    res = dict(model=name, tokens=tokens, rows=tokens * topk, launches_fused=lib_launches,
+               ops_fused=device_ops(fused), ops_glue=device_ops(glue),
+               max_abs_diff=float((got - ref).abs().max()), max_abs_ref=float(ref.abs().max()))
+    g_glue, g_fused = bitblas.CapturedStep(glue), bitblas.CapturedStep(fused)
+    for _ in range(2):    # alternate the two sides so drift on a shared host hits both
+        res["glue_eager_us"] = host_time(glue, torch.cuda.synchronize, iters)
+        res["fused_eager_us"] = host_time(fused, torch.cuda.synchronize, iters)
+        res["glue_graph_us"] = host_time(g_glue.run, g_glue.wait, iters)
+        res["fused_graph_us"] = host_time(g_fused.run, g_fused.wait, iters)
+    res["route_us"] = time_calls(lambda i: bitblas.moe.moe_route(ids, x, E), iters)
     return res
 
 
@@ -199,7 +228,7 @@ def main():
     ap.add_argument("--sweep-only", action="store_true")
     ap.add_argument("--no-sweep", action="store_true")
     ap.add_argument("--no-layer", action="store_true")
-    ap.add_argument("--layer-tokens", default="512,2048")
+    ap.add_argument("--layer-tokens", default="1,4,16,64,512,2048")
     ap.add_argument("--json", default=None, help="also write the results here")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "moe_bench measures on the GPU; there is no CPU fallback"
@@ -249,15 +278,18 @@ def main():
                 del layer
                 torch.cuda.empty_cache()
     if not args.no_layer:
-        print("\n# one prefill MoE layer (device routing, gate/up, SiLU gating, down): eager vs one CUDA-graph replay")
-        print(f"{'model':18s} {'tok':>5s} {'rows':>6s} | {'eager default us':>16s} {'eager capt us':>13s} {'graph us':>9s} | "
-              f"max |graph - default|")
+        print("\n# one MoE expert block (router output in, [T, H] out): MoEExperts.forward vs torch glue around the grouped calls")
+        print(f"{'model':18s} {'tok':>5s} {'rows':>6s} | {'glue eager':>10s} {'fused eager':>11s} {'glue graph':>10s} "
+              f"{'fused graph':>11s} {'graph x':>7s} | {'route us':>8s} {'share':>6s} | {'L':>2s} {'ops glue':>8s} {'ops fused':>9s} | "
+              f"max |fused - glue| (max |ref|)")
         for name in MODELS:
             for tok in map(int, args.layer_tokens.split(",")):
                 r = moe_layer(name, tok, max(5, min(args.iters, 20000 // tok)))
                 results.append(r)
-                print(f"{name:18s} {tok:5d} {r['rows']:6d} | {r['eager_default_us']:16.1f} {r['eager_capturable_us']:13.1f} "
-                      f"{r['graph_us']:9.1f} | {r['max_abs_diff_vs_default']:.3g}", flush=True)
+                print(f"{name:18s} {tok:5d} {r['rows']:6d} | {r['glue_eager_us']:10.1f} {r['fused_eager_us']:11.1f} "
+                      f"{r['glue_graph_us']:10.1f} {r['fused_graph_us']:11.1f} {r['glue_graph_us'] / r['fused_graph_us']:6.2f}x | "
+                      f"{r['route_us']:8.1f} {r['route_us'] / r['fused_graph_us']:6.1%} | {r['launches_fused']:2d} "
+                      f"{r['ops_glue']:8d} {r['ops_fused']:9d} | {r['max_abs_diff']:.3g} ({r['max_abs_ref']:.3g})", flush=True)
                 torch.cuda.empty_cache()
     if args.json:
         with open(args.json, "w") as f:
