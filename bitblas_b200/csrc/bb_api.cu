@@ -344,8 +344,22 @@ int bb_matmul_grouped_gemm_swiglu(const bb_matmul_desc* desc, int num_groups, co
   return launch_grouped_gemm(*desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows, (cudaStream_t)stream, true);
 }
 
-int bb_moe_route(const int32_t* topk_ids, int num_tokens, int top_k, int num_experts, const void* x, int a_dtype, int K,
-                 int32_t* offsets, int32_t* slot_rows, void* x_sorted, void* stream) {
+int bb_matmul_grouped_gemm_swiglu_gather(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets,
+                                         const int32_t* row_index, const void* A, int a_rows, const void* W, const void* scale,
+                                         const void* zeros, const void* bias, void* C, int total_rows, void* stream) {
+  if (validate(desc)) return 1;
+  if (!swiglu_shape_ok(desc) || !grouped_gemm_supported(*desc)) return 1;
+  const int rc = check_grouped_args(desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows);
+  if (rc) return rc < 0 ? 0 : rc;
+  if (!row_index) { set_error("gather: row_index must be a device pointer to total_rows int32 values"); return 1; }
+  if (a_rows < 1) { set_error("gather: a_rows must be >= 1 (got %d)", a_rows); return 1; }
+  if (reinterpret_cast<uintptr_t>(row_index) & 3) { set_error("gather: row_index must be 4-byte aligned"); return 5; }
+  return launch_grouped_gemm(*desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows, (cudaStream_t)stream, true,
+                             row_index, a_rows);
+}
+
+// the checks bb_moe_route and bb_moe_route_index share: 0 = valid
+static int check_route_args(int num_tokens, int top_k, int num_experts) {
   if (num_experts < 1 || num_experts > BB_GROUPED_MAX_GROUPS) {
     set_error("moe route: num_experts must be in [1, %d] (got %d)", BB_GROUPED_MAX_GROUPS, num_experts);
     return 1;
@@ -356,6 +370,12 @@ int bb_moe_route(const int32_t* topk_ids, int num_tokens, int top_k, int num_exp
     set_error("moe route: num_tokens * top_k must be below 2^31 (got %d x %d)", num_tokens, top_k);
     return 1;
   }
+  return 0;
+}
+
+int bb_moe_route(const int32_t* topk_ids, int num_tokens, int top_k, int num_experts, const void* x, int a_dtype, int K,
+                 int32_t* offsets, int32_t* slot_rows, void* x_sorted, void* stream) {
+  if (check_route_args(num_tokens, top_k, num_experts)) return 1;
   if (a_dtype != BB_F16 && a_dtype != BB_BF16) { set_error("moe route: x must be float16 or bfloat16 (a_dtype=%d)", a_dtype); return 1; }
   if (K <= 0 || K % 8) { set_error("moe route: needs K > 0 and K %% 8 == 0 (K=%d)", K); return 1; }
   if (num_tokens == 0) return 0;
@@ -366,7 +386,21 @@ int bb_moe_route(const int32_t* topk_ids, int num_tokens, int top_k, int num_exp
     set_error("moe route: x and x_sorted must be 16-byte aligned, the int32 arrays 4-byte aligned");
     return 5;
   }
-  return launch_moe_route(topk_ids, num_tokens * top_k, top_k, num_experts, x, K, offsets, slot_rows, x_sorted,
+  return launch_moe_route(topk_ids, num_tokens * top_k, top_k, num_experts, x, K, offsets, slot_rows, x_sorted, nullptr,
+                          (cudaStream_t)stream);
+}
+
+int bb_moe_route_index(const int32_t* topk_ids, int num_tokens, int top_k, int num_experts, int32_t* offsets,
+                       int32_t* slot_rows, int32_t* row_token, void* stream) {
+  if (check_route_args(num_tokens, top_k, num_experts)) return 1;
+  if (num_tokens == 0) return 0;
+  if (!topk_ids || !offsets || !slot_rows || !row_token) { set_error("moe route: every pointer must be non-null"); return 1; }
+  if ((reinterpret_cast<uintptr_t>(topk_ids) & 3) || (reinterpret_cast<uintptr_t>(offsets) & 3) ||
+      (reinterpret_cast<uintptr_t>(slot_rows) & 3) || (reinterpret_cast<uintptr_t>(row_token) & 3)) {
+    set_error("moe route: the int32 arrays must be 4-byte aligned");
+    return 5;
+  }
+  return launch_moe_route(topk_ids, num_tokens * top_k, top_k, num_experts, nullptr, 8, offsets, slot_rows, nullptr, row_token,
                           (cudaStream_t)stream);
 }
 

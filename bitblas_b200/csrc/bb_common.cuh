@@ -90,14 +90,16 @@ bool grouped_supported(const bb_matmul_desc& d);
 int launch_grouped(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
                    const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream,
                    bool swiglu = false);
-// grouped wgmma GEMM, bb_grouped_gemm.cu: the same operands and offset contract
+// grouped wgmma GEMM, bb_grouped_gemm.cu: the same operands and offset contract.  row_index (swiglu only): sorted row r reads
+// A[clamp(row_index[r], 0, a_rows - 1)] of A [a_rows, K] instead of A[r]
 bool grouped_gemm_supported(const bb_matmul_desc& d);
 int launch_grouped_gemm(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
                         const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream,
-                        bool swiglu = false);
-// mixture-of-experts routing and top-k combine, bb_moe.cu (arguments validated by the callers in bb_api.cu)
+                        bool swiglu = false, const int32_t* row_index = nullptr, int a_rows = 0);
+// mixture-of-experts routing and top-k combine, bb_moe.cu (arguments validated by the callers in bb_api.cu).  Routing copies x
+// into x_sorted, or, with x_sorted == nullptr, writes row_token instead (bb_moe_route_index)
 int launch_moe_route(const int32_t* topk_ids, int n_slots, int top_k, int num_experts, const void* x, int K, int32_t* offsets,
-                     int32_t* slot_rows, void* x_sorted, cudaStream_t stream);
+                     int32_t* slot_rows, void* x_sorted, int32_t* row_token, cudaStream_t stream);
 int launch_moe_combine(const int32_t* slot_rows, const float* topk_weights, const void* Y, int out_dtype, void* out,
                        int num_tokens, int top_k, int N, cudaStream_t stream);
 

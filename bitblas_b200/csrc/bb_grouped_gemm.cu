@@ -22,6 +22,16 @@
 //   * the offsets are untrusted, with bb_matmul_grouped's contract: clamped to [0, T], a group whose end is below its start is
 //     empty, and rows no group claims are not written.
 //   * SWIGLU instances (bb_matmul_grouped_gemm_swiglu): gate/up interleaved W, C [T, N / 2] = silu(gate) * up (store_tile).
+//   * GATHER instances (bb_matmul_grouped_gemm_swiglu_gather, SWIGLU only): sorted row r reads A[clamp(row_index[r], 0, a_rows - 1)]
+//     of A [a_rows, K], so a mixture-of-experts block reads its token rows in place instead of a routed copy.  Only the producer
+//     differs: TS_GATHER_WARPS producer warps (the launch has 3 more warps) copy the tile's rows with 16-byte cp.async, 8 lanes
+//     per 128-byte row, straight into the SW128 layout the consumers' descriptor reads (chunk c of row i at byte
+//     i * 128 + (c ^ (i & 7)) * 16 of the 1024-byte-aligned stage); each lane's cp.async.mbarrier.arrive and one arrival per
+//     producer warp join the stage's `full` barrier next to the weight TMA.  One TMA box {KB, 1} per row gives the same bits
+//     (TMA swizzles by the shared-memory address) but issues BM TMA operations per k-block and was slower still.  Rows past the
+//     expert's end are not copied (they are never stored, and a wgmma output column depends on its own activation row only).
+//     The consumers add one fence.proxy.async per stage: the cp.async writes are generic-proxy writes that wgmma reads through
+//     the async proxy.  tmA is not used (the launch passes tmW in its place).
 #include <algorithm>
 #include <climits>
 
@@ -37,7 +47,19 @@ struct GroupedTsParams {
   int E;                      // groups
   int T;                      // rows of A and C
   long long s_stride, z_stride, b_stride;   // bytes per group: scale, zeros, bias
+  const int32_t* row_index;   // [T], device (GATHER)
+  const void* a;              // A [a_rows, K] (GATHER)
+  int a_rows;
 };
+
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+// the mbarrier's phase also waits for this thread's earlier cp.async copies (net-zero on its pending count)
+__device__ __forceinline__ void cp_async_mbar_arrive(uint64_t* bar) {
+  asm volatile("cp.async.mbarrier.arrive.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // gemm_ts_kernel's epilogue for one destination and no split-K: acc[4i + 2h + j] = C^T[row rA + 8h][column 8i + 2t + j] ->
 // C[m, n] for the rows m < m_end, cast to out_dtype, then bias[e][n] added in out_dtype (fp32: in one sum), as bb_matmul rounds.
@@ -93,8 +115,15 @@ __device__ __forceinline__ void store_tile(const float (&acc)[BM / 2], const TsP
   }
 }
 
-template <typename T, int BITS, int BM, bool IL, bool SWIGLU = false>
-__global__ void __launch_bounds__(TS_THREADS, 1)
+// producer warps of the GATHER instances: one warp issuing the 16-byte copies left the gathering GEMM 1.8-3.8x slower than the
+// plain one, four bring it to 1.06-1.55x (H100 80GB HBM3, 700 W, tools/moe_bench.py shapes)
+constexpr int TS_GATHER_WARPS = 4;
+
+template <bool GATHER>
+constexpr int grouped_threads() { return TS_THREADS + (GATHER ? 32 * (TS_GATHER_WARPS - 1) : 0); }
+
+template <typename T, int BITS, int BM, bool IL, bool SWIGLU = false, bool GATHER = false>
+__global__ void __launch_bounds__(grouped_threads<GATHER>(), 1)
 gemm_ts_grouped_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                        const GroupedTsParams g) {
   using SM = TsSmem<T, BITS, BM>;
@@ -119,9 +148,10 @@ gemm_ts_grouped_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   const int n_tiles = p.N / TS_ROWS;
   const int num_kb = p.K / KB;
   if (warp == TS_CONSUMER_WARPS && lane == 0) {
-    tma_prefetch_desc(&tmA);
+    if constexpr (!GATHER) tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmW);
-    for (int i = 0; i < S; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], TS_CONSUMER_WARPS); }
+    // GATHER: `full` completes on one arrival per producer warp (plus the weight bytes and every lane's cp.async copies)
+    for (int i = 0; i < S; ++i) { mbar_init(&full[i], GATHER ? TS_GATHER_WARPS : 1); mbar_init(&empty[i], TS_CONSUMER_WARPS); }
     fence_barrier_init();
   }
   if (threadIdx.x < 32) grouped_schedule(g, BM, n_tiles, row0_s, rows_s, item0_s);
@@ -139,9 +169,49 @@ gemm_ts_grouped_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     n0 = nt * TS_ROWS;
   };
 
-  if (warp == TS_CONSUMER_WARPS) {
+  if (GATHER ? warp >= TS_CONSUMER_WARPS : warp == TS_CONSUMER_WARPS) {
     // ===== TMA producer: one continuous ring over all of this CTA's tiles =====
-    if (lane == 0) {
+    if constexpr (GATHER) {
+      // producer warp pw owns tile rows [pw * RW, (pw + 1) * RW): it reads their indices once per tile (only it uses them, so
+      // __syncwarp orders the reuse) and copies them every k-block, 8 lanes per 128-byte row
+      constexpr int RW = BM / TS_GATHER_WARPS;
+      __shared__ int src_s[BM];   // clamped source row of each tile row; -1 past the expert's end
+      const int pw = warp - TS_CONSUMER_WARPS;
+      int* const src_w = src_s + pw * RW;
+      const int c = lane & 7;     // the 16-byte chunk of a 128-byte row this lane copies
+      const T* a = reinterpret_cast<const T*>(g.a) + c * 8;
+      int s = 0, loads = 0;
+      uint32_t par = 1;
+      for (int item = blockIdx.x; item < total; item += gridDim.x) {
+        int e, m0, m_end, n0;
+        tile_of(item, e, m0, m_end, n0);
+        const int wrow = e * p.N + n0;
+        const int r0 = m0 + pw * RW;
+        __syncwarp();   // the previous tile's src_w reads are done
+        for (int i = lane; i < RW; i += 32) src_w[i] = r0 + i < m_end ? min(max(g.row_index[r0 + i], 0), g.a_rows - 1) : -1;
+        __syncwarp();
+        for (int kb = 0; kb < num_kb; ++kb, ++loads) {
+          if (loads >= S) mbar_wait(&empty[s], par);
+          const uint32_t dst = smem_u32(sA + s * SM::kActBytes) + uint32_t(c << 4);
+#pragma unroll
+          for (int i = lane >> 3; i < RW; i += 4) {
+            const int r = src_w[i], row = pw * RW + i;
+            if (r >= 0) cp_async16((dst + uint32_t(row * 128)) ^ uint32_t((row & 7) << 4), a + size_t(r) * p.K + kb * KB);
+          }
+          cp_async_mbar_arrive(&full[s]);
+          __syncwarp();   // every lane's tracking is registered before the warp's arrival can complete the phase
+          if (lane == 0) {
+            if (pw == 0) {
+              mbar_arrive_expect_tx(&full[s], SM::kWBytes);
+              tma_load_2d(sW + s * SM::kWBytes, &tmW, kb * PRB, wrow, &full[s]);
+            } else {
+              mbar_arrive(&full[s]);
+            }
+          }
+          if (++s == S) { s = 0; par ^= 1; }
+        }
+      }
+    } else if (lane == 0) {
       int s = 0, loads = 0;
       uint32_t par = 1;  // parity of the "previous use" of the stage: the first pass must not wait
       for (int item = blockIdx.x; item < total; item += gridDim.x) {
@@ -212,6 +282,7 @@ gemm_ts_grouped_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           }
         }
         mbar_wait(&full[st], full_par);
+        if constexpr (GATHER) fence_proxy_async_shared();
         const uint32_t wofs = uint32_t(st * SM::kWBytes);
         dequant_row<T, BITS, MODE, IL, 0>(srcA + wofs, t, fa, cA, lut4, false);
         dequant_row<T, BITS, MODE, IL, 0>(srcB + wofs, t, fb, cB, lut4, false);
@@ -256,32 +327,37 @@ gemm_ts_grouped_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   pdl_launch_dependents();
 }
 
-template <typename T, int BITS, int BM, bool IL, bool SWIGLU>
+template <typename T, int BITS, int BM, bool IL, bool SWIGLU, bool GATHER>
 int launch_grouped_gemm_inst(const GroupedTsParams& g, const void* A, const void* W, long long max_tiles, cudaStream_t stream) {
   using SM = TsSmem<T, BITS, BM>;
-  auto kernel = gemm_ts_grouped_kernel<T, BITS, BM, IL, SWIGLU>;
+  auto kernel = gemm_ts_grouped_kernel<T, BITS, BM, IL, SWIGLU, GATHER>;
+  constexpr int threads = grouped_threads<GATHER>();
   static int resident_per_sm[BB_MAX_DEVICES] = {};   // 0 until queried (cudaFuncSetAttribute is per device)
   const int dev = current_device();
   if (!resident_per_sm[dev]) {
     BB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kTotal));
     int occ = 0;
-    BB_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, TS_THREADS, SM::kTotal));
+    BB_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, SM::kTotal));
     if (occ <= 0) { set_error("grouped GEMM: the kernel cannot be resident on this device"); return 2; }
     resident_per_sm[dev] = occ;
   }
   CUtensorMap tmA, tmW;
   const CUtensorMapDataType adt = std::is_same<T, __half>::value ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   const TsParams& p = g.p;
-  int rc = make_map_2d(&tmA, adt, A, uint64_t(p.K), uint64_t(g.T), uint64_t(p.K) * sizeof(T), ElemInfo<T>::kKB, BM,
-                       CU_TENSOR_MAP_SWIZZLE_128B);
-  if (rc) return rc;
   const uint64_t wrow = uint64_t(p.K) * BITS / 8;
-  rc = make_map_2d(&tmW, CU_TENSOR_MAP_DATA_TYPE_UINT8, W, wrow, uint64_t(g.E) * uint64_t(p.N), wrow, SM::kPRB, TS_ROWS,
-                   CU_TENSOR_MAP_SWIZZLE_NONE);
+  int rc = make_map_2d(&tmW, CU_TENSOR_MAP_DATA_TYPE_UINT8, W, wrow, uint64_t(g.E) * uint64_t(p.N), wrow, SM::kPRB, TS_ROWS,
+                       CU_TENSOR_MAP_SWIZZLE_NONE);
   if (rc) return rc;
+  if constexpr (GATHER) {
+    tmA = tmW;   // the producer copies A with cp.async; the kernel never touches tmA
+  } else {
+    rc = make_map_2d(&tmA, adt, A, uint64_t(p.K), uint64_t(g.T), uint64_t(p.K) * sizeof(T), ElemInfo<T>::kKB, BM,
+                     CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+  }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(unsigned(std::min<long long>(max_tiles, (long long)resident_per_sm[dev] * device_sm_count())));
-  cfg.blockDim = dim3(TS_THREADS);
+  cfg.blockDim = dim3(threads);
   cfg.dynamicSmemBytes = SM::kTotal;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
@@ -294,7 +370,7 @@ int launch_grouped_gemm_inst(const GroupedTsParams& g, const void* A, const void
   return 0;
 }
 
-template <typename T, int BITS, bool IL, bool SWIGLU>
+template <typename T, int BITS, bool IL, bool SWIGLU, bool GATHER>
 int launch_grouped_gemm_bm(const GroupedTsParams& g, const void* A, const void* W, cudaStream_t stream) {
   // rows of A per tile from the mean rows per active group (T rows over at most min(E, T) groups), as launch_ts_bm picks BM
   // from m; tiles: sum_e ceil(m_e / BM) per n-tile <= ceil(T / BM) + (groups with rows)
@@ -302,20 +378,20 @@ int launch_grouped_gemm_bm(const GroupedTsParams& g, const void* A, const void* 
   const int mean_rows = (g.T + active - 1) / active;
   const int bm = mean_rows <= 32 ? 32 : (mean_rows <= 64 ? 64 : 128);
   const long long max_tiles = (long long)(g.p.N / TS_ROWS) * ((g.T + bm - 1) / bm + active);
-  if (bm == 32) return launch_grouped_gemm_inst<T, BITS, 32, IL, SWIGLU>(g, A, W, max_tiles, stream);
-  if (bm == 64) return launch_grouped_gemm_inst<T, BITS, 64, IL, SWIGLU>(g, A, W, max_tiles, stream);
-  return launch_grouped_gemm_inst<T, BITS, 128, IL, SWIGLU>(g, A, W, max_tiles, stream);
+  if (bm == 32) return launch_grouped_gemm_inst<T, BITS, 32, IL, SWIGLU, GATHER>(g, A, W, max_tiles, stream);
+  if (bm == 64) return launch_grouped_gemm_inst<T, BITS, 64, IL, SWIGLU, GATHER>(g, A, W, max_tiles, stream);
+  return launch_grouped_gemm_inst<T, BITS, 128, IL, SWIGLU, GATHER>(g, A, W, max_tiles, stream);
 }
 
-template <bool SWIGLU>
+template <bool SWIGLU, bool GATHER = false>
 int launch_grouped_gemm_typed(const bb_matmul_desc& d, bool il, const GroupedTsParams& g, const void* A, const void* W,
                               cudaStream_t s) {
   if (d.a_dtype == BB_F16) {
-    if (d.w_bits == 4) return il ? launch_grouped_gemm_bm<__half, 4, true, SWIGLU>(g, A, W, s) : launch_grouped_gemm_bm<__half, 4, false, SWIGLU>(g, A, W, s);
-    return il ? launch_grouped_gemm_bm<__half, 2, true, SWIGLU>(g, A, W, s) : launch_grouped_gemm_bm<__half, 2, false, SWIGLU>(g, A, W, s);
+    if (d.w_bits == 4) return il ? launch_grouped_gemm_bm<__half, 4, true, SWIGLU, GATHER>(g, A, W, s) : launch_grouped_gemm_bm<__half, 4, false, SWIGLU, GATHER>(g, A, W, s);
+    return il ? launch_grouped_gemm_bm<__half, 2, true, SWIGLU, GATHER>(g, A, W, s) : launch_grouped_gemm_bm<__half, 2, false, SWIGLU, GATHER>(g, A, W, s);
   }
-  if (d.w_bits == 4) return il ? launch_grouped_gemm_bm<__nv_bfloat16, 4, true, SWIGLU>(g, A, W, s) : launch_grouped_gemm_bm<__nv_bfloat16, 4, false, SWIGLU>(g, A, W, s);
-  return il ? launch_grouped_gemm_bm<__nv_bfloat16, 2, true, SWIGLU>(g, A, W, s) : launch_grouped_gemm_bm<__nv_bfloat16, 2, false, SWIGLU>(g, A, W, s);
+  if (d.w_bits == 4) return il ? launch_grouped_gemm_bm<__nv_bfloat16, 4, true, SWIGLU, GATHER>(g, A, W, s) : launch_grouped_gemm_bm<__nv_bfloat16, 4, false, SWIGLU, GATHER>(g, A, W, s);
+  return il ? launch_grouped_gemm_bm<__nv_bfloat16, 2, true, SWIGLU, GATHER>(g, A, W, s) : launch_grouped_gemm_bm<__nv_bfloat16, 2, false, SWIGLU, GATHER>(g, A, W, s);
 }
 
 }  // namespace
@@ -332,7 +408,7 @@ bool grouped_gemm_supported(const bb_matmul_desc& d) {
 
 int launch_grouped_gemm(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
                         const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream,
-                        bool swiglu) {
+                        bool swiglu, const int32_t* row_index, int a_rows) {
   MatmulArgs a = {};
   a.d = d; a.A = A; a.W = W; a.scale = scale; a.zeros = zeros; a.bias = bias; a.C = C; a.m = total_rows; a.n_peers = 0;
   GroupedTsParams g;
@@ -351,11 +427,13 @@ int launch_grouped_gemm(const bb_matmul_desc& d, int num_groups, const int32_t* 
   g.s_stride = N * G * 2;
   g.z_stride = d.zeros_mode == BB_ZEROS_QUANTIZED ? G * (N * d.w_bits / 8) : N * G * 2;
   g.b_stride = N * 2;
+  g.row_index = row_index; g.a = A; g.a_rows = a_rows;
   if ((N / TS_ROWS) * ((total_rows + 31) / 32 + std::min(num_groups, total_rows)) > INT_MAX) {
     set_error("grouped GEMM: N/128 x (T/32 + groups) exceeds 2^31 tiles");
     return 1;
   }
   const bool il = d.w_layout == BB_LAYOUT_INTERLEAVED_16;
+  if (row_index) return launch_grouped_gemm_typed<true, true>(d, il, g, A, W, stream);
   return swiglu ? launch_grouped_gemm_typed<true>(d, il, g, A, W, stream) : launch_grouped_gemm_typed<false>(d, il, g, A, W, stream);
 }
 

@@ -10,6 +10,8 @@
 //     chunk.  The chunk's rows of x are copied with 16-byte vectors.
 //   * ids outside [0, E) are dropped (slot_rows[s] = -1); sorted rows offsets[E] .. n - 1 are not written.
 //   * PDL: griddepcontrol.wait before the first read of ids and x; launch_dependents after the copy.
+//   * INDEX instance (bb_moe_route_index): the same offsets and slot_rows, but instead of copying x it writes the token of each
+//     sorted row, row_token[slot_rows[s]] = s / k, which the gathering grouped GEMM reads its A rows through.
 //
 // Combine (moe_combine_kernel): out[t, :] = sum_j w[t, j] * Y[slot_rows[t * k + j], :], accumulated in fp32 in j order and rounded
 // once; slots whose row is outside [0, T * k) add nothing.  One thread per 8 output elements, no atomics: deterministic.
@@ -34,6 +36,7 @@ struct RouteParams {
   int32_t* slot_rows;   // [n]
   uint4* x_sorted;      // [n, K / 8]
   int n, k, E, vecs;    // slots, top-k, experts, 16-byte vectors per row
+  int32_t* row_token;   // [n] (INDEX)
 };
 
 __device__ __forceinline__ int route_expert(const RouteParams& r, long long s) {
@@ -42,6 +45,7 @@ __device__ __forceinline__ int route_expert(const RouteParams& r, long long s) {
   return (e >= 0 && e < r.E) ? e : -1;
 }
 
+template <bool INDEX>
 __global__ void __launch_bounds__(ROUTE_THREADS) moe_route_kernel(const RouteParams r) {
   __shared__ int cnt_s[BB_GROUPED_MAX_GROUPS];      // slots of each expert (all n)
   __shared__ int run_s[BB_GROUPED_MAX_GROUPS];      // first sorted row of each expert's next slot in this CTA
@@ -119,19 +123,25 @@ __global__ void __launch_bounds__(ROUTE_THREADS) moe_route_kernel(const RoutePar
       for (int w = 0; w < warp; ++w) row += warp_s[w][e];
     }
     if (s < s1) r.slot_rows[s] = row;
-    dst_s[tid] = row;
+    if constexpr (INDEX) {
+      if (row >= 0) r.row_token[row] = int(s / r.k);
+    } else {
+      dst_s[tid] = row;
+    }
     __syncthreads();
     if (leader) {
       atomicAdd(&run_s[e], __popc(peers));
       warp_s[warp][e] = 0;
     }
-    // copy the chunk's rows: x[s / k] -> x_sorted[row]
-    const int len = int(min((long long)ROUTE_THREADS, s1 - c0));
-    const long long total = (long long)len * r.vecs;
-    for (long long idx = tid; idx < total; idx += ROUTE_THREADS) {
-      const int i = int(idx / r.vecs), v = int(idx - (long long)i * r.vecs);
-      const int dst = dst_s[i];
-      if (dst >= 0) r.x_sorted[size_t(dst) * r.vecs + v] = r.x[size_t((c0 + i) / r.k) * r.vecs + v];
+    if constexpr (!INDEX) {
+      // copy the chunk's rows: x[s / k] -> x_sorted[row]
+      const int len = int(min((long long)ROUTE_THREADS, s1 - c0));
+      const long long total = (long long)len * r.vecs;
+      for (long long idx = tid; idx < total; idx += ROUTE_THREADS) {
+        const int i = int(idx / r.vecs), v = int(idx - (long long)i * r.vecs);
+        const int dst = dst_s[i];
+        if (dst >= 0) r.x_sorted[size_t(dst) * r.vecs + v] = r.x[size_t((c0 + i) / r.k) * r.vecs + v];
+      }
     }
     __syncthreads();   // run_s, warp_s and dst_s are final for the next chunk
   }
@@ -210,20 +220,24 @@ cudaLaunchAttribute pdl_attr() {
 
 }  // namespace
 
+// x_sorted == nullptr: the INDEX instance, which writes row_token instead of copying x
 int launch_moe_route(const int32_t* topk_ids, int n_slots, int top_k, int num_experts, const void* x, int K, int32_t* offsets,
-                     int32_t* slot_rows, void* x_sorted, cudaStream_t stream) {
-  static int resident_per_sm[BB_MAX_DEVICES] = {};
+                     int32_t* slot_rows, void* x_sorted, int32_t* row_token, cudaStream_t stream) {
+  const bool index = x_sorted == nullptr;
+  auto kernel = index ? moe_route_kernel<true> : moe_route_kernel<false>;
+  static int resident_per_sm[2][BB_MAX_DEVICES] = {};
   const int dev = current_device();
-  if (!resident_per_sm[dev]) {
+  if (!resident_per_sm[index][dev]) {
     int occ = 0;
-    BB_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, moe_route_kernel, ROUTE_THREADS, 0));
+    BB_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, ROUTE_THREADS, 0));
     if (occ <= 0) { set_error("moe route: the kernel cannot be resident on this device"); return 2; }
-    resident_per_sm[dev] = std::min(occ, ROUTE_CTAS_PER_SM);
+    resident_per_sm[index][dev] = std::min(occ, ROUTE_CTAS_PER_SM);
   }
   RouteParams r;
   r.ids = topk_ids; r.x = reinterpret_cast<const uint4*>(x); r.offsets = offsets; r.slot_rows = slot_rows;
   r.x_sorted = reinterpret_cast<uint4*>(x_sorted); r.n = n_slots; r.k = top_k; r.E = num_experts; r.vecs = K / 8;
-  const int resident = resident_per_sm[dev] * device_sm_count();
+  r.row_token = row_token;
+  const int resident = resident_per_sm[index][dev] * device_sm_count();
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(std::max(1, std::min((n_slots + ROUTE_MIN_SLOTS - 1) / ROUTE_MIN_SLOTS, resident)));
   cfg.blockDim = dim3(ROUTE_THREADS);
@@ -231,7 +245,7 @@ int launch_moe_route(const int32_t* topk_ids, int n_slots, int top_k, int num_ex
   cudaLaunchAttribute attr[1] = {pdl_attr()};
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, moe_route_kernel, r));
+  BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, r));
   BB_LAUNCH_CHECK();
   return 0;
 }

@@ -1,5 +1,11 @@
-"""Mixture-of-experts expert block: device routing (bb_moe_route), the gate/up interleave that the SwiGLU grouped calls read, the
-weighted top-k combine (bb_moe_combine), and ``MoEExperts``, which runs router output to layer output in four library launches.
+"""Mixture-of-experts expert block: device routing (bb_moe_route; bb_moe_route_index without the copy), the gate/up interleave
+that the SwiGLU grouped calls read, the weighted top-k combine (bb_moe_combine), and ``MoEExperts``, which runs router output to
+layer output in four library launches.
+
+Above 8 rows per expert, moe_route_index -> forward_grouped_swiglu(x, ..., row_index=row_token) -> down -> moe_combine computes
+MoEExperts' bits without the [T*k, H] routed copy of x (T*k*H*2 bytes: 64 MiB per layer at 2048 tokens, top-8, H = 2048).
+MoEExperts keeps the copy: the gathering GEMM measured 1.06-1.55x the time of the plain one (H100 80GB HBM3, 700 W, 64-2048
+tokens), more than the copy costs, at every measured point.
 
 Gate/up interleave (include/bitblas_b200.h): the fused gate/up projection of I rows each is stored as 2I rows in which stored row
 16b + i is gate row 8b + i for i < 8 and up row 8b + i - 8 for i >= 8.  Every per-row buffer follows the same permutation:
@@ -101,6 +107,24 @@ def moe_route(topk_ids: torch.Tensor, x: torch.Tensor, num_experts: int):
                                       offsets.data_ptr(), slot_rows.data_ptr(), x_sorted.data_ptr(), stream)
     _lib.check(rc, "bb_moe_route")
     return offsets, slot_rows, x_sorted
+
+
+def moe_route_index(topk_ids: torch.Tensor, num_experts: int):
+    """moe_route without the copy, in one launch (bb_moe_route_index).  Returns (offsets int32 [E + 1], slot_rows int32 [T*k],
+    row_token int32 [T*k]): offsets and slot_rows are exactly moe_route's, and row_token[slot_rows[s]] = s // k for every kept
+    slot s, so x[row_token] is moe_route's x_sorted.  Rows offsets[E] .. T*k - 1 of row_token are left unwritten."""
+    _check(topk_ids, "topk_ids", torch.int32, 2)
+    T, k = topk_ids.shape
+    dev, stream = _device_ready(topk_ids)
+    E = int(num_experts)
+    offsets = torch.empty(max(E, 0) + 1, dtype=torch.int32, device=dev)
+    slot_rows = torch.empty(T * k, dtype=torch.int32, device=dev)
+    row_token = torch.empty(T * k, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        rc = _lib.load().bb_moe_route_index(topk_ids.data_ptr(), T, k, E, offsets.data_ptr(), slot_rows.data_ptr(),
+                                            row_token.data_ptr(), stream)
+    _lib.check(rc, "bb_moe_route_index")
+    return offsets, slot_rows, row_token
 
 
 def moe_combine(y_sorted: torch.Tensor, slot_rows: torch.Tensor, topk_weights: torch.Tensor, output: torch.Tensor = None):
@@ -206,4 +230,4 @@ class MoEExperts(nn.Module):
         self._repack(gate_modules, up_modules, down_modules, device, v2=True)
 
 
-__all__ = ["MoEExperts", "moe_route", "moe_combine", "interleave_gate_up", "deinterleave_gate_up"]
+__all__ = ["MoEExperts", "moe_route", "moe_route_index", "moe_combine", "interleave_gate_up", "deinterleave_gate_up"]

@@ -275,6 +275,7 @@ class Matmul(Operator):
         self._checked_key = None
         self._grouped_checked_key = None
         self._grouped_gemm_ok = False   # bb_matmul_grouped_gemm covers the checked parameter set (N % 128 == 0)
+        self._grouped_gemm_err = ""     # the library's message where it does not
         self._torch_a_dtype = getattr(torch, config.A_dtype, None)
         self._desc_ref = None
         self.weight_executors = None
@@ -576,14 +577,21 @@ class Matmul(Operator):
                 self._forward_grouped_per_group(A, W, offsets, scale, zeros, bias, output, dev, stream)
         return output
 
-    def forward_grouped_swiglu(self, A, W, offsets, scale=None, zeros=None, bias=None, output=None):
+    def forward_grouped_swiglu(self, A, W, offsets, scale=None, zeros=None, bias=None, output=None, row_index=None):
         """The gate/up projection of a SwiGLU mixture-of-experts block in ONE graph-capturable launch: this operator's N = 2I rows
         hold gate and up in the gate/up interleave (bitblas_b200.moe.interleave_gate_up), and the output [T, I] is
         silu(gate) * up, formed in the kernel epilogue from exactly the values forward_grouped(capturable=True) would store
         (bb_matmul_grouped_swiglu / bb_matmul_grouped_gemm_swiglu, picked by the same rule).  Operands and offsets as in
-        forward_grouped."""
+        forward_grouped.
+
+        row_index (int32 CUDA tensor of T entries, e.g. the row_token of bitblas_b200.moe.moe_route_index): sorted row r reads
+        A[clamp(row_index[r], 0, a_rows - 1)] of A [a_rows, K] in the GEMM's producer, so the rows need not be gathered first;
+        the output is [T, I].  This always runs the grouped wgmma GEMM (bb_matmul_grouped_gemm_swiglu_gather) and raises
+        ValueError where it does not cover the config (2I % 128 != 0)."""
         if self.consistent:
             raise NotImplementedError("forward_grouped_swiglu needs a low-bit weight operator")
+        if row_index is not None:
+            return self._forward_grouped_swiglu_gather(A, W, offsets, scale, zeros, bias, output, row_index)
         E, T, ptrs, output, dev, stream = self._grouped_prepare(A, W, offsets, scale, zeros, bias, output, self.config.N // 2,
                                                                 swiglu=True)
         name = "bb_matmul_grouped_swiglu" if self._grouped_single_launch(T, E) == "gemv" else "bb_matmul_grouped_gemm_swiglu"
@@ -594,15 +602,35 @@ class Matmul(Operator):
             raise RuntimeError(f"{name} failed (code {rc}): {_lib.last_error()}")
         return output
 
+    def _forward_grouped_swiglu_gather(self, A, W, offsets, scale, zeros, bias, output, row_index):
+        name = "bb_matmul_grouped_gemm_swiglu_gather"
+        if not isinstance(row_index, torch.Tensor) or row_index.dtype != torch.int32 or row_index.dim() != 1:
+            raise TypeError("row_index must be a 1-D int32 torch.Tensor (one row of A per sorted row)")
+        E, T, ptrs, output, dev, stream = self._grouped_prepare(A, W, offsets, scale, zeros, bias, output, self.config.N // 2,
+                                                                swiglu=True, rows=row_index.numel())
+        if not self._grouped_gemm_ok:
+            raise ValueError(f"{name} does not cover this configuration: {self._grouped_gemm_err}")
+        self._check_tensor(row_index, "row_index", torch.int32)
+        if row_index.device != dev:
+            raise ValueError("row_index must be on A's device")
+        if T > 0 and A.shape[0] < 1:
+            raise ValueError("A must have at least one row to gather from")
+        with torch.cuda.device(dev):
+            rc = self.lib._c.bb_matmul_grouped_gemm_swiglu_gather(self._desc_ref, E, offsets.data_ptr(), row_index.data_ptr(),
+                                                                   A.data_ptr(), A.shape[0], *ptrs, output.data_ptr(), T, stream)
+        if rc != 0:
+            raise RuntimeError(f"{name} failed (code {rc}): {_lib.last_error()}")
+        return output
+
     def _grouped_single_launch(self, T: int, E: int) -> str:
         """the kernel of the one capturable grouped launch for T rows over E groups: the grouped GEMV ("gemv") up to
         GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E rows and where the grouped GEMM does not cover the config (N % 128 != 0),
         the grouped wgmma GEMM ("gemm") above"""
         return "gemm" if T > GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E and self._grouped_gemm_ok else "gemv"
 
-    def _grouped_prepare(self, A, W, offsets, scale, zeros, bias, output, out_cols, swiglu=False):
+    def _grouped_prepare(self, A, W, offsets, scale, zeros, bias, output, out_cols, swiglu=False, rows=None):
         """argument checks of the grouped forwards (parameters once per distinct set); returns (E, T, parameter pointers, output
-        [T, out_cols], device, stream)"""
+        [T, out_cols], device, stream).  T is A's row count, or `rows` (the gathering call, whose A has any number of rows)."""
         c = self.config
         if not isinstance(offsets, torch.Tensor) or offsets.dtype != torch.int32:
             raise TypeError("offsets must be an int32 torch.Tensor of num_groups + 1 row offsets")
@@ -616,10 +644,11 @@ class Matmul(Operator):
             self._check_grouped_params(E, W, scale, zeros, bias)
             self.check_grouped(E, swiglu)
             self._grouped_gemm_ok = self.lib._c.bb_matmul_grouped_gemm(self._desc_ref, E, 0, 0, 0, 0, 0, 0, 0, 0, 0) == 0
+            self._grouped_gemm_err = "" if self._grouped_gemm_ok else _lib.last_error()
             self._grouped_checked_key = key
         if not isinstance(A, torch.Tensor) or A.dim() != 2 or A.shape[1] != c.K:
             raise ValueError(f"A must be [T, K={c.K}], got {tuple(A.shape) if isinstance(A, torch.Tensor) else type(A)}")
-        T = A.shape[0]
+        T = A.shape[0] if rows is None else rows
         if output is not None and (not isinstance(output, torch.Tensor) or tuple(output.shape) != (T, out_cols)):
             raise ValueError(f"output must be [T={T}, {out_cols}]")
         self._check_tensor(A, "A", self._torch_a_dtype)

@@ -173,6 +173,18 @@ int bb_matmul_grouped_swiglu(const bb_matmul_desc* desc, int num_groups, const i
 int bb_matmul_grouped_gemm_swiglu(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
                                   const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream);
 
+/* bb_matmul_grouped_gemm_swiglu reading its rows through an index: sorted row r of group e is A[clamp(row_index[r], 0,
+ * a_rows - 1)] of A [a_rows, K], so a mixture-of-experts block multiplies the token rows in place (row_index = the row_token of
+ * bb_moe_route_index) instead of a routed copy.  row_index is a DEVICE int32 array of total_rows entries, 4-byte aligned, read
+ * on the device; any value is clamped, so every read stays inside A.  Everything else -- coverage (N % 128 == 0), rejections,
+ * offsets, the instance choice from total_rows and num_groups, the SwiGLU epilogue and C [total_rows, N / 2] -- is that of
+ * bb_matmul_grouped_gemm_swiglu, and the result equals that call on the gathered rows bit for bit.  a_rows >= 1 when
+ * total_rows > 0.  ONE launch, CUDA-graph capturable, programmatic stream serialization. */
+int bb_matmul_grouped_gemm_swiglu_gather(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets,
+                                         const int32_t* row_index, const void* A, int a_rows, const void* W,
+                                         const void* scale, const void* zeros, const void* bias, void* C,
+                                         int total_rows, void* stream);
+
 /* Mixture-of-experts routing on the device: slot s = t * top_k + j of the DEVICE int32 table topk_ids [num_tokens, top_k] goes to
  * expert topk_ids[s].  Writes offsets [num_experts + 1] (the offsets of bb_matmul_grouped), slot_rows [T * top_k] (the sorted row
  * of each slot) and x_sorted [T * top_k, K] with x_sorted[slot_rows[s]] = x[s / top_k].  Rows are ordered by expert and, within
@@ -183,6 +195,14 @@ int bb_matmul_grouped_gemm_swiglu(const bb_matmul_desc* desc, int num_groups, co
  * nothing read before the preceding kernel has completed.  num_tokens == 0 validates and returns 0 without touching the device. */
 int bb_moe_route(const int32_t* topk_ids, int num_tokens, int top_k, int num_experts, const void* x, int a_dtype, int K,
                  int32_t* offsets, int32_t* slot_rows, void* x_sorted, void* stream);
+
+/* bb_moe_route without the copy: offsets and slot_rows bit-identical to bb_moe_route's for the same ids, and, for every kept
+ * slot s, row_token[slot_rows[s]] = s / top_k (the token whose row sorted row slot_rows[s] would hold) -- the row_index of
+ * bb_matmul_grouped_gemm_swiglu_gather.  Rows offsets[num_experts] .. T * top_k - 1 of row_token are not written.  The checks of
+ * bb_moe_route without those on x, K and a_dtype; the int32 arrays 4-byte aligned.  ONE launch, no workspace, graph-capturable;
+ * num_tokens == 0 validates and returns 0 without touching the device. */
+int bb_moe_route_index(const int32_t* topk_ids, int num_tokens, int top_k, int num_experts, int32_t* offsets,
+                       int32_t* slot_rows, int32_t* row_token, void* stream);
 
 /* Weighted top-k combine: out[t, :] = sum_j topk_weights[t, j] * Y[slot_rows[t * top_k + j], :], accumulated in fp32 over
  * j = 0 .. top_k - 1 in that order and rounded once to out_dtype (float16 | bfloat16 | float32, also the type of Y [T * top_k, N]).

@@ -1,7 +1,7 @@
 """Mixture-of-experts projections: the grouped matmul (Matmul.forward_grouped, one launch) against what a caller does without it
 (one bitblas.Linear per active expert, counts known on the host).
 
-    python tools/moe_bench.py [--iters 200] [--sweep-only | --no-sweep] [--no-layer]
+    python tools/moe_bench.py [--iters 200] [--sweep-only | --no-sweep] [--no-layer | --layer-only]
 
 Expert shapes (uint4, group 128, quantized zeros, fp16), gate/up (fused) and down as separate cases:
     Mixtral-8x7B      E=8,   top-2, gate/up 28672 x 4096, down 4096 x 14336
@@ -14,8 +14,11 @@ shape up to a few thousand tokens, forward_grouped(capturable=True) (the grouped
 GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP rows per expert, the grouped wgmma GEMM above it) against both sides of the default
 forward_grouped: the single grouped GEMV launch and the per-group bb_matmul path.  The layer section times one MoE expert block
 from router output to layer output, MoEExperts.forward against the torch glue around the two grouped calls (both with the top-k
-weighted combine), eager and replayed from one CUDA graph, with the share of the device routing (bb_moe_route, which copies the
-x rows by expert) in the replayed block.
+weighted combine), eager and replayed from one CUDA graph.  Above 8 rows per expert it also times the copy-free block
+(moe_route_index -> forward_grouped_swiglu(x, row_index=row_token) -> down -> combine), which gives MoEExperts' bits without
+moe_route's [T*k, H] copy of x, eager and replayed, with each block's routing launch (bb_moe_route / bb_moe_route_index) and its
+share of the replayed block, the peak memory each block allocates, and the gate/up call alone: the gathering GEMM on x against
+the plain GEMM on the pre-gathered rows, at the BM the launch picks.
 """
 from __future__ import annotations
 
@@ -185,6 +188,21 @@ def moe_layer(name, tokens, iters):
     def fused():
         return moe(x, ids, w, output=out)
 
+    mm, gu = moe.gate_up.bitblas_matmul, moe.gate_up
+
+    def gathering():   # MoEExperts.forward without moe_route's copy of x: the gate/up GEMM reads x through row_token
+        offsets, slot_rows, row_token = bitblas.moe.moe_route_index(ids, E)
+        h = mm.forward_grouped_swiglu(x, gu.qweight, offsets, gu.scales, gu.zeros, row_index=row_token)
+        return bitblas.moe.moe_combine(moe.down(h, offsets, capturable=True), slot_rows, w, out)
+
+    def peak_bytes(fn):   # allocated by one block beyond what is live before it
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        base = torch.cuda.memory_allocated()
+        fn()
+        torch.cuda.synchronize()
+        return torch.cuda.max_memory_allocated() - base
+
     def host_time(run, sync, n):
         for _ in range(3):
             run()
@@ -210,13 +228,35 @@ def moe_layer(name, tokens, iters):
     res = dict(model=name, tokens=tokens, rows=tokens * topk, launches_fused=lib_launches,
                ops_fused=device_ops(fused), ops_glue=device_ops(glue),
                max_abs_diff=float((got - ref).abs().max()), max_abs_ref=float(ref.abs().max()))
+    # the gathering gate/up call is the grouped GEMM at every T; MoEExperts' is the GEMM (same bits) above 8 rows per expert
+    gathers = tokens * topk > GM.GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E
+    res["gathers"] = gathers
     g_glue, g_fused = bitblas.CapturedStep(glue), bitblas.CapturedStep(fused)
-    for _ in range(2):    # alternate the two sides so drift on a shared host hits both
+    g_gath = bitblas.CapturedStep(gathering) if gathers else None
+    res["peak_fused_MB"] = peak_bytes(fused) / 2**20
+    for _ in range(2):    # alternate the sides so drift on a shared host hits all of them
         res["glue_eager_us"] = host_time(glue, torch.cuda.synchronize, iters)
         res["fused_eager_us"] = host_time(fused, torch.cuda.synchronize, iters)
         res["glue_graph_us"] = host_time(g_glue.run, g_glue.wait, iters)
         res["fused_graph_us"] = host_time(g_fused.run, g_fused.wait, iters)
+        if gathers:
+            res["gath_eager_us"] = host_time(gathering, torch.cuda.synchronize, iters)
+            res["gath_graph_us"] = host_time(g_gath.run, g_gath.wait, iters)
     res["route_us"] = time_calls(lambda i: bitblas.moe.moe_route(ids, x, E), iters)
+    if gathers:   # the gate/up call alone: gathering GEMM on x vs the plain GEMM on the pre-gathered rows
+        res["gath_equal"] = bool(torch.equal(gathering().float(), got))
+        res["peak_gath_MB"] = peak_bytes(gathering) / 2**20
+        res["route_index_us"] = time_calls(lambda i: bitblas.moe.moe_route_index(ids, E), iters)
+        offsets, _, row_token = bitblas.moe.moe_route_index(ids, E)
+        xs = x[row_token.long()]
+        rows = tokens * topk
+        mean = -(-rows // min(E, rows))
+        res["bm"] = 32 if mean <= 32 else (64 if mean <= 64 else 128)
+        for _ in range(2):
+            res["gemm_gather_us"] = time_calls(
+                lambda i: mm.forward_grouped_swiglu(x, gu.qweight, offsets, gu.scales, gu.zeros, row_index=row_token), iters)
+            res["gemm_plain_us"] = time_calls(lambda i: mm.forward_grouped_swiglu(xs, gu.qweight, offsets, gu.scales, gu.zeros),
+                                              iters)
     return res
 
 
@@ -228,13 +268,16 @@ def main():
     ap.add_argument("--sweep-only", action="store_true")
     ap.add_argument("--no-sweep", action="store_true")
     ap.add_argument("--no-layer", action="store_true")
-    ap.add_argument("--layer-tokens", default="1,4,16,64,512,2048")
+    ap.add_argument("--layer-only", action="store_true", help="only the MoE expert block section")
+    ap.add_argument("--layer-tokens", default="1,4,16,64,256,512,1024,2048")
     ap.add_argument("--json", default=None, help="also write the results here")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "moe_bench measures on the GPU; there is no CPU fallback"
     print(f"# {card()}")
     print(f"# GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP = {GM.GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP}")
     results = []
+    if args.layer_only:
+        args.sweep_only = args.no_sweep = True
     if not args.sweep_only:
         print(f"{'model':18s} {'proj':8s} {'tok':>5s} {'T':>6s} {'act':>4s} {'MB':>8s} | "
               f"{'grouped us':>10s} {'GB/s':>7s} {'HBM':>6s} {'L':>3s} | {'loop us':>9s} {'GB/s':>7s} {'HBM':>6s} {'L':>4s} | speedup | "
@@ -279,17 +322,30 @@ def main():
                 torch.cuda.empty_cache()
     if not args.no_layer:
         print("\n# one MoE expert block (router output in, [T, H] out): MoEExperts.forward vs torch glue around the grouped calls")
-        print(f"{'model':18s} {'tok':>5s} {'rows':>6s} | {'glue eager':>10s} {'fused eager':>11s} {'glue graph':>10s} "
-              f"{'fused graph':>11s} {'graph x':>7s} | {'route us':>8s} {'share':>6s} | {'L':>2s} {'ops glue':>8s} {'ops fused':>9s} | "
-              f"max |fused - glue| (max |ref|)")
+        print("# fused = MoEExperts.forward (moe_route's copy of x); gath = the copy-free block (moe_route_index + the gathering "
+              "gate/up GEMM), above 8 rows per expert;\n# route = the routing launch alone (its share of the replayed block); "
+              "peak = MB allocated by one block; gather/plain = the gate/up GEMM alone; = fused: bit-identical")
+        print(f"{'model':18s} {'tok':>5s} {'rows':>6s} | {'glue eager':>10s} {'fused eager':>11s} {'gath eager':>10s} "
+              f"{'glue graph':>10s} {'fused graph':>11s} {'gath graph':>10s} {'fused/gath':>10s} | {'route us':>8s} {'share':>6s} "
+              f"{'idx rt':>7s} {'share':>6s} | {'peak MB':>7s} {'gath MB':>7s} | {'BM':>3s} {'gather us':>9s} {'plain us':>8s} | "
+              f"{'L':>2s} {'ops glue':>8s} {'ops fused':>9s} | = fused | max |fused - glue| (max |ref|)")
         for name in MODELS:
             for tok in map(int, args.layer_tokens.split(",")):
                 r = moe_layer(name, tok, max(5, min(args.iters, 20000 // tok)))
                 results.append(r)
-                print(f"{name:18s} {tok:5d} {r['rows']:6d} | {r['glue_eager_us']:10.1f} {r['fused_eager_us']:11.1f} "
-                      f"{r['glue_graph_us']:10.1f} {r['fused_graph_us']:11.1f} {r['glue_graph_us'] / r['fused_graph_us']:6.2f}x | "
-                      f"{r['route_us']:8.1f} {r['route_us'] / r['fused_graph_us']:6.1%} | {r['launches_fused']:2d} "
-                      f"{r['ops_glue']:8d} {r['ops_fused']:9d} | {r['max_abs_diff']:.3g} ({r['max_abs_ref']:.3g})", flush=True)
+                if r["gathers"]:
+                    gath = (f"{r['gath_eager_us']:10.1f}", f"{r['gath_graph_us']:10.1f}",
+                            f"{r['fused_graph_us'] / r['gath_graph_us']:9.3f}x",
+                            f"{r['route_index_us']:7.1f} {r['route_index_us'] / r['gath_graph_us']:6.1%}", f"{r['peak_gath_MB']:7.1f}",
+                            f"{r['bm']:3d} {r['gemm_gather_us']:9.1f} {r['gemm_plain_us']:8.1f}", "y" if r["gath_equal"] else "N")
+                else:
+                    gath = (f"{'-':>10s}", f"{'-':>10s}", f"{'-':>10s}", f"{'-':>7s} {'-':>6s}", f"{'-':>7s}",
+                            f"{'-':>3s} {'-':>9s} {'-':>8s}", "-")
+                print(f"{name:18s} {tok:5d} {r['rows']:6d} | {r['glue_eager_us']:10.1f} {r['fused_eager_us']:11.1f} {gath[0]} "
+                      f"{r['glue_graph_us']:10.1f} {r['fused_graph_us']:11.1f} {gath[1]} {gath[2]} | "
+                      f"{r['route_us']:8.1f} {r['route_us'] / r['fused_graph_us']:6.1%} {gath[3]} | {r['peak_fused_MB']:7.1f} {gath[4]} | "
+                      f"{gath[5]} | {r['launches_fused']:2d} {r['ops_glue']:8d} {r['ops_fused']:9d} | {gath[6]:>7s} "
+                      f"| {r['max_abs_diff']:.3g} ({r['max_abs_ref']:.3g})", flush=True)
                 torch.cuda.empty_cache()
     if args.json:
         with open(args.json, "w") as f:
