@@ -277,46 +277,6 @@ int bb_matmul_scatter(const bb_matmul_desc* desc, const void* A, const void* W, 
                      workspace_bytes, stream);
 }
 
-// the argument checks of both grouped entry points, after the configuration check: 0 = launch, -1 = nothing to do
-// (total_rows == 0), otherwise the error code to return
-static int check_grouped_args(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
-                              const void* scale, const void* zeros, const void* bias, void* C, int total_rows) {
-  if (num_groups < 1 || num_groups > BB_GROUPED_MAX_GROUPS) {
-    set_error("num_groups must be in [1, %d] (got %d)", BB_GROUPED_MAX_GROUPS, num_groups);
-    return 1;
-  }
-  if (total_rows < 0) { set_error("total_rows must be >= 0 (got %d)", total_rows); return 1; }
-  if (total_rows == 0) return -1;
-  if (!offsets) { set_error("offsets must be a device pointer to num_groups + 1 int32 values"); return 1; }
-  if (!A || !W || !C) { set_error("A, W and C must be non-null"); return 1; }
-  if (desc->with_scaling && !scale) { set_error("with_scaling is set but scale is null"); return 1; }
-  if (desc->with_zeros && !zeros) { set_error("with_zeros is set but zeros is null"); return 1; }
-  if (desc->with_bias && !bias) { set_error("with_bias is set but bias is null"); return 1; }
-  if ((reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(W) & 15) || (reinterpret_cast<uintptr_t>(offsets) & 3)) {
-    set_error("grouped matmul: A and W must be 16-byte aligned, offsets 4-byte aligned");
-    return 5;
-  }
-  return 0;
-}
-
-int bb_matmul_grouped(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
-                      const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream) {
-  if (validate(desc)) return 1;
-  if (!grouped_supported(*desc)) return 1;
-  const int rc = check_grouped_args(desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows);
-  if (rc) return rc < 0 ? 0 : rc;
-  return launch_grouped(*desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows, (cudaStream_t)stream);
-}
-
-int bb_matmul_grouped_gemm(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
-                           const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream) {
-  if (validate(desc)) return 1;
-  if (!grouped_gemm_supported(*desc)) return 1;
-  const int rc = check_grouped_args(desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows);
-  if (rc) return rc < 0 ? 0 : rc;
-  return launch_grouped_gemm(*desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows, (cudaStream_t)stream);
-}
-
 // the gate/up interleave pairs 8 gate rows with 8 up rows in every 16-row block of W: N = 2I with I % 8 == 0
 static bool swiglu_shape_ok(const bb_matmul_desc* desc) {
   if (desc && desc->N % 16) {
@@ -326,36 +286,73 @@ static bool swiglu_shape_ok(const bb_matmul_desc* desc) {
   return true;
 }
 
+// the grouped entry points: gemm picks the grouped wgmma GEMM instead of the grouped GEMV, swiglu the fused gate/up epilogue,
+// gather (GEMM with swiglu) the A rows through row_index.  Every rejection has its own message and code, so the order of the
+// checks is part of the interface.
+static int grouped_call(bool gemm, bool swiglu, bool gather, const bb_matmul_desc* desc, int num_groups, const int32_t* offsets,
+                        const int32_t* row_index, const void* A, int a_rows, const void* W, const void* scale, const void* zeros,
+                        const void* bias, void* C, int total_rows, void* stream) {
+  if (validate(desc)) return 1;
+  if (swiglu && !swiglu_shape_ok(desc)) return 1;
+  if (!(gemm ? grouped_gemm_supported(*desc) : grouped_supported(*desc))) return 1;
+  if (num_groups < 1 || num_groups > BB_GROUPED_MAX_GROUPS) {
+    set_error("num_groups must be in [1, %d] (got %d)", BB_GROUPED_MAX_GROUPS, num_groups);
+    return 1;
+  }
+  if (total_rows < 0) { set_error("total_rows must be >= 0 (got %d)", total_rows); return 1; }
+  if (total_rows == 0) return 0;
+  if (!offsets) { set_error("offsets must be a device pointer to num_groups + 1 int32 values"); return 1; }
+  if (!A || !W || !C) { set_error("A, W and C must be non-null"); return 1; }
+  if (desc->with_scaling && !scale) { set_error("with_scaling is set but scale is null"); return 1; }
+  if (desc->with_zeros && !zeros) { set_error("with_zeros is set but zeros is null"); return 1; }
+  if (desc->with_bias && !bias) { set_error("with_bias is set but bias is null"); return 1; }
+  if ((reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(W) & 15) || (reinterpret_cast<uintptr_t>(offsets) & 3)) {
+    set_error("grouped matmul: A and W must be 16-byte aligned, offsets 4-byte aligned");
+    return 5;
+  }
+  if (gather) {
+    if (!row_index) { set_error("gather: row_index must be a device pointer to total_rows int32 values"); return 1; }
+    if (a_rows < 1) { set_error("gather: a_rows must be >= 1 (got %d)", a_rows); return 1; }
+    if (reinterpret_cast<uintptr_t>(row_index) & 3) { set_error("gather: row_index must be 4-byte aligned"); return 5; }
+  }
+  GroupedArgs g;
+  g.d = *desc; g.num_groups = num_groups; g.offsets = offsets; g.A = A; g.W = W; g.scale = scale; g.zeros = zeros; g.bias = bias;
+  g.C = C; g.total_rows = total_rows; g.stream = (cudaStream_t)stream;
+  g.swiglu = swiglu; g.row_index = row_index; g.a_rows = a_rows;
+  // the stacked parameters: W [E, N, K * bits / 8], scale [E, N, G], zeros [E, N, G] ([E, G, N * bits / 8] quantized), bias [E, N]
+  const long long N = desc->N, G = desc->K / (desc->group_size <= 0 ? desc->K : desc->group_size);
+  g.w_stride = N * desc->K * desc->w_bits / 8;
+  g.s_stride = N * G * 2;
+  g.z_stride = desc->zeros_mode == BB_ZEROS_QUANTIZED ? G * (N * desc->w_bits / 8) : N * G * 2;
+  g.b_stride = N * 2;
+  return gemm ? launch_grouped_gemm(g) : launch_grouped(g);
+}
+
+int bb_matmul_grouped(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                      const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream) {
+  return grouped_call(false, false, false, desc, num_groups, offsets, nullptr, A, 0, W, scale, zeros, bias, C, total_rows, stream);
+}
+
+int bb_matmul_grouped_gemm(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
+                           const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream) {
+  return grouped_call(true, false, false, desc, num_groups, offsets, nullptr, A, 0, W, scale, zeros, bias, C, total_rows, stream);
+}
+
 int bb_matmul_grouped_swiglu(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
                              const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream) {
-  if (validate(desc)) return 1;
-  if (!swiglu_shape_ok(desc) || !grouped_supported(*desc)) return 1;
-  const int rc = check_grouped_args(desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows);
-  if (rc) return rc < 0 ? 0 : rc;
-  return launch_grouped(*desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows, (cudaStream_t)stream, true);
+  return grouped_call(false, true, false, desc, num_groups, offsets, nullptr, A, 0, W, scale, zeros, bias, C, total_rows, stream);
 }
 
 int bb_matmul_grouped_gemm_swiglu(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const void* W,
                                   const void* scale, const void* zeros, const void* bias, void* C, int total_rows, void* stream) {
-  if (validate(desc)) return 1;
-  if (!swiglu_shape_ok(desc) || !grouped_gemm_supported(*desc)) return 1;
-  const int rc = check_grouped_args(desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows);
-  if (rc) return rc < 0 ? 0 : rc;
-  return launch_grouped_gemm(*desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows, (cudaStream_t)stream, true);
+  return grouped_call(true, true, false, desc, num_groups, offsets, nullptr, A, 0, W, scale, zeros, bias, C, total_rows, stream);
 }
 
 int bb_matmul_grouped_gemm_swiglu_gather(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets,
                                          const int32_t* row_index, const void* A, int a_rows, const void* W, const void* scale,
                                          const void* zeros, const void* bias, void* C, int total_rows, void* stream) {
-  if (validate(desc)) return 1;
-  if (!swiglu_shape_ok(desc) || !grouped_gemm_supported(*desc)) return 1;
-  const int rc = check_grouped_args(desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows);
-  if (rc) return rc < 0 ? 0 : rc;
-  if (!row_index) { set_error("gather: row_index must be a device pointer to total_rows int32 values"); return 1; }
-  if (a_rows < 1) { set_error("gather: a_rows must be >= 1 (got %d)", a_rows); return 1; }
-  if (reinterpret_cast<uintptr_t>(row_index) & 3) { set_error("gather: row_index must be 4-byte aligned"); return 5; }
-  return launch_grouped_gemm(*desc, num_groups, offsets, A, W, scale, zeros, bias, C, total_rows, (cudaStream_t)stream, true,
-                             row_index, a_rows);
+  return grouped_call(true, true, true, desc, num_groups, offsets, row_index, A, a_rows, W, scale, zeros, bias, C, total_rows,
+                      stream);
 }
 
 // the checks bb_moe_route and bb_moe_route_index share: 0 = valid
@@ -436,15 +433,7 @@ int bb_peer_barrier(void* const* peer_flags, int n_peers, int rank, void* stream
   for (int i = 0; i < BB_MAX_PEERS; ++i) a.flags[i] = i < n_peers ? reinterpret_cast<uint32_t*>(peer_flags[i]) : nullptr;
   for (int i = 0; i < n_peers; ++i) if (!a.flags[i] || (reinterpret_cast<uintptr_t>(a.flags[i]) & 3)) { set_error("bb_peer_barrier: flag block %d is null or unaligned", i); return 1; }
   a.n = n_peers; a.rank = rank;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(1); cfg.blockDim = dim3(32); cfg.dynamicSmemBytes = 0; cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, peer_barrier_kernel, a));
-  BB_LAUNCH_CHECK();
-  return 0;
+  return launch_pdl(peer_barrier_kernel, 1, 32, 0, (cudaStream_t)stream, true, a);
 }
 
 }  // extern "C"

@@ -9,6 +9,7 @@
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
+#include <utility>
 
 #include "../../include/bitblas_b200.h"
 
@@ -65,6 +66,58 @@ int device_sm_count();    // SM count of the current device (cached per device)
 // whether the streaming kernels launch with programmatic dependent launch (default on; BB_PDL=0 restores plain stream order)
 bool pdl_enabled();
 
+// kernel<<<grid, block, smem, stream>>>(args...) with the programmatic-stream-serialization attribute set to `overlap`
+// (pdl_enabled() for the library's matmul kernels): the launch may then begin while its predecessor on the stream finishes.
+// Counts the launch; returns 0, or 2 / 3 with the error set as BB_CHECK_CUDA / BB_LAUNCH_CHECK do.
+template <typename... Params, typename... Args>
+int launch_pdl(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, bool overlap, Args&&... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = overlap ? 1 : 0;
+  cfg.attrs = attr; cfg.numAttrs = 1;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+  if (e != cudaSuccess) {
+    set_error("cudaLaunchKernelEx failed: %s (%s:%d)", cudaGetErrorString(e), __FILE__, __LINE__);
+    return 2;
+  }
+  BB_LAUNCH_CHECK();
+  return 0;
+}
+
+// One-time set-up of a kernel instance, done once per device.  A launcher keeps one `static KernelCache` per kernel instance
+// (several instances share one function-pointer type, so the storage cannot be keyed on the type), with SLOTS results per
+// device: one per block size it launches the instance with.
+template <int SLOTS = 1>
+struct KernelCache {
+  std::atomic<int> v[BB_MAX_DEVICES][SLOTS];   // 0: not set up on that device yet; -1: cannot be resident
+};
+constexpr size_t kSmemOptinMax = ~size_t(0);
+
+// Sets `kernel` up on device `dev` (the current device), once per (device, slot) of `cache`: raises its dynamic shared-memory
+// limit to smem_limit bytes (kSmemOptinMax: the device's opt-in maximum; 0: leaves it), then, with threads > 0, queries how many
+// CTAs of `threads` threads and `smem` dynamic bytes are resident per SM.  Returns that count (1 when threads == 0), or 0 when
+// the kernel cannot be resident or a runtime call failed; a failed call's error is cleared and nothing is cached.
+template <int SLOTS, typename Kernel>
+int kernel_setup(KernelCache<SLOTS>& cache, Kernel kernel, size_t smem_limit, int threads = 0, size_t smem = 0, int slot = 0,
+                 int dev = current_device()) {
+  std::atomic<int>& c = cache.v[dev][slot];
+  const int cached = c.load(std::memory_order_relaxed);
+  if (cached != 0) return cached > 0 ? cached : 0;
+  int limit = int(smem_limit), occ = 1;
+  bool ok = true;
+  if (smem_limit == kSmemOptinMax) ok = cudaDeviceGetAttribute(&limit, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) == cudaSuccess;
+  if (ok && smem_limit != 0) ok = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, limit) == cudaSuccess;
+  if (ok && threads > 0) ok = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, smem) == cudaSuccess;
+  if (!ok) {
+    cudaGetLastError();
+    return 0;
+  }
+  c.store(occ > 0 ? occ : -1, std::memory_order_relaxed);
+  return occ > 0 ? occ : 0;
+}
+
 // the driver's cuTensorMapEncodeTiled, looked up once through the runtime (no libcuda link); null when unavailable
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -84,18 +137,31 @@ int launch_gemv_i8(const MatmulArgs& a);
 bool gemm_ts_supported(const bb_matmul_desc& d, int m);
 int launch_gemm_ts(const MatmulArgs& a);
 size_t gemm_ts_workspace_bytes(const bb_matmul_desc& d, int m);
-// grouped (mixture-of-experts) matmul, bb_grouped.cu: grouped_supported sets the error message when it returns false.
-// swiglu: W holds gate/up interleaved (2I = d.N rows), C is [total_rows, d.N / 2] = silu(gate) * up (store_swiglu below)
+// one grouped (mixture-of-experts) call, validated by bb_api.cu: num_groups problems of descriptor d, group e on rows
+// [offsets[e], offsets[e + 1]) of A and C; W, scale, zeros and bias are stacked over the groups
+struct GroupedArgs {
+  bb_matmul_desc d;
+  int num_groups;
+  const int32_t* offsets;   // [num_groups + 1], device
+  const void* A;
+  const void* W;
+  const void* scale;
+  const void* zeros;
+  const void* bias;
+  void* C;
+  int total_rows;
+  cudaStream_t stream;
+  bool swiglu;              // W holds gate/up interleaved (2I = d.N rows), C is [total_rows, d.N / 2] = silu(gate) * up
+  const int32_t* row_index; // gathering GEMM (swiglu only), else null: sorted row r reads A[clamp(row_index[r], 0, a_rows - 1)]
+  int a_rows;               //   of A [a_rows, K] instead of A[r]
+  long long w_stride, s_stride, z_stride, b_stride;   // bytes per group of W, scale, zeros and bias
+};
+// grouped matmul, bb_grouped.cu (the decode GEMV's kernel), and grouped wgmma GEMM, bb_grouped_gemm.cu: *_supported set the
+// error message when they return false (store_swiglu below is the SwiGLU epilogue of both)
 bool grouped_supported(const bb_matmul_desc& d);
-int launch_grouped(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
-                   const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream,
-                   bool swiglu = false);
-// grouped wgmma GEMM, bb_grouped_gemm.cu: the same operands and offset contract.  row_index (swiglu only): sorted row r reads
-// A[clamp(row_index[r], 0, a_rows - 1)] of A [a_rows, K] instead of A[r]
+int launch_grouped(const GroupedArgs& g);
 bool grouped_gemm_supported(const bb_matmul_desc& d);
-int launch_grouped_gemm(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
-                        const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream,
-                        bool swiglu = false, const int32_t* row_index = nullptr, int a_rows = 0);
+int launch_grouped_gemm(const GroupedArgs& g);
 // mixture-of-experts routing and top-k combine, bb_moe.cu (arguments validated by the callers in bb_api.cu).  Routing copies x
 // into x_sorted, or, with x_sorted == nullptr, writes row_token instead (bb_moe_route_index)
 int launch_moe_route(const int32_t* topk_ids, int n_slots, int top_k, int num_experts, const void* x, int K, int32_t* offsets,
@@ -140,17 +206,19 @@ struct OutSpec {
   long long ld;          // row stride in elements
   long long col0;        // column offset of this shard
 };
-inline OutSpec make_outspec(const MatmulArgs& a) {
+inline OutSpec make_outspec(void* C, long long ld) {   // the single output C
   OutSpec o;
-  if (a.n_peers > 0) {
-    o.n = a.n_peers;
-    for (int i = 0; i < BB_MAX_PEERS; ++i) o.ptr[i] = i < a.n_peers ? a.peer_C[i] : nullptr;
-    o.ld = a.ldc; o.col0 = a.col_offset;
-  } else {
-    o.n = 1;
-    for (int i = 0; i < BB_MAX_PEERS; ++i) o.ptr[i] = i == 0 ? a.C : nullptr;
-    o.ld = a.d.N; o.col0 = 0;
-  }
+  o.n = 1;
+  for (int i = 0; i < BB_MAX_PEERS; ++i) o.ptr[i] = i == 0 ? C : nullptr;
+  o.ld = ld; o.col0 = 0;
+  return o;
+}
+inline OutSpec make_outspec(const MatmulArgs& a) {
+  if (a.n_peers == 0) return make_outspec(a.C, a.d.N);
+  OutSpec o;
+  o.n = a.n_peers;
+  for (int i = 0; i < BB_MAX_PEERS; ++i) o.ptr[i] = i < a.n_peers ? a.peer_C[i] : nullptr;
+  o.ld = a.ldc; o.col0 = a.col_offset;
   return o;
 }
 

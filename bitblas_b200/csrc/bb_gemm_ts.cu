@@ -372,11 +372,10 @@ int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
   using SM = TsSmem<T, BITS, BM>;
   using EI = ElemInfo<T>;
   auto kernel = gemm_ts_kernel<T, BITS, BM, IL, FMT>;
-  static bool attr_set[BB_MAX_DEVICES] = {};   // cudaFuncSetAttribute is per device
-  const int dev = current_device();
-  if (!attr_set[dev]) {
-    BB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kTotal));
-    attr_set[dev] = true;
+  static KernelCache<> cache;
+  if (!kernel_setup(cache, kernel, SM::kTotal)) {
+    set_error("gemm_ts: cannot raise the kernel's dynamic shared memory to %d bytes on this device", SM::kTotal);
+    return 2;
   }
   TsParams p = p0;
   p.m_tiles = (a.m + BM - 1) / BM;
@@ -472,16 +471,7 @@ int launch_gemm_ts(const MatmulArgs& a) {
     set_error("gemm_ts: A and W must be 16-byte aligned");
     return 5;
   }
-  TsParams p;
-  p.scale = d.with_scaling ? a.scale : nullptr;
-  p.zeros = d.with_zeros ? a.zeros : nullptr;
-  p.bias = d.with_bias ? a.bias : nullptr;
-  p.out = make_outspec(a); p.M = a.m; p.N = d.N; p.K = d.K; p.g = a.gsize(); p.G = a.groups();
-  p.mode = !d.with_scaling ? 0 : (!d.with_zeros ? 1 : 2 + d.zeros_mode);
-  p.zp_const = d.w_fmt == BB_W_INT ? (1 << (d.w_bits - 1)) : 0;
-  p.out_dtype = d.out_dtype; p.a_dtype = d.a_dtype; p.m_tiles = 1;
-  p.lut = d.w_fmt == BB_W_NF ? a.lut : nullptr;
-  p.w_fmt = d.w_fmt;
+  const TsParams p = make_ts_params(d, a.scale, a.zeros, a.bias, a.lut, make_outspec(a), a.m);
   if (d.w_fmt == BB_W_NF || d.w_fmt == BB_W_FP4)
     return d.a_dtype == BB_F16 ? launch_ts_bm<__half, 4, false, 1>(a, p) : launch_ts_bm<__nv_bfloat16, 4, false, 1>(a, p);
   if (d.w_fmt == BB_W_FP8_E4M3 || d.w_fmt == BB_W_FP8_E5M2)

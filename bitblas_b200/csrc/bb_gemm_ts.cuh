@@ -106,6 +106,23 @@ struct TsParams {
   int w_tiled;       // BB_TILE_SLAB weight storage: tmW is the 4-D map {512 B, 32 rows, segments per row, row blocks}
 };
 
+// the parameters of M rows of A against W, up to the split-K fields and w_tiled (set by the launcher)
+inline TsParams make_ts_params(const bb_matmul_desc& d, const void* scale, const void* zeros, const void* bias, const void* lut,
+                               const OutSpec& out, int M) {
+  TsParams p;
+  p.scale = d.with_scaling ? scale : nullptr;
+  p.zeros = d.with_zeros ? zeros : nullptr;
+  p.bias = d.with_bias ? bias : nullptr;
+  p.out = out; p.M = M; p.N = d.N; p.K = d.K;
+  p.g = d.group_size <= 0 ? d.K : d.group_size; p.G = d.K / p.g;
+  p.mode = !d.with_scaling ? 0 : (!d.with_zeros ? 1 : 2 + d.zeros_mode);
+  p.zp_const = d.w_fmt == BB_W_INT ? (1 << (d.w_bits - 1)) : 0;
+  p.out_dtype = d.out_dtype; p.a_dtype = d.a_dtype; p.m_tiles = 1;
+  p.lut = d.w_fmt == BB_W_NF ? lut : nullptr;
+  p.w_fmt = d.w_fmt;
+  return p;
+}
+
 template <typename T>
 struct ElemInfo {
   static constexpr bool kInt8 = false;

@@ -20,8 +20,6 @@
 //     compressed layout are both consumed with zero re-ordering cost (the B fragment is permuted instead).
 //   * per-group scale is applied to the group's partial sum; non-integer zero points / "rescale" zeros use a
 //     third MMA against a ones fragment to obtain sum(a) per group.
-#include <algorithm>
-
 #include "bb_gemv_mma.cuh"
 
 namespace bb {
@@ -168,53 +166,12 @@ gemv_i8_kernel(const GemvParams p) {
   }
 }
 
-GemvParams make_params(const MatmulArgs& a) {
-  GemvParams p;
-  const bb_matmul_desc& d = a.d;
-  p.A = a.A; p.W = (const uint8_t*)a.W; p.scale = d.with_scaling ? a.scale : nullptr;
-  p.zeros = d.with_zeros ? a.zeros : nullptr; p.bias = d.with_bias ? a.bias : nullptr; p.out = make_outspec(a);
-  p.M = a.m; p.N = d.N; p.K = d.K;
-  p.g = a.gsize(); p.G = a.groups();
-  p.with_scaling = d.with_scaling;
-  p.zmode = d.with_zeros ? (d.zeros_mode + 1) : 0;
-  p.zp_const = (d.w_fmt == BB_W_INT) ? (1 << (d.w_bits - 1)) : 0;
-  p.out_dtype = d.out_dtype;
-  p.ks = 1;
-  return p;
-}
-
-// K splits per 16-row block (= warps per CTA): the largest count for which EVERY CTA of the grid is resident at once
-// (occupancy queried from the runtime for this kernel instantiation, cached).  When not even two warps per CTA fit in one wave
-// (N >= ~24k rows), the full split is used and the grid runs in several waves rather than with one resident warp per row
-// block.
-template <typename KernelT>
-int pick_ks(KernelT kernel, int (&occ_cache)[MAX_KS + 1], int max_ks, int row_blocks, int steps) {
-  const int sms = device_sm_count();
-  for (int ks = max_ks; ks >= 2; --ks) {
-    if (ks > steps) continue;
-    if (occ_cache[ks] < 0) {
-      int occ = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, ks * 32, 0) != cudaSuccess) occ = 0;
-      occ_cache[ks] = occ;
-    }
-    if (row_blocks <= sms * occ_cache[ks]) return ks;
-  }
-  return std::max(1, std::min(max_ks, steps));
-}
-
-static_assert(MAX_KS == 8, "BB_GEMV_GO initialises one occupancy cache entry per K split");
-#define BB_GEMV_GO(KERNEL, MAXKS)                                              \
-  {                                                                            \
-    static int occ_cache[MAX_KS + 1] = {-1, -1, -1, -1, -1, -1, -1, -1, -1};   \
-    p.ks = pick_ks(KERNEL, occ_cache, MAXKS, nb, p.K / 128);                   \
-    cudaLaunchConfig_t cfg = {};                                               \
-    cfg.gridDim = dim3(nb); cfg.blockDim = dim3(p.ks * 32);                    \
-    cfg.dynamicSmemBytes = 0; cfg.stream = a.stream;                           \
-    cudaLaunchAttribute attr[1];                                               \
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;           \
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0; \
-    cfg.attrs = attr; cfg.numAttrs = 1;                                        \
-    BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, KERNEL, p));                        \
+// one CTA per 16-row block, the K split from pick_ks
+#define BB_GEMV_GO(KERNEL, MAXKS)                                                 \
+  {                                                                               \
+    static KernelCache<MAX_KS + 1> cache;                                         \
+    p.ks = pick_ks(cache, KERNEL, MAXKS, nb, p.K / 128);                          \
+    return launch_pdl(KERNEL, nb, p.ks * 32, 0, a.stream, pdl_enabled(), p);      \
   }
 
 template <typename T, int BITS, bool IL>
@@ -231,9 +188,9 @@ int launch_mma_nt(const MatmulArgs& a, GemvParams p) {
   else if (p.zmode == 2) { BB_GEMV_NT(2, true) }
   else { BB_GEMV_NT(3, true) }
 #undef BB_GEMV_NT
-  BB_LAUNCH_CHECK();
-  return 0;
 }
+
+GemvParams make_params(const MatmulArgs& a) { return make_params(a.d, a.A, a.W, a.scale, a.zeros, a.bias, make_outspec(a), a.m); }
 
 }  // namespace
 
@@ -300,8 +257,6 @@ int launch_gemv_i8(const MatmulArgs& a) {
     else if (nt == 2) BB_GEMV_GO((gemv_i8_kernel<4, 2>), MAX_KS)
     else BB_GEMV_GO((gemv_i8_kernel<4, 4>), MAX_KS)
   }
-  BB_LAUNCH_CHECK();
-  return 0;
 }
 
 }  // namespace bb

@@ -2,6 +2,7 @@
 // gemv_mma_kernel (bb_gemv.cu) runs it once per CTA; gemv_grouped_kernel (bb_grouped.cu) runs it for every (expert, row block,
 // row chunk) work item a persistent CTA takes.  The design notes are at the top of bb_gemv.cu.
 #pragma once
+#include <algorithm>
 #include <type_traits>
 
 #include "bb_common.cuh"
@@ -31,6 +32,35 @@ struct GemvParams {
   int out_dtype;
   int ks;         // warps per CTA
 };
+
+// the parameters of M rows of A against W (the launcher sets ks)
+inline GemvParams make_params(const bb_matmul_desc& d, const void* A, const void* W, const void* scale, const void* zeros,
+                              const void* bias, const OutSpec& out, int M) {
+  GemvParams p;
+  p.A = A; p.W = reinterpret_cast<const uint8_t*>(W); p.scale = d.with_scaling ? scale : nullptr;
+  p.zeros = d.with_zeros ? zeros : nullptr; p.bias = d.with_bias ? bias : nullptr; p.out = out;
+  p.M = M; p.N = d.N; p.K = d.K;
+  p.g = d.group_size <= 0 ? d.K : d.group_size; p.G = d.K / p.g;
+  p.with_scaling = d.with_scaling;
+  p.zmode = d.with_zeros ? (d.zeros_mode + 1) : 0;
+  p.zp_const = (d.w_fmt == BB_W_INT) ? (1 << (d.w_bits - 1)) : 0;
+  p.out_dtype = d.out_dtype;
+  p.ks = 1;
+  return p;
+}
+
+// K splits per CTA (= warps per CTA) for a grid of `ctas` CTAs over rows of `steps` 128-k steps: the largest count up to max_ks
+// for which EVERY CTA is resident at once (occupancy of this kernel instance, cached in `cache` per device and split).  When not
+// even two warps per CTA fit in one wave (the decode GEMV at N >= ~24k rows), the full split is used and the grid runs in several
+// waves rather than with one resident warp per CTA.
+template <typename Kernel>
+int pick_ks(KernelCache<MAX_KS + 1>& cache, Kernel kernel, int max_ks, int ctas, int steps) {
+  const int full = std::max(1, std::min(max_ks, steps));
+  const int dev = current_device(), sms = device_sm_count();
+  for (int ks = full; ks >= 2; --ks)
+    if (ctas <= sms * kernel_setup(cache, kernel, 0, ks * 32, 0, ks, dev)) return ks;
+  return full;
+}
 
 template <typename T>
 __device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1);

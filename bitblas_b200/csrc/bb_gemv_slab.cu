@@ -673,40 +673,14 @@ bool get_w_map(CUtensorMap* tm, const void* W, int N, int K) {
 }
 
 
-// CTAs per SM of one instance on the current device (< 0: it does not fit), queried once per device; the shared-memory opt-in
-// (the device maximum) is a per-device function attribute
-template <typename T, bool IL, int FMT>
-int gs_occupancy(int dev) {
-  static std::atomic<int> occ_dev[BB_MAX_DEVICES];   // 0 = not queried yet
-  int occ = occ_dev[dev].load(std::memory_order_relaxed);
-  if (occ == 0) {
-    auto k = gemv_slab_kernel<T, IL, FMT>;
-    int optin = 0;
-    if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess) { cudaGetLastError(); return -1; }
-    if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, optin) != cudaSuccess) { cudaGetLastError(); return -1; }
-    int o = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, k, GS_THREADS, size_t(GS_SMEM_BYTES)) != cudaSuccess) { cudaGetLastError(); o = 0; }
-    occ = o < 1 ? -1 : o;
-    occ_dev[dev].store(occ, std::memory_order_relaxed);
-  }
-  return occ;
-}
-
 template <typename T, bool IL, int FMT>
 int launch_slab(const MatmulArgs& a, const CUtensorMap& tm, const SlabParams& p) {
-  const int occ = gs_occupancy<T, IL, FMT>(current_device());
-  if (occ < 0) { set_error("gemv_slab: kernel does not fit on this device"); return 4; }
+  auto kernel = gemv_slab_kernel<T, IL, FMT>;
+  static KernelCache<> cache;
+  const int occ = kernel_setup(cache, kernel, kSmemOptinMax, GS_THREADS, GS_SMEM_BYTES);
+  if (occ < 1) { set_error("gemv_slab: kernel does not fit on this device"); return 4; }
   const int grid = std::max(1, std::min(p.T, std::min(occ, GS_MINB) * device_sm_count()));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(GS_THREADS);
-  cfg.dynamicSmemBytes = GS_SMEM_BYTES; cfg.stream = a.stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemv_slab_kernel<T, IL, FMT>, tm, p));
-  BB_LAUNCH_CHECK();
-  return 0;
+  return launch_pdl(kernel, grid, GS_THREADS, GS_SMEM_BYTES, a.stream, pdl_enabled(), tm, p);
 }
 
 }  // namespace

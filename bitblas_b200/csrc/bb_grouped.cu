@@ -74,51 +74,24 @@ gemv_grouped_kernel(const GroupedParams g) {
   pdl_launch_dependents();
 }
 
-// CTAs of ks warps resident on the device; occ_cache (one per instance) holds the per-SM count, -1 until queried
+// K splits (warps per CTA) as the decode GEMV picks them, for an upper bound of the work items as the CTA count; the grid is
+// that bound, capped at the resident CTAs.
 template <typename KernelT>
-int resident_ctas(KernelT kernel, int (&occ_cache)[MAX_KS + 1], int ks) {
-  if (occ_cache[ks] < 0) {
-    int occ = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, ks * 32, 0) != cudaSuccess) { cudaGetLastError(); occ = 0; }
-    occ_cache[ks] = occ;
-  }
-  return occ_cache[ks] * device_sm_count();
-}
-
-// K splits (warps per CTA): the largest count for which an upper bound of the work items fits in one resident wave, as the
-// decode GEMV chooses it; the grid is that bound, capped at the resident CTAs.
-template <typename KernelT>
-int launch_grouped_kernel(KernelT kernel, int (&occ_cache)[MAX_KS + 1], GroupedParams g, int max_items, int max_ks,
+int launch_grouped_kernel(KernelT kernel, KernelCache<MAX_KS + 1>& cache, GroupedParams g, int max_items, int max_ks,
                           cudaStream_t stream) {
-  const int steps = g.p.K / 128;
-  int ks = std::max(1, std::min(max_ks, steps));
-  for (int k = ks; k >= 2; --k) {
-    if (max_items <= resident_ctas(kernel, occ_cache, k)) { ks = k; break; }
-  }
+  const int ks = pick_ks(cache, kernel, max_ks, max_items, g.p.K / 128);
   g.p.ks = ks;
-  const int resident = resident_ctas(kernel, occ_cache, ks);
+  const int resident = kernel_setup(cache, kernel, 0, ks * 32, 0, ks) * device_sm_count();
   if (resident <= 0) { set_error("grouped matmul: the kernel cannot be resident on this device"); return 2; }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(std::min(max_items, resident));
-  cfg.blockDim = dim3(ks * 32);
-  cfg.dynamicSmemBytes = 0;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, g));
-  BB_LAUNCH_CHECK();
-  return 0;
+  return launch_pdl(kernel, std::min(max_items, resident), ks * 32, 0, stream, pdl_enabled(), g);
 }
 
 template <typename T, int BITS, bool IL, bool SWIGLU>
 int launch_grouped_nt(const GroupedParams& g, int nt, const int (&max_items)[3], cudaStream_t s) {
 #define BB_GROUPED_GO(NTV, ZKV, SCV, MAXKS)                                                                   \
   {                                                                                                          \
-    static int occ_cache[MAX_KS + 1] = {-1, -1, -1, -1, -1, -1, -1, -1, -1};                                 \
-    return launch_grouped_kernel(gemv_grouped_kernel<T, BITS, IL, NTV, ZKV, SCV, SWIGLU>, occ_cache, g,     \
+    static KernelCache<MAX_KS + 1> cache;                                                                    \
+    return launch_grouped_kernel(gemv_grouped_kernel<T, BITS, IL, NTV, ZKV, SCV, SWIGLU>, cache, g,         \
                                  max_items[NTV == 1 ? 0 : (NTV == 2 ? 1 : 2)], MAXKS, s);                    \
   }
 #define BB_GROUPED_NT(ZKV, SCV)                     \
@@ -169,35 +142,16 @@ bool grouped_supported(const bb_matmul_desc& d) {
   return true;
 }
 
-int launch_grouped(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
-                   const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream,
-                   bool swiglu) {
-  MatmulArgs a = {};
-  a.d = d; a.A = A; a.W = W; a.scale = scale; a.zeros = zeros; a.bias = bias; a.C = C; a.m = total_rows; a.n_peers = 0;
+int launch_grouped(const GroupedArgs& a) {
+  const bb_matmul_desc& d = a.d;
   GroupedParams g;
-  GemvParams& p = g.p;
-  p.A = A; p.W = reinterpret_cast<const uint8_t*>(W);
-  p.scale = d.with_scaling ? scale : nullptr;
-  p.zeros = d.with_zeros ? zeros : nullptr;
-  p.bias = d.with_bias ? bias : nullptr;
-  p.out = make_outspec(a);
-  if (swiglu) p.out.ld = d.N / 2;
-  p.M = 0; p.N = d.N; p.K = d.K;
-  p.g = a.gsize(); p.G = a.groups();
-  p.with_scaling = d.with_scaling;
-  p.zmode = d.with_zeros ? (d.zeros_mode + 1) : 0;
-  p.zp_const = (d.w_fmt == BB_W_INT) ? (1 << (d.w_bits - 1)) : 0;
-  p.out_dtype = d.out_dtype;
-  p.ks = 1;
-  const long long N = d.N, G = p.G;
-  g.offsets = offsets; g.E = num_groups; g.T = total_rows;
-  g.w_stride = N * d.K * d.w_bits / 8;
-  g.s_stride = N * G * 2;
-  g.z_stride = d.zeros_mode == BB_ZEROS_QUANTIZED ? G * (N * d.w_bits / 8) : N * G * 2;
-  g.b_stride = N * 2;
+  g.p = make_params(d, a.A, a.W, a.scale, a.zeros, a.bias, make_outspec(a.C, a.swiglu ? d.N / 2 : d.N), 0);
+  g.offsets = a.offsets; g.E = a.num_groups; g.T = a.total_rows;
+  g.w_stride = a.w_stride; g.s_stride = a.s_stride; g.z_stride = a.z_stride; g.b_stride = a.b_stride;
   g.out_bytes = int(elem_bytes(d.out_dtype));
   // rows per pass: 8, 16 or 32, from the mean rows per active group (T rows over at most min(E, T) groups)
-  const int active = std::min(num_groups, total_rows);
+  const int total_rows = a.total_rows;
+  const int active = std::min(a.num_groups, total_rows);
   const int mean_rows = (total_rows + active - 1) / active;
   const int nt = mean_rows <= 8 ? 1 : (mean_rows <= 16 ? 2 : 4);
   // work items: sum_e ceil(m_e / R) row chunks per 16-row block <= T / R + (groups with rows)
@@ -210,7 +164,8 @@ int launch_grouped(const bb_matmul_desc& d, int num_groups, const int32_t* offse
     max_items[i] = int(items);
   }
   const bool il = d.w_layout == BB_LAYOUT_INTERLEAVED_16;
-  return swiglu ? launch_grouped_typed<true>(d, il, g, nt, max_items, stream) : launch_grouped_typed<false>(d, il, g, nt, max_items, stream);
+  return a.swiglu ? launch_grouped_typed<true>(d, il, g, nt, max_items, a.stream)
+                  : launch_grouped_typed<false>(d, il, g, nt, max_items, a.stream);
 }
 
 }  // namespace bb

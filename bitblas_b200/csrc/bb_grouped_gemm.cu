@@ -332,15 +332,9 @@ int launch_grouped_gemm_inst(const GroupedTsParams& g, const void* A, const void
   using SM = TsSmem<T, BITS, BM>;
   auto kernel = gemm_ts_grouped_kernel<T, BITS, BM, IL, SWIGLU, GATHER>;
   constexpr int threads = grouped_threads<GATHER>();
-  static int resident_per_sm[BB_MAX_DEVICES] = {};   // 0 until queried (cudaFuncSetAttribute is per device)
-  const int dev = current_device();
-  if (!resident_per_sm[dev]) {
-    BB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kTotal));
-    int occ = 0;
-    BB_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, SM::kTotal));
-    if (occ <= 0) { set_error("grouped GEMM: the kernel cannot be resident on this device"); return 2; }
-    resident_per_sm[dev] = occ;
-  }
+  static KernelCache<> cache;
+  const int resident_per_sm = kernel_setup(cache, kernel, SM::kTotal, threads, SM::kTotal);
+  if (resident_per_sm <= 0) { set_error("grouped GEMM: the kernel cannot be resident on this device"); return 2; }
   CUtensorMap tmA, tmW;
   const CUtensorMapDataType adt = std::is_same<T, __half>::value ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   const TsParams& p = g.p;
@@ -355,19 +349,8 @@ int launch_grouped_gemm_inst(const GroupedTsParams& g, const void* A, const void
                      CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(unsigned(std::min<long long>(max_tiles, (long long)resident_per_sm[dev] * device_sm_count())));
-  cfg.blockDim = dim3(threads);
-  cfg.dynamicSmemBytes = SM::kTotal;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, tmA, tmW, g));
-  BB_LAUNCH_CHECK();
-  return 0;
+  const unsigned grid = unsigned(std::min<long long>(max_tiles, (long long)resident_per_sm * device_sm_count()));
+  return launch_pdl(kernel, grid, threads, SM::kTotal, stream, pdl_enabled(), tmA, tmW, g);
 }
 
 template <typename T, int BITS, bool IL, bool SWIGLU, bool GATHER>
@@ -406,35 +389,22 @@ bool grouped_gemm_supported(const bb_matmul_desc& d) {
   return true;
 }
 
-int launch_grouped_gemm(const bb_matmul_desc& d, int num_groups, const int32_t* offsets, const void* A, const void* W,
-                        const void* scale, const void* zeros, const void* bias, void* C, int total_rows, cudaStream_t stream,
-                        bool swiglu, const int32_t* row_index, int a_rows) {
-  MatmulArgs a = {};
-  a.d = d; a.A = A; a.W = W; a.scale = scale; a.zeros = zeros; a.bias = bias; a.C = C; a.m = total_rows; a.n_peers = 0;
+int launch_grouped_gemm(const GroupedArgs& a) {
+  const bb_matmul_desc& d = a.d;
   GroupedTsParams g;
-  TsParams& p = g.p;
-  p.scale = d.with_scaling ? scale : nullptr;
-  p.zeros = d.with_zeros ? zeros : nullptr;
-  p.bias = d.with_bias ? bias : nullptr;
-  p.out = make_outspec(a); p.M = total_rows; p.N = d.N; p.K = d.K; p.g = a.gsize(); p.G = a.groups();
-  p.mode = !d.with_scaling ? 0 : (!d.with_zeros ? 1 : 2 + d.zeros_mode);
-  p.zp_const = d.w_fmt == BB_W_INT ? (1 << (d.w_bits - 1)) : 0;
-  p.out_dtype = d.out_dtype; p.a_dtype = d.a_dtype; p.m_tiles = 1;
-  p.splits = 1; p.kb_per_split = d.K / 64; p.ws = nullptr;
-  p.lut = nullptr; p.w_fmt = d.w_fmt; p.w_tiled = 0;
-  const long long N = d.N, G = p.G;
-  g.offsets = offsets; g.E = num_groups; g.T = total_rows;
-  g.s_stride = N * G * 2;
-  g.z_stride = d.zeros_mode == BB_ZEROS_QUANTIZED ? G * (N * d.w_bits / 8) : N * G * 2;
-  g.b_stride = N * 2;
-  g.row_index = row_index; g.a = A; g.a_rows = a_rows;
-  if ((N / TS_ROWS) * ((total_rows + 31) / 32 + std::min(num_groups, total_rows)) > INT_MAX) {
+  g.p = make_ts_params(d, a.scale, a.zeros, a.bias, nullptr, make_outspec(a.C, d.N), a.total_rows);
+  g.p.splits = 1; g.p.kb_per_split = d.K / 64; g.p.ws = nullptr; g.p.w_tiled = 0;
+  g.offsets = a.offsets; g.E = a.num_groups; g.T = a.total_rows;
+  g.s_stride = a.s_stride; g.z_stride = a.z_stride; g.b_stride = a.b_stride;
+  g.row_index = a.row_index; g.a = a.A; g.a_rows = a.a_rows;
+  if ((long long)(d.N / TS_ROWS) * ((a.total_rows + 31) / 32 + std::min(a.num_groups, a.total_rows)) > INT_MAX) {
     set_error("grouped GEMM: N/128 x (T/32 + groups) exceeds 2^31 tiles");
     return 1;
   }
   const bool il = d.w_layout == BB_LAYOUT_INTERLEAVED_16;
-  if (row_index) return launch_grouped_gemm_typed<true, true>(d, il, g, A, W, stream);
-  return swiglu ? launch_grouped_gemm_typed<true>(d, il, g, A, W, stream) : launch_grouped_gemm_typed<false>(d, il, g, A, W, stream);
+  if (a.row_index) return launch_grouped_gemm_typed<true, true>(d, il, g, a.A, a.W, a.stream);
+  return a.swiglu ? launch_grouped_gemm_typed<true>(d, il, g, a.A, a.W, a.stream)
+                  : launch_grouped_gemm_typed<false>(d, il, g, a.A, a.W, a.stream);
 }
 
 }  // namespace bb

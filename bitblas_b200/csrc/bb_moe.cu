@@ -211,13 +211,6 @@ __global__ void __launch_bounds__(256) moe_combine_kernel(const CombineParams c)
   pdl_launch_dependents();
 }
 
-cudaLaunchAttribute pdl_attr() {
-  cudaLaunchAttribute a;
-  a.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  a.val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  return a;
-}
-
 }  // namespace
 
 // x_sorted == nullptr: the INDEX instance, which writes row_token instead of copying x
@@ -225,29 +218,16 @@ int launch_moe_route(const int32_t* topk_ids, int n_slots, int top_k, int num_ex
                      int32_t* slot_rows, void* x_sorted, int32_t* row_token, cudaStream_t stream) {
   const bool index = x_sorted == nullptr;
   auto kernel = index ? moe_route_kernel<true> : moe_route_kernel<false>;
-  static int resident_per_sm[2][BB_MAX_DEVICES] = {};
-  const int dev = current_device();
-  if (!resident_per_sm[index][dev]) {
-    int occ = 0;
-    BB_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, ROUTE_THREADS, 0));
-    if (occ <= 0) { set_error("moe route: the kernel cannot be resident on this device"); return 2; }
-    resident_per_sm[index][dev] = std::min(occ, ROUTE_CTAS_PER_SM);
-  }
+  static KernelCache<> cache[2];   // [index]
+  const int occ = kernel_setup(cache[index], kernel, 0, ROUTE_THREADS);
+  if (occ <= 0) { set_error("moe route: the kernel cannot be resident on this device"); return 2; }
   RouteParams r;
   r.ids = topk_ids; r.x = reinterpret_cast<const uint4*>(x); r.offsets = offsets; r.slot_rows = slot_rows;
   r.x_sorted = reinterpret_cast<uint4*>(x_sorted); r.n = n_slots; r.k = top_k; r.E = num_experts; r.vecs = K / 8;
   r.row_token = row_token;
-  const int resident = resident_per_sm[index][dev] * device_sm_count();
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(std::max(1, std::min((n_slots + ROUTE_MIN_SLOTS - 1) / ROUTE_MIN_SLOTS, resident)));
-  cfg.blockDim = dim3(ROUTE_THREADS);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1] = {pdl_attr()};
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, r));
-  BB_LAUNCH_CHECK();
-  return 0;
+  const int resident = std::min(occ, ROUTE_CTAS_PER_SM) * device_sm_count();
+  const int grid = std::max(1, std::min((n_slots + ROUTE_MIN_SLOTS - 1) / ROUTE_MIN_SLOTS, resident));
+  return launch_pdl(kernel, grid, ROUTE_THREADS, 0, stream, pdl_enabled(), r);
 }
 
 int launch_moe_combine(const int32_t* slot_rows, const float* topk_weights, const void* Y, int out_dtype, void* out,
@@ -256,18 +236,9 @@ int launch_moe_combine(const int32_t* slot_rows, const float* topk_weights, cons
   c.slot_rows = slot_rows; c.w = topk_weights; c.Y = Y; c.out = out; c.k = top_k; c.cols8 = N / 8;
   c.T = num_tokens; c.n = (long long)num_tokens * top_k; c.out_dtype = out_dtype;
   const long long threads = c.T * c.cols8;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(unsigned((threads + 255) / 256));
-  cfg.blockDim = dim3(256);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1] = {pdl_attr()};
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  if (out_dtype == BB_F16) BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, moe_combine_kernel<__half>, c));
-  else if (out_dtype == BB_BF16) BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, moe_combine_kernel<__nv_bfloat16>, c));
-  else BB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, moe_combine_kernel<float>, c));
-  BB_LAUNCH_CHECK();
-  return 0;
+  auto kernel = out_dtype == BB_F16 ? moe_combine_kernel<__half>
+                                    : (out_dtype == BB_BF16 ? moe_combine_kernel<__nv_bfloat16> : moe_combine_kernel<float>);
+  return launch_pdl(kernel, unsigned((threads + 255) / 256), 256, 0, stream, pdl_enabled(), c);
 }
 
 }  // namespace bb

@@ -569,10 +569,7 @@ class Matmul(Operator):
         with torch.cuda.device(dev):   # the kernels launch on the calling thread's current device
             if T <= GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E or capturable:
                 name = "bb_matmul_grouped" if self._grouped_single_launch(T, E) == "gemv" else "bb_matmul_grouped_gemm"
-                rc = getattr(self.lib._c, name)(self._desc_ref, E, offsets.data_ptr(), A.data_ptr(), *ptrs, output.data_ptr(),
-                                                T, stream)
-                if rc != 0:
-                    raise RuntimeError(f"{name} failed (code {rc}): {_lib.last_error()}")
+                self._grouped_call(name, dev, E, offsets.data_ptr(), A.data_ptr(), *ptrs, output.data_ptr(), T, stream)
             else:
                 self._forward_grouped_per_group(A, W, offsets, scale, zeros, bias, output, dev, stream)
         return output
@@ -595,11 +592,7 @@ class Matmul(Operator):
         E, T, ptrs, output, dev, stream = self._grouped_prepare(A, W, offsets, scale, zeros, bias, output, self.config.N // 2,
                                                                 swiglu=True)
         name = "bb_matmul_grouped_swiglu" if self._grouped_single_launch(T, E) == "gemv" else "bb_matmul_grouped_gemm_swiglu"
-        with torch.cuda.device(dev):
-            rc = getattr(self.lib._c, name)(self._desc_ref, E, offsets.data_ptr(), A.data_ptr(), *ptrs, output.data_ptr(), T,
-                                            stream)
-        if rc != 0:
-            raise RuntimeError(f"{name} failed (code {rc}): {_lib.last_error()}")
+        self._grouped_call(name, dev, E, offsets.data_ptr(), A.data_ptr(), *ptrs, output.data_ptr(), T, stream)
         return output
 
     def _forward_grouped_swiglu_gather(self, A, W, offsets, scale, zeros, bias, output, row_index):
@@ -615,12 +608,16 @@ class Matmul(Operator):
             raise ValueError("row_index must be on A's device")
         if T > 0 and A.shape[0] < 1:
             raise ValueError("A must have at least one row to gather from")
-        with torch.cuda.device(dev):
-            rc = self.lib._c.bb_matmul_grouped_gemm_swiglu_gather(self._desc_ref, E, offsets.data_ptr(), row_index.data_ptr(),
-                                                                   A.data_ptr(), A.shape[0], *ptrs, output.data_ptr(), T, stream)
-        if rc != 0:
-            raise RuntimeError(f"{name} failed (code {rc}): {_lib.last_error()}")
+        self._grouped_call(name, dev, E, offsets.data_ptr(), row_index.data_ptr(), A.data_ptr(), A.shape[0], *ptrs,
+                           output.data_ptr(), T, stream)
         return output
+
+    def _grouped_call(self, name, dev, *args):
+        """the grouped library entry point `name` on this operator's descriptor, launched on `dev` (the kernels run on the calling
+        thread's current device); raises RuntimeError with the library's message when it fails"""
+        with torch.cuda.device(dev):
+            rc = getattr(self.lib._c, name)(self._desc_ref, *args)
+        _lib.check(rc, name)
 
     def _grouped_single_launch(self, T: int, E: int) -> str:
         """the kernel of the one capturable grouped launch for T rows over E groups: the grouped GEMV ("gemv") up to

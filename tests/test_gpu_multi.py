@@ -106,3 +106,24 @@ def test_one_process_two_devices():
             torch.cuda.synchronize(dev)
             H.assert_fp_close(out.cpu(), ref, f"M={M} on {dev}")
             assert torch.cuda.current_device() == 0, "the library changed the caller's current device"
+    # one grouped launch over 4 experts: the grouped GEMV at <= 8 rows per expert, the grouped wgmma GEMM (> 48 KB of dynamic
+    # shared memory) above
+    E, N, K = 4, 256, 2048
+    experts = [H.make_case(1, N, K, W_dtype="uint4", group_size=128, with_scaling=True, with_zeros=True, zeros_mode="quantized",
+                           seed=100 + e) for e in range(E)]
+    op = H.product_operator(experts[0], M=[1, 16])
+    for rows, kernel in ((5, "gemv"), (40, "gemm")):
+        T = rows * E
+        A = (torch.rand((T, K), generator=torch.Generator().manual_seed(rows)) - 0.5).to(experts[0]["A"].dtype)
+        ref = torch.cat([H.oracle_output(dict(c, A=A[e * rows:(e + 1) * rows]), fast_decoding=bool(op.fast_decoding))
+                         for e, c in enumerate(experts)])
+        for dev in ("cuda:1", "cuda:0", "cuda:1"):
+            W = torch.stack([H.product_weight(op, c, dev) for c in experts])
+            scale, zeros = (torch.stack([c[k] for c in experts]).to(dev) for k in ("scale", "zeros"))
+            offsets = torch.arange(0, T + 1, rows, dtype=torch.int32, device=dev)
+            out = op.forward_grouped(A.to(dev), W, offsets, scale=scale, zeros=zeros, capturable=True)
+            assert op._grouped_single_launch(T, E) == kernel
+            assert out.device == torch.device(dev)
+            torch.cuda.synchronize(dev)
+            H.assert_fp_close(out.cpu(), ref, f"grouped {kernel}, {rows} rows per expert on {dev}")
+            assert torch.cuda.current_device() == 0, "the library changed the caller's current device"
