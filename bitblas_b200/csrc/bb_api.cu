@@ -424,6 +424,30 @@ int bb_moe_combine(const int32_t* slot_rows, const float* topk_weights, const vo
   return launch_moe_combine(slot_rows, topk_weights, Y, out_dtype, out, num_tokens, top_k, N, (cudaStream_t)stream);
 }
 
+int bb_permute_cols(const void* A, void* out, const int32_t* perm, int rows, int K, int a_dtype, int num_groups,
+                    const int32_t* offsets, void* stream) {
+  if (a_dtype != BB_F16 && a_dtype != BB_BF16) { set_error("permute cols: A must be float16 or bfloat16 (a_dtype=%d)", a_dtype); return 1; }
+  if (K <= 0 || K % 8) { set_error("permute cols: needs K > 0 and K %% 8 == 0 (K=%d)", K); return 1; }
+  if (K > PERMUTE_MAX_K) { set_error("permute cols: K=%d exceeds %d (one row is staged in shared memory)", K, PERMUTE_MAX_K); return 1; }
+  if (num_groups < 1 || num_groups > BB_GROUPED_MAX_GROUPS) {
+    set_error("permute cols: num_groups must be in [1, %d] (got %d)", BB_GROUPED_MAX_GROUPS, num_groups);
+    return 1;
+  }
+  if (num_groups > 1 && !offsets) { set_error("permute cols: num_groups > 1 needs offsets (a device pointer to num_groups + 1 int32 values)"); return 1; }
+  if (rows < 0) { set_error("permute cols: rows must be >= 0 (got %d)", rows); return 1; }
+  if (rows == 0) return 0;
+  if (!A || !out || !perm) { set_error("permute cols: A, out and perm must be non-null"); return 1; }
+  if ((reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(out) & 15)) {
+    set_error("permute cols: A and out must be 16-byte aligned");
+    return 5;
+  }
+  if ((reinterpret_cast<uintptr_t>(perm) & 3) || (reinterpret_cast<uintptr_t>(offsets) & 3)) {
+    set_error("permute cols: perm and offsets must be 4-byte aligned");
+    return 5;
+  }
+  return launch_permute_cols(A, out, perm, rows, K, num_groups, offsets, (cudaStream_t)stream);
+}
+
 int bb_peer_barrier(void* const* peer_flags, int n_peers, int rank, void* stream) {
   if (!peer_flags || n_peers < 1 || n_peers > BB_MAX_PEERS || rank < 0 || rank >= n_peers) {
     set_error("bb_peer_barrier: need 1 <= n_peers <= %d flag blocks and 0 <= rank < n_peers", BB_MAX_PEERS);

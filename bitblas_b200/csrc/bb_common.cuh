@@ -168,6 +168,11 @@ int launch_moe_route(const int32_t* topk_ids, int n_slots, int top_k, int num_ex
                      int32_t* slot_rows, void* x_sorted, int32_t* row_token, cudaStream_t stream);
 int launch_moe_combine(const int32_t* slot_rows, const float* topk_weights, const void* Y, int out_dtype, void* out,
                        int num_tokens, int top_k, int N, cudaStream_t stream);
+// act-order column gather, bb_permute.cu (validated by bb_api.cu): one row of A is staged in shared memory, so K <= PERMUTE_MAX_K
+// (H100: 227 KB per block, less the 3 KB of the kernel's static arrays)
+constexpr int PERMUTE_MAX_K = 112640;
+int launch_permute_cols(const void* A, void* out, const int32_t* perm, int rows, int K, int num_groups, const int32_t* offsets,
+                        cudaStream_t stream);
 
 // bit position of logical element `o` (0 .. 32/bits-1) inside its 32-bit storage word, for each weight
 // layout (restates bitblas/quantization/utils.py:73-110 + testing/cpp/lop3_type_conversion/fast_decoding.hpp:30-95,607-668)

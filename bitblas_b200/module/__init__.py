@@ -17,7 +17,7 @@ from typing import List, Optional, Union
 import torch
 import torch.nn as nn
 
-from .. import _lib
+from .. import _lib, act_order
 from ..cache import get_database_path, global_operator_cache
 from ..ops.general_matmul import Matmul, MatmulConfig
 from ..quantization.utils import general_compress
@@ -26,6 +26,13 @@ from ..utils import auto_detect_nvidia_target
 logger = getLogger(__name__)
 
 BITBLAS_DATABASE_PATH = get_database_path()
+
+
+def _load_perm_from_state_dict(layer, state_dict, prefix):
+    """`perm` is a buffer only on act-order layers (a layer without it keeps the reference's state_dict): take its presence and
+    shape from the state dict being loaded, so that a strict load works in either direction."""
+    saved = state_dict.get(prefix + "perm")
+    layer.perm = None if saved is None else torch.empty_like(saved, device=layer.scales.device)
 
 
 def unpack_qzeros(qzeros, bits):
@@ -94,6 +101,9 @@ class Linear(nn.Module):
             self.register_buffer(name, torch.zeros(shape, dtype=dtype))
         if not bias:
             self.bias = None
+        # GPTQ act-order: int32 [K], sorted column j of qweight is input column perm[j]; None (and absent from the state_dict)
+        # for every other layer
+        self.register_buffer("perm", None)
         self.q_params = None
         self._q_param_key = None
 
@@ -162,6 +172,8 @@ class Linear(nn.Module):
             self.init_params()
         if output is None:
             output = torch.empty(A.shape[:-1] + (self.out_features,), dtype=getattr(torch, op.out_dtype), device=A.device)
+        if self.perm is not None:   # act-order: the weight's K axis is sorted, so A's columns are gathered to match
+            A = act_order.permute_cols(A.view(-1, self.in_features), self.perm).view(A.shape)
         args = [ctypes.c_void_p(A.data_ptr()), *self.q_params, ctypes.c_void_p(output.data_ptr())]
         if op.dynamic_range is not None:
             args.append(reduce(operator.mul, A.shape[:-1], 1))
@@ -187,10 +199,17 @@ class Linear(nn.Module):
                 self.zeros = zeros
             if bias is not None:
                 self.bias = bias
+            self.perm = None   # field values come in input-column order
         self.q_params = None
 
+    def _load_from_state_dict(self, state_dict, prefix, *args, **kwargs):
+        if not self.consistent:
+            _load_perm_from_state_dict(self, state_dict, prefix)
+        super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)
+
     def _repack(self, gptq_module, device, v2: bool):
-        """module/__init__.py:315-363 as two device kernels (qweight transpose+permute, qzeros unpack)."""
+        """module/__init__.py:315-363 as two device kernels (qweight transpose+permute, qzeros unpack).  An act-order module
+        (g_idx, see act_order.py) has its qweight's K axis sorted first and keeps the order in `perm`."""
         lib = _lib.load()
         dev = torch.device(device)
         if dev.type != "cuda":
@@ -202,6 +221,12 @@ class Linear(nn.Module):
         qw = gptq_module.qweight.to(dev).contiguous().view(torch.int32)  # [K*bits/32, N]
         K, N = self.in_features, self.out_features
         assert qw.shape == (K * bits // 32, N), f"unexpected GPTQ qweight shape {tuple(qw.shape)}"
+        perm = act_order.perm_from_g_idx(getattr(gptq_module, "g_idx", None), K, self.group_size)
+        if perm is not None:
+            if self.torch_dtype not in (torch.float16, torch.bfloat16):
+                raise ValueError("act-order GPTQ checkpoints need float16 or bfloat16 activations (the column gather)")
+            perm = perm.to(dev)
+            qw = act_order.permute_gptq_qweight(qw, perm, bits)
         out = torch.empty(op.retrieve_weight_shape(), dtype=torch.int8, device=dev)
         tgt = op.weight_transform.interleave_target if op.weight_transform is not None else 0
         with torch.cuda.device(dev):
@@ -222,6 +247,7 @@ class Linear(nn.Module):
             self.zeros = zeros
         if self.bias is not None:
             self.bias = gptq_module.bias.data.to(dev).to(torch.float16).contiguous()
+        self.perm = perm
         self.q_params = None
 
     def repack_from_gptq(self, gptq_module, device="cuda"):
@@ -239,7 +265,8 @@ class GroupedLinear(nn.Module):
     """E quantized linear layers of one shape -- the experts of a mixture-of-experts projection -- run as one grouped matmul
     (``Matmul.forward_grouped``).  Constructor arguments after ``num_groups`` are those of ``Linear``; the buffers are
     ``Linear``'s stacked over the experts: ``qweight`` [E, N, K*bits/8], ``scales`` [E, N, K/g], ``zeros`` [E, N, K/g] (or
-    [E, K/g, N*bits/8] for ``zeros_mode="quantized"``) and ``bias`` [E, N].  ``forward(A, offsets)`` takes the activations sorted
+    [E, K/g, N*bits/8] for ``zeros_mode="quantized"``), ``bias`` [E, N] and, when some expert's GPTQ checkpoint is act-order,
+    ``perm`` int32 [E, K] (the identity for the other experts), which ``forward`` gathers the activations with.  ``forward(A, offsets)`` takes the activations sorted
     by expert and the int32 device row offsets [E + 1]; routing, top-k weighting and combining stay with the caller (``MoEExperts``
     runs the whole SwiGLU expert block)."""
 
@@ -263,11 +290,19 @@ class GroupedLinear(nn.Module):
             self.register_buffer(name, torch.zeros((num_groups, *shape), dtype=dtype))
         if not bias:
             self.bias = None
+        self.register_buffer("perm", None)
+
+    def _load_from_state_dict(self, state_dict, prefix, *args, **kwargs):
+        _load_perm_from_state_dict(self, state_dict, prefix)
+        super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)
 
     def forward(self, A, offsets, output=None, capturable=False):
-        """capturable=True: one graph-capturable launch at every token count (see Matmul.forward_grouped)"""
+        """capturable=True: one graph-capturable launch at every token count (see Matmul.forward_grouped); an act-order layer
+        launches the grouped column gather (act_order.permute_cols) first"""
         op = self.bitblas_matmul
         cfg = op.config
+        if self.perm is not None:
+            A = act_order.permute_cols(A, self.perm, offsets)
         return op.forward_grouped(A, self.qweight, offsets, scale=self.scales if cfg.with_scaling else None,
                                   zeros=self.zeros if cfg.with_zeros else None, bias=self.bias, output=output,
                                   capturable=capturable)
@@ -285,9 +320,12 @@ class GroupedLinear(nn.Module):
             self.zeros = zeros
         if bias is not None:
             self.bias = bias
+        self.perm = None
 
-    def _repack(self, gptq_modules, device, v2: bool):
-        """Linear's device repack (bb_repack_gptq_*_device) per expert, copied into the expert's slice of the stacked buffers."""
+    def _repack(self, gptq_modules, device, v2: bool, keep_perm: bool = True):
+        """Linear's device repack (bb_repack_gptq_*_device) per expert, copied into the expert's slice of the stacked buffers.
+        keep_perm=False: the act-order experts' K axes are sorted, but the caller feeds inputs already in that order (MoEExperts'
+        down projection, whose perm is absorbed into the gate/up rows), so no perm is kept."""
         from types import SimpleNamespace
         if len(gptq_modules) != self.num_groups:
             raise ValueError(f"expected {self.num_groups} GPTQ modules, got {len(gptq_modules)}")
@@ -298,6 +336,7 @@ class GroupedLinear(nn.Module):
             t = getattr(self, name)
             if t is not None and t.device != dev:
                 setattr(self, name, t.to(dev))
+        perms = []
         for e, gm in enumerate(gptq_modules):
             one = SimpleNamespace(**self._expert_attrs, bias=None if self.bias is None else self.bias[e])
             Linear._repack(one, gm, dev, v2)
@@ -306,6 +345,8 @@ class GroupedLinear(nn.Module):
             self.zeros[e].copy_(one.zeros)
             if self.bias is not None:
                 self.bias[e].copy_(one.bias)
+            perms.append(one.perm)
+        self.perm = act_order.stack_perms(perms, self.in_features, dev) if keep_perm else None
 
     def repack_from_gptq(self, gptq_modules, device="cuda"):
         """one GPTQ QuantLinear per expert (how GPTQ mixture-of-experts checkpoints store them)"""

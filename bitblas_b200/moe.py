@@ -161,7 +161,12 @@ class MoEExperts(nn.Module):
     ``y[t] = sum_j w[t, j] * down_e(silu(gate_e(x[t])) * up_e(x[t]))`` with e = topk_ids[t, j], as four library launches with no
     host synchronisation (CUDA-graph capturable): moe_route -> grouped gate/up with SwiGLU in the epilogue -> grouped down ->
     moe_combine.  ``gate_up`` (H -> 2I, gate/up interleaved) and ``down`` (I -> H) are ``GroupedLinear``s built from the
-    ``Linear`` keyword arguments; ``out_dtype`` must equal ``A_dtype`` (the gate/up output is the down projection's input)."""
+    ``Linear`` keyword arguments; ``out_dtype`` must equal ``A_dtype`` (the gate/up output is the down projection's input).
+
+    GPTQ act-order experts (act_order.py): the gate/up projections' column order is ``gate_up.perm`` [E, H], and ``forward`` gathers
+    the routed rows with it (one more launch, five in all).  The down projection's order costs nothing at run time: each expert's
+    gate and up output rows are loaded in that order, so the SwiGLU output arrives already sorted for the down projection's K axis.
+    The copy-free path (moe_route_index + forward_grouped_swiglu(row_index=)) cannot apply a column order."""
 
     def __init__(self, num_experts: int, hidden_size: int, intermediate_size: int, bias: bool = False, **linear_kwargs):
         super().__init__()
@@ -185,6 +190,9 @@ class MoEExperts(nn.Module):
             raise ValueError("topk_ids and topk_weights must have the same [T, k] shape")
         offsets, slot_rows, x_sorted = moe_route(topk_ids, x, self.num_experts)
         gu, cfg = self.gate_up, self.gate_up.bitblas_matmul.config
+        if gu.perm is not None:
+            from .act_order import permute_cols
+            x_sorted = permute_cols(x_sorted, gu.perm, offsets)
         h = gu.bitblas_matmul.forward_grouped_swiglu(x_sorted, gu.qweight, offsets, gu.scales if cfg.with_scaling else None,
                                                      gu.zeros if cfg.with_zeros else None, gu.bias)
         y = self.down(h, offsets, capturable=True)
@@ -205,7 +213,23 @@ class MoEExperts(nn.Module):
         self.down.load_and_transform_weight(*down)
 
     def _repack(self, gate_modules, up_modules, down_modules, device, v2):
+        from .act_order import perm_from_g_idx, permute_gptq_rows
         from .module import GroupedLinear
+        E, H, I = self.num_experts, self.hidden_size, self.intermediate_size
+        if not len(gate_modules) == len(up_modules) == len(down_modules) == E:
+            raise ValueError(f"expected {E} GPTQ modules per projection, got {len(gate_modules)}, {len(up_modules)}, {len(down_modules)}")
+        gate_modules, up_modules = list(gate_modules), list(up_modules)
+        for e in range(E):
+            pg, pu = (perm_from_g_idx(getattr(m[e], "g_idx", None), H, self.gate_up.group_size) for m in (gate_modules, up_modules))
+            if (pg is None) != (pu is None) or (pg is not None and not torch.equal(pg.cpu(), pu.cpu())):
+                raise ValueError(f"expert {e}: gate and up have different g_idx; they read the same input, so act-order "
+                                 "checkpoints must give them the same column order")
+            # the down projection's column order, absorbed into the gate/up output rows: h comes out in its sorted K order
+            pd = perm_from_g_idx(getattr(down_modules[e], "g_idx", None), I, self.down.group_size)
+            if pd is not None:
+                bits = self.gate_up.bits
+                gate_modules[e] = permute_gptq_rows(gate_modules[e], pd, bits)
+                up_modules[e] = permute_gptq_rows(up_modules[e], pd, bits)
         kw = dict(self._linear_kwargs)
         bias = kw.pop("bias")
         halves = []
@@ -220,10 +244,12 @@ class MoEExperts(nn.Module):
         gu.zeros = interleave_gate_up(g.zeros, u.zeros, self._zeros_kind(), gu.bits)
         if gu.bias is not None:
             gu.bias = interleave_gate_up(g.bias, u.bias, "bias")
-        self.down._repack(down_modules, device, v2)
+        gu.perm = g.perm
+        self.down._repack(down_modules, device, v2, keep_perm=False)
 
     def repack_from_gptq(self, gate_modules, up_modules, down_modules, device="cuda"):
-        """one GPTQ QuantLinear per expert and projection: GroupedLinear's repack of gate and up, then the interleave"""
+        """one GPTQ QuantLinear per expert and projection: GroupedLinear's repack of gate and up, then the interleave.  Act-order
+        modules (g_idx) are taken as described in the class documentation; an expert's gate and up must have the same g_idx."""
         self._repack(gate_modules, up_modules, down_modules, device, v2=False)
 
     def repack_from_gptq_v2(self, gate_modules, up_modules, down_modules, device="cuda"):

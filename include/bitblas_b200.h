@@ -212,6 +212,22 @@ int bb_moe_route_index(const int32_t* topk_ids, int num_tokens, int top_k, int n
 int bb_moe_combine(const int32_t* slot_rows, const float* topk_weights, const void* Y, int out_dtype, void* out, int num_tokens,
                    int top_k, int N, void* stream);
 
+/* Column gather of the activations of a GPTQ act-order layer: out[r, j] = A[r, perm[e * K + j]], e the group of row r.  An act-order
+ * checkpoint puts input column k in quantization group g_idx[k]; with perm = stable_argsort(g_idx) the loader sorts the weight's
+ * K axis into the contiguous group layout the matmuls read, and y = A[:, perm] x W_sorted^T.  A and out are [rows, K] of a_dtype
+ * (float16 | bfloat16; the values are moved, not converted), both 16-byte aligned; K % 8 == 0 and K <= 112640.
+ *   - num_groups == 1, offsets == NULL: perm [K] (DEVICE int32) applies to every row (a dense layer).
+ *   - offsets (DEVICE int32 [num_groups + 1], the offset contract of bb_matmul_grouped): perm is [num_groups, K] and group e owns
+ *     rows [offsets[e], offsets[e + 1]).  Offsets are clamped to [0, rows], a group whose end is below its start is empty, and rows
+ *     no group claims are not written.
+ * Perm values are clamped to [0, K - 1], so every read stays inside A's row.  perm and offsets 4-byte aligned (code 5 otherwise,
+ * as for A and out).  1 <= num_groups <= BB_GROUPED_MAX_GROUPS.  ONE launch, no workspace, no host synchronisation
+ * (CUDA-graph capturable); programmatic stream serialization: offsets and A are read only after the preceding kernel has
+ * completed, and the next kernel may launch once this one has stored its rows.  rows == 0 validates and
+ * returns 0 without touching the device.  Callers of bb_matmul on an act-order weight gather A with this call first. */
+int bb_permute_cols(const void* A, void* out, const int32_t* perm, int rows, int K, int a_dtype, int num_groups,
+                    const int32_t* offsets, void* stream);
+
 /* Cross-rank barrier for the column-parallel path (no reference counterpart): rank `rank` of `n_peers` signals every peer and
  * waits for all of them, on `stream`, as ONE small kernel -- ordered after the preceding kernels' peer stores (it is launched as a
  * programmatic dependent and waits for them), so after it every rank may read what bb_matmul_scatter calls issued before it wrote.
