@@ -32,7 +32,7 @@ ZEROS_IDS = {"original": BB_ZEROS_ORIGINAL, "rescale": BB_ZEROS_RESCALE, "quanti
 EXPORTS = [
     "bb_init", "bb_matmul", "bb_matmul_scatter", "bb_matmul_grouped", "bb_matmul_grouped_gemm", "bb_matmul_grouped_swiglu",
     "bb_matmul_grouped_gemm_swiglu", "bb_matmul_grouped_gemm_swiglu_gather", "bb_moe_route", "bb_moe_route_index",
-    "bb_moe_combine", "bb_permute_cols", "bb_peer_barrier", "bb_workspace_bytes", "bb_select_kernel", "bb_kernel_name", "bb_set_kernel_override",
+    "bb_moe_combine", "bb_moe_topk", "bb_permute_cols", "bb_peer_barrier", "bb_workspace_bytes", "bb_select_kernel", "bb_kernel_name", "bb_set_kernel_override",
     "bb_launch_count", "bb_last_error", "bb_version", "bb_compress_host", "bb_interleave_host",
     "bb_transform_weight_device", "bb_repack_gptq_qweight_device", "bb_repack_gptq_qzeros_device",
     "bb_retile_weight_device", "bb_debug_decode", "bb_debug_dequant",
@@ -77,6 +77,8 @@ def load() -> ctypes.CDLL:
     lib.bb_moe_route.argtypes = [vp, i32, i32, i32, vp, i32, i32, vp, vp, vp, vp]; lib.bb_moe_route.restype = i32
     lib.bb_moe_route_index.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp]; lib.bb_moe_route_index.restype = i32
     lib.bb_moe_combine.argtypes = [vp, vp, vp, i32, vp, i32, i32, i32, vp]; lib.bb_moe_combine.restype = i32
+    lib.bb_moe_topk.argtypes = [vp, i32, i32, i32, i32, i32, vp, i32, i32, i32, i32, ctypes.c_float, vp, vp, vp]
+    lib.bb_moe_topk.restype = i32
     lib.bb_permute_cols.argtypes = [vp, vp, vp, i32, i32, i32, i32, vp, vp]; lib.bb_permute_cols.restype = i32
     lib.bb_peer_barrier.argtypes = [ctypes.POINTER(vp), i32, i32, vp]; lib.bb_peer_barrier.restype = i32
     lib.bb_workspace_bytes.argtypes = [dp, i32]; lib.bb_workspace_bytes.restype = sz

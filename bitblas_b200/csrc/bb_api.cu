@@ -6,7 +6,9 @@
 //   m <= 8   : memory-bound streaming kernels (bb_gemv.cu)
 //   m  > 8   : wgmma tensor-core kernel (bb_gemm_ts.cu), split-K when the tile grid is smaller than the chip
 //   anything the fast kernels do not cover: the generic SIMT kernel (bb_generic.cu).
+#include <algorithm>
 #include <climits>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
@@ -422,6 +424,75 @@ int bb_moe_combine(const int32_t* slot_rows, const float* topk_weights, const vo
     return 5;
   }
   return launch_moe_combine(slot_rows, topk_weights, Y, out_dtype, out, num_tokens, top_k, N, (cudaStream_t)stream);
+}
+
+int bb_moe_topk(const void* logits, int logits_dtype, int num_tokens, int num_experts, int top_k, int scoring,
+                const float* correction_bias, int num_expert_group, int topk_group, int group_score, int renormalize,
+                float routed_scaling_factor, int32_t* topk_ids, float* topk_weights, void* stream) {
+  if (logits_dtype != BB_F16 && logits_dtype != BB_BF16 && logits_dtype != BB_F32) {
+    set_error("moe topk: logits must be float16, bfloat16 or float32 (logits_dtype=%d)", logits_dtype);
+    return 1;
+  }
+  if (num_experts < 1 || num_experts > BB_GROUPED_MAX_GROUPS) {
+    set_error("moe topk: num_experts must be in [1, %d] (got %d)", BB_GROUPED_MAX_GROUPS, num_experts);
+    return 1;
+  }
+  if (top_k < 1 || top_k > std::min(num_experts, 32)) {
+    set_error("moe topk: top_k must be in [1, min(num_experts, 32) = %d] (got %d)", std::min(num_experts, 32), top_k);
+    return 1;
+  }
+  if (num_tokens < 0) { set_error("moe topk: num_tokens must be >= 0 (got %d)", num_tokens); return 1; }
+  if ((long long)num_tokens * top_k > INT_MAX) {
+    set_error("moe topk: num_tokens * top_k must be below 2^31 (got %d x %d)", num_tokens, top_k);
+    return 1;
+  }
+  if (scoring != 0 && scoring != 1) { set_error("moe topk: scoring must be 0 (softmax) or 1 (sigmoid) (got %d)", scoring); return 1; }
+  if (num_expert_group > 1) {
+    const int n = num_expert_group;
+    if (n > 32) { set_error("moe topk: num_expert_group must be <= 32 (got %d)", n); return 1; }
+    if (num_experts % n) {
+      set_error("moe topk: num_expert_group (%d) must divide num_experts (%d)", n, num_experts);
+      return 1;
+    }
+    if (topk_group < 1 || topk_group > n) {
+      set_error("moe topk: topk_group must be in [1, num_expert_group = %d] (got %d)", n, topk_group);
+      return 1;
+    }
+    if (group_score != 0 && group_score != 1) {
+      set_error("moe topk: group_score must be 0 (max) or 1 (top2_sum) (got %d)", group_score);
+      return 1;
+    }
+    if (group_score == 1 && num_experts / n < 2) {
+      set_error("moe topk: top2_sum needs at least 2 experts per group (num_experts / num_expert_group = %d)", num_experts / n);
+      return 1;
+    }
+    if (top_k > topk_group * (num_experts / n)) {
+      set_error("moe topk: top_k (%d) exceeds the %d experts of the topk_group kept groups", top_k, topk_group * (num_experts / n));
+      return 1;
+    }
+  }
+  if (!std::isfinite(routed_scaling_factor)) {
+    set_error("moe topk: routed_scaling_factor must be finite (got %g)", (double)routed_scaling_factor);
+    return 1;
+  }
+  if (num_tokens == 0) {   // counted like a launching call: every accepted call is one step of bb_launch_count
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return 0;
+  }
+  if (!logits) { set_error("moe topk: logits must be non-null"); return 1; }
+  if (!topk_ids) { set_error("moe topk: topk_ids must be non-null"); return 1; }
+  if (!topk_weights) { set_error("moe topk: topk_weights must be non-null"); return 1; }
+  const uintptr_t elem = logits_dtype == BB_F32 ? 4 : 2;
+  if (reinterpret_cast<uintptr_t>(logits) & (elem - 1)) {
+    set_error("moe topk: logits must be aligned to their element size (%d bytes)", int(elem));
+    return 5;
+  }
+  if (reinterpret_cast<uintptr_t>(topk_ids) & 3) { set_error("moe topk: topk_ids must be 4-byte aligned"); return 5; }
+  if (reinterpret_cast<uintptr_t>(topk_weights) & 3) { set_error("moe topk: topk_weights must be 4-byte aligned"); return 5; }
+  if (reinterpret_cast<uintptr_t>(correction_bias) & 3) { set_error("moe topk: correction_bias must be 4-byte aligned"); return 5; }
+  return launch_moe_topk(logits, logits_dtype, num_tokens, num_experts, top_k, scoring, correction_bias, num_expert_group,
+                         topk_group, group_score, renormalize, routed_scaling_factor, topk_ids, topk_weights,
+                         (cudaStream_t)stream);
 }
 
 int bb_permute_cols(const void* A, void* out, const int32_t* perm, int rows, int K, int a_dtype, int num_groups,

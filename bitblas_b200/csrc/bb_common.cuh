@@ -168,6 +168,10 @@ int launch_moe_route(const int32_t* topk_ids, int n_slots, int top_k, int num_ex
                      int32_t* slot_rows, void* x_sorted, int32_t* row_token, cudaStream_t stream);
 int launch_moe_combine(const int32_t* slot_rows, const float* topk_weights, const void* Y, int out_dtype, void* out,
                        int num_tokens, int top_k, int N, cudaStream_t stream);
+// top-k gating from router logits, bb_moe.cu (validated by bb_moe_topk in bb_api.cu)
+int launch_moe_topk(const void* logits, int logits_dtype, int num_tokens, int num_experts, int top_k, int scoring,
+                    const float* correction_bias, int num_expert_group, int topk_group, int group_score, int renormalize,
+                    float routed_scaling_factor, int32_t* topk_ids, float* topk_weights, cudaStream_t stream);
 // act-order column gather, bb_permute.cu (validated by bb_api.cu): one row of A is staged in shared memory, so K <= PERMUTE_MAX_K
 // (H100: 227 KB per block, less the 3 KB of the kernel's static arrays)
 constexpr int PERMUTE_MAX_K = 112640;

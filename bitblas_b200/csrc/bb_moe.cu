@@ -1,4 +1,5 @@
-// bb_moe.cu -- the two ends of a mixture-of-experts expert block around the grouped matmuls (bb_moe_route, bb_moe_combine).
+// bb_moe.cu -- the two ends of a mixture-of-experts expert block around the grouped matmuls (bb_moe_route, bb_moe_combine), and
+// the top-k gating that produces the block's router output (bb_moe_topk).
 //
 // Routing (moe_route_kernel): slot s = t * k + j of a [T, k] top-k id table goes to expert ids[s]; rows are sorted by expert and,
 // within an expert, by slot, so the order is stable and independent of the grid.  One persistent launch, no workspace:
@@ -15,7 +16,15 @@
 //
 // Combine (moe_combine_kernel): out[t, :] = sum_j w[t, j] * Y[slot_rows[t * k + j], :], accumulated in fp32 in j order and rounded
 // once; slots whose row is outside [0, T * k) add nothing.  One thread per 8 output elements, no atomics: deterministic.
+//
+// Top-k gating (moe_topk_kernel): router logits [T, E] -> the [T, k] ids and fp32 weights routing and combine read.  One warp per
+// token, lane l holding the scores of experts l, l + 32, ... (E <= 256: 8 per lane) in registers; softmax or sigmoid scores, the
+// optional selection bias, the optional group limit (one lane per group over the warp's values in shared memory), then k rounds
+// of warp arg-max, each removing its winner.  Ties go to the lower expert index and a NaN ranks below every number, so the ids,
+// their order and the weights are a function of the logits alone.  PDL: griddepcontrol.wait before the first read,
+// launch_dependents after the stores.
 #include <algorithm>
+#include <climits>
 #include <type_traits>
 
 #include "bb_common.cuh"
@@ -211,6 +220,170 @@ __global__ void __launch_bounds__(256) moe_combine_kernel(const CombineParams c)
   pdl_launch_dependents();
 }
 
+constexpr int TOPK_WARPS = 4;                                  // tokens per CTA
+constexpr int TOPK_PER_LANE = BB_GROUPED_MAX_GROUPS / 32;      // experts per lane
+
+struct TopkParams {
+  const void* logits;   // [T, E]
+  const float* bias;    // [E] or null
+  int32_t* ids;         // [T, k]
+  float* weights;       // [T, k]
+  int T, E, k;
+  bool sigmoid, top2, renormalize;
+  int groups, topk_group;   // groups <= 1: no group limit
+  float scale;
+};
+
+// (a, ia) ranks before (b, ib): the larger value first, a NaN below every number, ties to the lower index
+__device__ __forceinline__ bool topk_before(float a, int ia, float b, int ib) {
+  if (isnan(a)) return isnan(b) && ia < ib;
+  if (isnan(b)) return true;
+  return a > b || (a == b && ia < ib);
+}
+
+template <typename LT>
+__device__ __forceinline__ float logit_to_float(LT v) {
+  if constexpr (std::is_same<LT, float>::value) return v;
+  else return TypeTraits<LT>::to_float(v);
+}
+
+template <typename LT>
+__global__ void __launch_bounds__(TOPK_WARPS * 32) moe_topk_kernel(const TopkParams p) {
+  __shared__ float v_s[TOPK_WARPS][BB_GROUPED_MAX_GROUPS];   // selection values of each warp's token (group limit only)
+  constexpr unsigned FULL = 0xffffffffu;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long t = (long long)blockIdx.x * TOPK_WARPS + warp;
+  pdl_wait();   // the logits are the preceding kernel's output
+  if (t < p.T) {
+    const LT* row = reinterpret_cast<const LT*>(p.logits) + size_t(t) * p.E;
+    float s[TOPK_PER_LANE], v[TOPK_PER_LANE];
+    unsigned live = 0;   // bit i: expert lane + 32 i exists and can still be chosen
+#pragma unroll
+    for (int i = 0; i < TOPK_PER_LANE; ++i) {
+      const int e = lane + 32 * i;
+      s[i] = 0.f;
+      if (e < p.E) {
+        s[i] = logit_to_float(row[e]);
+        live |= 1u << i;
+      }
+    }
+    if (p.sigmoid) {
+#pragma unroll
+      for (int i = 0; i < TOPK_PER_LANE; ++i) s[i] = 1.f / (1.f + expf(-s[i]));
+    } else {
+      // softmax over the experts; NaN logits stay NaN and add nothing to the max or the sum.  The xor butterflies give every lane
+      // the same bits (fmaxf and + are commutative).
+      float m = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < TOPK_PER_LANE; ++i)
+        if ((live >> i) & 1) m = fmaxf(m, s[i]);
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) m = fmaxf(m, __shfl_xor_sync(FULL, m, d));
+      float sum = 0.f;
+#pragma unroll
+      for (int i = 0; i < TOPK_PER_LANE; ++i) {
+        if (((live >> i) & 1) && !isnan(s[i])) {
+          s[i] = expf(s[i] - m);
+          sum += s[i];
+        }
+      }
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(FULL, sum, d);
+#pragma unroll
+      for (int i = 0; i < TOPK_PER_LANE; ++i) s[i] = s[i] / sum;
+    }
+#pragma unroll
+    for (int i = 0; i < TOPK_PER_LANE; ++i) {
+      const int e = lane + 32 * i;
+      v[i] = (p.bias && e < p.E) ? s[i] + p.bias[e] : s[i];
+    }
+
+    if (p.groups > 1) {
+      // lane g scores group g (experts [g * gs, (g + 1) * gs)) from shared memory, ranks it against the other groups, and the
+      // experts of groups outside the topk_group best leave `live`
+#pragma unroll
+      for (int i = 0; i < TOPK_PER_LANE; ++i)
+        if (lane + 32 * i < p.E) v_s[warp][lane + 32 * i] = v[i];
+      __syncwarp();
+      const int gs = p.E / p.groups;
+      float score = __int_as_float(0x7fffffff);
+      if (lane < p.groups) {
+        float b1 = __int_as_float(0x7fffffff), b2 = b1;   // the two best values of the group
+        int i1 = INT_MAX, i2 = INT_MAX;
+        // lane g starts at offset g % gs of its group and wraps around, so that with gs a multiple of 32 the lanes read 32
+        // different banks; the two best are the same in any scan order (topk_before is a strict total order)
+        const int e0 = lane * gs, e1 = e0 + gs;
+        int e = e0 + lane % gs;
+        for (int n = 0; n < gs; ++n, e = e + 1 == e1 ? e0 : e + 1) {
+          const float x = v_s[warp][e];
+          if (topk_before(x, e, b1, i1)) {
+            b2 = b1; i2 = i1; b1 = x; i1 = e;
+          } else if (topk_before(x, e, b2, i2)) {
+            b2 = x; i2 = e;
+          }
+        }
+        score = p.top2 ? b1 + b2 : b1;
+      }
+      int rank = 0;
+      for (int g = 0; g < p.groups; ++g) {
+        const float o = __shfl_sync(FULL, score, g);
+        if (topk_before(o, g, score, lane)) ++rank;
+      }
+      const unsigned kept = __ballot_sync(FULL, lane < p.groups && rank < p.topk_group);
+#pragma unroll
+      for (int i = 0; i < TOPK_PER_LANE; ++i) {
+        const int e = lane + 32 * i;
+        if (e < p.E && !((kept >> (e / gs)) & 1)) live &= ~(1u << i);
+      }
+    }
+
+    // k rounds of warp arg-max; lane j keeps the j-th choice.  The weights' sum runs in j order.
+    int my_id = 0;
+    float my_w = 0.f, wsum = 0.f;
+    for (int j = 0; j < p.k; ++j) {
+      float bv = __int_as_float(0x7fffffff);
+      int bi = INT_MAX;
+#pragma unroll
+      for (int i = 0; i < TOPK_PER_LANE; ++i) {
+        if (((live >> i) & 1) && topk_before(v[i], lane + 32 * i, bv, bi)) {
+          bv = v[i];
+          bi = lane + 32 * i;
+        }
+      }
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) {   // topk_before is a strict total order: every lane ends with the same winner
+        const float ov = __shfl_xor_sync(FULL, bv, d);
+        const int oi = __shfl_xor_sync(FULL, bi, d);
+        if (topk_before(ov, oi, bv, bi)) {
+          bv = ov;
+          bi = oi;
+        }
+      }
+      // the validated k leaves a live expert for every round, so bi < E
+      const int owner = bi & 31, slot = bi >> 5;
+      float mine = 0.f;
+#pragma unroll
+      for (int i = 0; i < TOPK_PER_LANE; ++i)
+        if (i == slot) mine = s[i];
+      if (lane == owner) live &= ~(1u << slot);
+      const float w = __shfl_sync(FULL, mine, owner);
+      wsum += w;
+      if (lane == j) {
+        my_id = bi;
+        my_w = w;
+      }
+    }
+    if (lane < p.k) {
+      float w = my_w;
+      if (p.renormalize) w = wsum != 0.f ? w / wsum : 0.f;
+      const size_t o = size_t(t) * p.k + lane;
+      p.ids[o] = my_id;
+      p.weights[o] = w * p.scale;
+    }
+  }
+  pdl_launch_dependents();
+}
+
 }  // namespace
 
 // x_sorted == nullptr: the INDEX instance, which writes row_token instead of copying x
@@ -239,6 +412,20 @@ int launch_moe_combine(const int32_t* slot_rows, const float* topk_weights, cons
   auto kernel = out_dtype == BB_F16 ? moe_combine_kernel<__half>
                                     : (out_dtype == BB_BF16 ? moe_combine_kernel<__nv_bfloat16> : moe_combine_kernel<float>);
   return launch_pdl(kernel, unsigned((threads + 255) / 256), 256, 0, stream, pdl_enabled(), c);
+}
+
+int launch_moe_topk(const void* logits, int logits_dtype, int num_tokens, int num_experts, int top_k, int scoring,
+                    const float* correction_bias, int num_expert_group, int topk_group, int group_score, int renormalize,
+                    float routed_scaling_factor, int32_t* topk_ids, float* topk_weights, cudaStream_t stream) {
+  TopkParams p;
+  p.logits = logits; p.bias = correction_bias; p.ids = topk_ids; p.weights = topk_weights;
+  p.T = num_tokens; p.E = num_experts; p.k = top_k;
+  p.sigmoid = scoring == 1; p.top2 = group_score == 1; p.renormalize = renormalize != 0;
+  p.groups = num_expert_group > 1 ? num_expert_group : 1; p.topk_group = topk_group;
+  p.scale = routed_scaling_factor;
+  auto kernel = logits_dtype == BB_F16 ? moe_topk_kernel<__half>
+                                       : (logits_dtype == BB_BF16 ? moe_topk_kernel<__nv_bfloat16> : moe_topk_kernel<float>);
+  return launch_pdl(kernel, unsigned((num_tokens + TOPK_WARPS - 1) / TOPK_WARPS), TOPK_WARPS * 32, 0, stream, pdl_enabled(), p);
 }
 
 }  // namespace bb

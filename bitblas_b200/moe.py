@@ -1,6 +1,6 @@
-"""Mixture-of-experts expert block: device routing (bb_moe_route; bb_moe_route_index without the copy), the gate/up interleave
-that the SwiGLU grouped calls read, the weighted top-k combine (bb_moe_combine), and ``MoEExperts``, which runs router output to
-layer output in four library launches.
+"""Mixture-of-experts expert block: top-k gating from router logits (bb_moe_topk), device routing (bb_moe_route;
+bb_moe_route_index without the copy), the gate/up interleave that the SwiGLU grouped calls read, the weighted top-k combine
+(bb_moe_combine), and ``MoEExperts``, which runs router output to layer output in four library launches.
 
 Above 8 rows per expert, moe_route_index -> forward_grouped_swiglu(x, ..., row_index=row_token) -> down -> moe_combine computes
 MoEExperts' bits without the [T*k, H] routed copy of x (T*k*H*2 bytes: 64 MiB per layer at 2048 tokens, top-8, H = 2048).
@@ -156,6 +156,71 @@ def moe_combine(y_sorted: torch.Tensor, slot_rows: torch.Tensor, topk_weights: t
     return output
 
 
+_SCORING = {"softmax": 0, "sigmoid": 1}
+_GROUP_SCORE = {"max": 0, "top2_sum": 1}
+
+
+def moe_topk(router_logits: torch.Tensor, top_k: int, scoring: str = "softmax", renormalize: bool = False,
+             correction_bias: torch.Tensor = None, num_expert_group: int = None, topk_group: int = None,
+             group_score: str = "max", routed_scaling_factor: float = 1.0):
+    """Top-k gating on the device in one launch (bb_moe_topk): router_logits [T, E] (fp16 / bf16 / fp32) -> (topk_ids int32
+    [T, k], topk_weights float32 [T, k]), what ``MoEExperts.forward`` takes.
+
+    Per token: scores s = softmax(logits) or sigmoid(logits) in fp32; selection values v = s + correction_bias (fp32 [E], which
+    steers the selection only); with ``num_expert_group`` = n > 1, the experts form n contiguous groups, each scored by the max of
+    its v ("max") or the sum of its two largest ("top2_sum"), and only the ``topk_group`` best groups can be chosen; then the k
+    largest v in descending order, ties to the lower expert (group) index, NaN below every number.  The weights are the chosen s,
+    divided by their fp32 sum in slot order with ``renormalize``, times ``routed_scaling_factor``.  The ids and their order are
+    library-defined, so two runs and graph replays are bit-identical.  1 <= E <= 256, 1 <= k <= min(E, 32).
+
+    Presets:
+
+    ================  ==========================================================================================================
+    model             arguments
+    ================  ==========================================================================================================
+    Mixtral-8x7B      ``moe_topk(logits, 2, renormalize=True)``
+    Qwen3-30B-A3B     ``moe_topk(logits, 8, renormalize=True)`` (``norm_topk_prob``)
+    Qwen1.5/2-MoE     ``moe_topk(logits, 4)``
+    DeepSeek-V2-Lite  ``moe_topk(logits, 6)`` (``routed_scaling_factor`` 1.0)
+    DeepSeek-V2       ``moe_topk(logits, 6, num_expert_group=8, topk_group=3, group_score="max", routed_scaling_factor=16.0)``
+    DeepSeek-V3       ``moe_topk(logits, 8, scoring="sigmoid", correction_bias=e_score_correction_bias, num_expert_group=8,
+                      topk_group=4, group_score="top2_sum", renormalize=True, routed_scaling_factor=2.5)``
+    ================  ==========================================================================================================
+    """
+    if not isinstance(router_logits, torch.Tensor) or router_logits.dtype not in (torch.float16, torch.bfloat16, torch.float32):
+        raise TypeError("router_logits must be a float16, bfloat16 or float32 torch.Tensor")
+    if router_logits.dim() != 2:
+        raise TypeError(f"router_logits must be a 2-D [T, E] tensor (got {router_logits.dim()}-D)")
+    T, E = router_logits.shape
+    if scoring not in _SCORING:
+        raise ValueError(f"scoring must be one of {sorted(_SCORING)} (got {scoring!r})")
+    if group_score not in _GROUP_SCORE:
+        raise ValueError(f"group_score must be one of {sorted(_GROUP_SCORE)} (got {group_score!r})")
+    grouped = num_expert_group is not None and int(num_expert_group) > 1
+    if grouped and topk_group is None:
+        raise ValueError("num_expert_group > 1 needs topk_group")
+    if correction_bias is not None:
+        if not isinstance(correction_bias, torch.Tensor) or correction_bias.dtype != torch.float32 or \
+                tuple(correction_bias.shape) != (E,):
+            raise TypeError(f"correction_bias must be a float32 tensor of shape [E={E}]")
+        if correction_bias.device != router_logits.device:
+            raise ValueError("router_logits and correction_bias must be on the same device")
+        _check(correction_bias, "correction_bias", torch.float32, 1)
+    _check(router_logits, "router_logits", router_logits.dtype, 2)
+    dev, stream = _device_ready(router_logits)
+    k = int(top_k)
+    topk_ids = torch.empty((T, max(k, 0)), dtype=torch.int32, device=dev)
+    topk_weights = torch.empty((T, max(k, 0)), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        rc = _lib.load().bb_moe_topk(router_logits.data_ptr(), _lib.DTYPE_IDS[str(router_logits.dtype)[6:]], T, E, k,
+                                     _SCORING[scoring], None if correction_bias is None else correction_bias.data_ptr(),
+                                     int(num_expert_group) if grouped else 0, int(topk_group) if grouped else 0,
+                                     _GROUP_SCORE[group_score], int(bool(renormalize)), float(routed_scaling_factor),
+                                     topk_ids.data_ptr(), topk_weights.data_ptr(), stream)
+    _lib.check(rc, "bb_moe_topk")
+    return topk_ids, topk_weights
+
+
 class MoEExperts(nn.Module):
     """The expert block of a SwiGLU mixture-of-experts layer, from router output to layer output:
     ``y[t] = sum_j w[t, j] * down_e(silu(gate_e(x[t])) * up_e(x[t]))`` with e = topk_ids[t, j], as four library launches with no
@@ -256,4 +321,4 @@ class MoEExperts(nn.Module):
         self._repack(gate_modules, up_modules, down_modules, device, v2=True)
 
 
-__all__ = ["MoEExperts", "moe_route", "moe_route_index", "moe_combine", "interleave_gate_up", "deinterleave_gate_up"]
+__all__ = ["MoEExperts", "moe_topk", "moe_route", "moe_route_index", "moe_combine", "interleave_gate_up", "deinterleave_gate_up"]

@@ -212,6 +212,32 @@ int bb_moe_route_index(const int32_t* topk_ids, int num_tokens, int top_k, int n
 int bb_moe_combine(const int32_t* slot_rows, const float* topk_weights, const void* Y, int out_dtype, void* out, int num_tokens,
                    int top_k, int N, void* stream);
 
+/* Mixture-of-experts top-k gating: router logits [num_tokens, num_experts] (DEVICE, logits_dtype float16 | bfloat16 | float32,
+ * converted to fp32) -> topk_ids int32 [T, top_k] and topk_weights float32 [T, top_k], the router output bb_moe_route and
+ * bb_moe_combine read.  Per token, with l[e] the logits (expf is the full-precision fp32 exponential):
+ *   1. score: scoring 0 (softmax) s[e] = expf(l[e] - max) / sum_e' expf(l[e'] - max) over every expert (NaN logits are left
+ *      out of the max and the sum, and their score is NaN); scoring 1 (sigmoid) s[e] = 1 / (1 + expf(-l[e])).
+ *   2. selection value v[e] = s[e] + correction_bias[e] (fp32 [num_experts], DEVICE; NULL: no bias).  The bias steers the
+ *      selection only.
+ *   3. group limit, num_expert_group = n > 1: the experts form n contiguous groups of num_experts / n; a group's score is the
+ *      max of its v (group_score 0) or the sum of its two largest v (group_score 1, "top2_sum"); only the topk_group groups
+ *      with the highest scores can be chosen.  num_expert_group <= 1: no group limit (topk_group and group_score are ignored).
+ *   4. the top_k experts with the largest v, in descending order of v: slot j holds the j-th choice.  Ties go to the lower expert
+ *      (or group) index, and a NaN ranks below every number.
+ *   5. weights w[j] = s[id[j]] (without the bias); renormalize != 0: w[j] /= sum_j' w[j'], summed in fp32 in j order (a zero
+ *      sum gives zero weights); then w[j] *= routed_scaling_factor.
+ * The order is part of the result: two runs, and a CUDA-graph replay, are bit-identical.  1 <= num_experts <=
+ * BB_GROUPED_MAX_GROUPS; 1 <= top_k <= min(num_experts, 32); T * top_k < 2^31; scoring 0 | 1; with a group limit n <= 32 divides
+ * num_experts, 1 <= topk_group <= n, group_score 0 | 1 (1 needs num_experts / n >= 2) and top_k <= topk_group * num_experts / n;
+ * routed_scaling_factor finite (code 1 otherwise, each with its own message).  logits aligned to their element size, the other
+ * arrays 4-byte aligned (code 5).  ONE launch, no workspace, no host synchronisation (CUDA-graph capturable); programmatic stream
+ * serialization: the logits are read only after the preceding kernel has completed, and the next kernel may launch once this
+ * one has stored its results.  num_tokens == 0 validates and returns 0 without touching the device; unlike the bb_moe_route /
+ * bb_moe_combine calls it is still counted in bb_launch_count, so every accepted call adds exactly one step whatever T is. */
+int bb_moe_topk(const void* logits, int logits_dtype, int num_tokens, int num_experts, int top_k, int scoring,
+                const float* correction_bias, int num_expert_group, int topk_group, int group_score, int renormalize,
+                float routed_scaling_factor, int32_t* topk_ids, float* topk_weights, void* stream);
+
 /* Column gather of the activations of a GPTQ act-order layer: out[r, j] = A[r, perm[e * K + j]], e the group of row r.  An act-order
  * checkpoint puts input column k in quantization group g_idx[k]; with perm = stable_argsort(g_idx) the loader sorts the weight's
  * K axis into the contiguous group layout the matmuls read, and y = A[:, perm] x W_sorted^T.  A and out are [rows, K] of a_dtype
