@@ -9,6 +9,7 @@
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
+#include <type_traits>
 #include <utility>
 
 #include "../../include/bitblas_b200.h"
@@ -482,22 +483,37 @@ __device__ __forceinline__ void grouped_schedule(const GP& g, int R, int per_chu
   }
   if (lane == 31) item0_s[g.E] = incl;
 }
+// ---- output rounding: how every epilogue turns one accumulator into an output element -------------------------------------------
+// Float accumulators: cast to out_dtype, then the bias (a float of A_dtype, 0 without one) added in out_dtype; an fp32 output is
+// one sum.  This is bb_matmul's rounding; the grouped kernels are bit-identical to it because they round the same way.
+template <typename O>
+__device__ __forceinline__ O round_out(float v, bool has_bias, float bias) {
+  if constexpr (std::is_same<O, float>::value) {
+    return v + bias;
+  } else {
+    O r = TypeTraits<O>::from_float(v);
+    if (has_bias) r = __hadd(r, TypeTraits<O>::from_float(bias));
+    return r;
+  }
+}
+// Int32 accumulators (int8 activations): the sum and the int8 bias b are each converted to out_dtype and added there
+__device__ __forceinline__ void store_out_i32(void* C, size_t o, int v, int b, int out_dtype) {
+  switch (out_dtype) {
+    case BB_I32: reinterpret_cast<int*>(C)[o] = v + b; break;
+    case BB_I8: reinterpret_cast<int8_t*>(C)[o] = int8_t(int8_t(v) + b); break;
+    case BB_F32: reinterpret_cast<float*>(C)[o] = float(v) + float(b); break;
+    case BB_F16: reinterpret_cast<__half*>(C)[o] = __hadd(__int2half_rn(v), __int2half_rn(b)); break;
+    default: reinterpret_cast<__nv_bfloat16*>(C)[o] = __hadd(__int2bfloat16_rn(v), __int2bfloat16_rn(b));
+  }
+}
+
 // ---- SwiGLU epilogue of the grouped kernels (gate/up interleave: weight row 16b + i is gate row 8b + i for i < 8, up row 8b + i - 8
 // for i >= 8; both halves of a 16-row block are owned by the same thread) ----------------------------------------------------------
-// one pre-activation as the plain grouped epilogue stores it: cast to out_dtype, then the bias (already a float of A_dtype) added in
-// out_dtype; fp32 output: one fp32 sum (bias = 0 without one)
+// one pre-activation as the plain grouped epilogue stores it
 __device__ __forceinline__ float swiglu_operand(float v, bool has_bias, float bias, int out_dtype) {
-  if (out_dtype == BB_F16) {
-    __half h = __float2half_rn(v);
-    if (has_bias) h = __hadd(h, __float2half_rn(bias));
-    return __half2float(h);
-  }
-  if (out_dtype == BB_BF16) {
-    __nv_bfloat16 h = __float2bfloat16_rn(v);
-    if (has_bias) h = __hadd(h, __float2bfloat16_rn(bias));
-    return __bfloat162float(h);
-  }
-  return v + bias;
+  if (out_dtype == BB_F16) return __half2float(round_out<__half>(v, has_bias, bias));
+  if (out_dtype == BB_BF16) return __bfloat162float(round_out<__nv_bfloat16>(v, has_bias, bias));
+  return round_out<float>(v, has_bias, bias);
 }
 // C[o] = silu(g) * u = g / (1 + exp(-g)) * u in fp32, rounded once to out_dtype
 __device__ __forceinline__ void store_swiglu(void* C, size_t o, float g, float u, int out_dtype) {

@@ -223,17 +223,8 @@ gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if constexpr (INT8) {
           const int a = int(v);
           const int b = int(bias_f[h]);
-          auto put = [&](void* Cd) {
-            switch (p.out_dtype) {
-              case BB_I32: reinterpret_cast<int*>(Cd)[o] = a + b; break;
-              case BB_I8: reinterpret_cast<int8_t*>(Cd)[o] = int8_t(int8_t(a) + b); break;
-              case BB_F32: reinterpret_cast<float*>(Cd)[o] = float(a) + float(b); break;
-              case BB_F16: reinterpret_cast<__half*>(Cd)[o] = __hadd(__int2half_rn(a), __int2half_rn(b)); break;
-              default: reinterpret_cast<__nv_bfloat16*>(Cd)[o] = __hadd(__int2bfloat16_rn(a), __int2bfloat16_rn(b));
-            }
-          };
-          put(C0);
-          for (int d = 1; d < ndst; ++d) put(p.out.ptr[d]);
+          store_out_i32(C0, o, a, b, p.out_dtype);
+          for (int d = 1; d < ndst; ++d) store_out_i32(p.out.ptr[d], o, a, b, p.out_dtype);
         } else {
           if (p.out_dtype == BB_F16) {
             __half r = __float2half_rn(v);

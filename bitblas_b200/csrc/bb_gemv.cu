@@ -153,16 +153,7 @@ gemv_i8_kernel(const GemvParams p) {
     const int n = rb * 16 + row;
     const int b = p.bias ? int(reinterpret_cast<const int8_t*>(p.bias)[n]) : 0;
     const size_t o = size_t(m) * size_t(p.out.ld) + size_t(p.out.col0) + n;
-    for (int d = 0; d < p.out.n; ++d) {
-      void* Cd = p.out.ptr[d];
-      switch (p.out_dtype) {
-        case BB_I32: reinterpret_cast<int*>(Cd)[o] = v + b; break;
-        case BB_I8: reinterpret_cast<int8_t*>(Cd)[o] = int8_t(int8_t(v) + b); break;
-        case BB_F32: reinterpret_cast<float*>(Cd)[o] = float(v) + float(b); break;
-        case BB_F16: reinterpret_cast<__half*>(Cd)[o] = __hadd(__int2half_rn(v), __int2half_rn(b)); break;
-        default: reinterpret_cast<__nv_bfloat16*>(Cd)[o] = __hadd(__int2bfloat16_rn(v), __int2bfloat16_rn(b));
-      }
-    }
+    for (int d = 0; d < p.out.n; ++d) store_out_i32(p.out.ptr[d], o, v, b, p.out_dtype);
   }
 }
 

@@ -194,15 +194,13 @@ __device__ __forceinline__ void gs_store(const SlabParams& p, int n, float v) {
   const size_t o = size_t(p.out.col0) + n;   // m == 0
   const float bf = p.bias ? TypeTraits<T>::to_float(reinterpret_cast<const T*>(p.bias)[n]) : 0.f;
   if (p.out_dtype == BB_F16) {
-    __half h = __float2half_rn(v);
-    if (p.bias) h = __hadd(h, __float2half_rn(bf));
+    const __half h = round_out<__half>(v, p.bias, bf);
     for (int d = 0; d < p.out.n; ++d) reinterpret_cast<__half*>(p.out.ptr[d])[o] = h;
   } else if (p.out_dtype == BB_BF16) {
-    __nv_bfloat16 h = __float2bfloat16_rn(v);
-    if (p.bias) h = __hadd(h, __float2bfloat16_rn(bf));
+    const __nv_bfloat16 h = round_out<__nv_bfloat16>(v, p.bias, bf);
     for (int d = 0; d < p.out.n; ++d) reinterpret_cast<__nv_bfloat16*>(p.out.ptr[d])[o] = h;
   } else {
-    for (int d = 0; d < p.out.n; ++d) reinterpret_cast<float*>(p.out.ptr[d])[o] = v + bf;
+    for (int d = 0; d < p.out.n; ++d) reinterpret_cast<float*>(p.out.ptr[d])[o] = round_out<float>(v, p.bias, bf);
   }
 }
 
