@@ -146,6 +146,16 @@ class Linear(nn.Module):
             named = [("qweight", True), ("scales", cfg.with_scaling), ("zeros", cfg.with_zeros), ("bias", cfg.with_bias)]
         return [getattr(self, name) for name, used in named if used]
 
+    def _check_live_params(self, params, device):
+        """the operator's parameter checks (dtype, element count, contiguity, CUDA) on the live buffers, and all of them on
+        `device`, A's: `lib.call` hands the kernel bare pointers"""
+        cfg = self.bitblas_matmul.config
+        self.bitblas_matmul._check_params(self.qweight, self.scales if cfg.with_scaling else None,
+                                          self.zeros if cfg.with_zeros else None, self.bias if cfg.with_bias else None)
+        for t in params:
+            if t.device != device:
+                raise ValueError(f"the layer's buffers must be on A's device {device} (a buffer is on {t.device})")
+
     def init_params(self):
         tensors = self._live_params()
         self.q_params = [ctypes.c_void_p(t.data_ptr()) for t in tensors]
@@ -167,11 +177,13 @@ class Linear(nn.Module):
         if A.shape[-1] != self.in_features:
             raise ValueError(f"A has inner dimension {A.shape[-1]}, expected {self.in_features}")
         stream = torch.cuda.current_stream(A.device)
-        # the reference rebuilds this list on every call (module/__init__.py:274); rebuild only if a buffer moved
-        if self.q_params is None or self._q_param_key != tuple(t.data_ptr() for t in self._live_params()):
+        # the reference rebuilds this list on every call (module/__init__.py:274); rebuild, and validate the buffers the kernel
+        # reads through raw pointers, only if a buffer moved
+        params = self._live_params()
+        if self.q_params is None or self._q_param_key != tuple(t.data_ptr() for t in params):
+            self._check_live_params(params, A.device)
             self.init_params()
-        if output is None:
-            output = torch.empty(A.shape[:-1] + (self.out_features,), dtype=getattr(torch, op.out_dtype), device=A.device)
+        output = op._output_for(A, output)
         if self.perm is not None:   # act-order: the weight's K axis is sorted, so A's columns are gathered to match
             A = act_order.permute_cols(A.view(-1, self.in_features), self.perm).view(A.shape)
         args = [ctypes.c_void_p(A.data_ptr()), *self.q_params, ctypes.c_void_p(output.data_ptr())]
@@ -214,8 +226,13 @@ class Linear(nn.Module):
         dev = torch.device(device)
         if dev.type != "cuda":
             raise RuntimeError("repack_from_gptq needs a CUDA device: bitblas_b200 has no CPU path")
-        _lib.ensure_init(dev.index if dev.index is not None else torch.cuda.current_device())
         op = self.bitblas_matmul
+        if self.torch_dtype not in (torch.float16, torch.bfloat16):
+            raise ValueError(f"GPTQ checkpoints need float16 or bfloat16 activations (A_dtype {op.A_dtype}): their scales are "
+                             "stored in the activations' type")
+        if self.bias is not None and getattr(gptq_module, "bias", None) is None:
+            raise ValueError("the layer has bias=True but the GPTQ module has no bias")
+        _lib.ensure_init(dev.index if dev.index is not None else torch.cuda.current_device())
         bits = self.bits
         stream = torch.cuda.current_stream(dev).cuda_stream
         qw = gptq_module.qweight.to(dev).contiguous().view(torch.int32)  # [K*bits/32, N]
@@ -223,8 +240,6 @@ class Linear(nn.Module):
         assert qw.shape == (K * bits // 32, N), f"unexpected GPTQ qweight shape {tuple(qw.shape)}"
         perm = act_order.perm_from_g_idx(getattr(gptq_module, "g_idx", None), K, self.group_size)
         if perm is not None:
-            if self.torch_dtype not in (torch.float16, torch.bfloat16):
-                raise ValueError("act-order GPTQ checkpoints need float16 or bfloat16 activations (the column gather)")
             perm = perm.to(dev)
             qw = act_order.permute_gptq_qweight(qw, perm, bits)
         out = torch.empty(op.retrieve_weight_shape(), dtype=torch.int8, device=dev)
@@ -233,7 +248,8 @@ class Linear(nn.Module):
             _lib.check(lib.bb_repack_gptq_qweight_device(qw.data_ptr(), out.data_ptr(), K, N, bits, tgt, stream),
                        "bb_repack_gptq_qweight_device")
             self.qweight = op.tile_weight(out) if op.weight_tiled else out   # propagate_b: slab tiling of the packed rows
-            self.scales = gptq_module.scales.to(dev).T.contiguous().view(self.torch_dtype)
+            # converted, not reinterpreted: checkpoints usually store float16 scales, whatever the layer's type
+            self.scales = gptq_module.scales.to(dev).T.to(self.torch_dtype).contiguous()
             qz = gptq_module.qzeros.to(dev).contiguous().view(torch.int32)  # [K/g, N*bits/32]
             G = K // self.group_size
             mode = op.config.zeros_mode
@@ -246,7 +262,7 @@ class Linear(nn.Module):
                        "bb_repack_gptq_qzeros_device")
             self.zeros = zeros
         if self.bias is not None:
-            self.bias = gptq_module.bias.data.to(dev).to(torch.float16).contiguous()
+            self.bias = gptq_module.bias.data.to(dev).to(self.torch_dtype).contiguous()
         self.perm = perm
         self.q_params = None
 

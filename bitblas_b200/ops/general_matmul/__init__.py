@@ -423,6 +423,16 @@ class Matmul(Operator):
                 raise ValueError("with_bias=True but bias is None")
             self._check_tensor(bias, "bias", adt, c.N)
 
+    def _output_for(self, A, output):
+        """the output of A [.., K]: a new [.., N] tensor on A's device, or the caller's, checked to hold the m * N values"""
+        N = self.config.N
+        if output is None:
+            return torch.empty(A.shape[:-1] + (N,), dtype=self.torch_output_dtype, device=A.device)
+        numel = A.numel() // self.config.K * N
+        if not (output.is_cuda and output.dtype == self.torch_output_dtype and output.is_contiguous() and output.numel() == numel):
+            self._check_tensor(output, "output", self.torch_output_dtype, numel)
+        return output
+
     def forward(self, A, W, scale=None, zeros=None, bias=None, output=None) -> Any:
         if self.consistent:
             return self._forward_consistent(A, W, bias, output)
@@ -443,10 +453,7 @@ class Matmul(Operator):
         if self.dynamic_range is None and m != int(c.M):
             raise ValueError(f"operator was created for static M={c.M}, got {m} rows")
         dev = A.device
-        if output is None:
-            output = torch.empty(A.shape[:-1] + (c.N,), dtype=self.torch_output_dtype, device=dev)
-        elif not (output.is_cuda and output.dtype == self.torch_output_dtype and output.is_contiguous() and output.numel() == m * c.N):
-            self._check_tensor(output, "output", self.torch_output_dtype, m * c.N)
+        output = self._output_for(A, output)
         idx = dev.index if dev.index is not None else torch.cuda.current_device()
         if idx not in _lib._inited:
             _lib.ensure_init(idx)

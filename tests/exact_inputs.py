@@ -167,6 +167,62 @@ def product_weight(op, case, device):
     return w
 
 
+# ---- GPTQ checkpoints of exact cases ------------------------------------------------------------------------------------------------
+def _pack_int32(vals, bits, dim):
+    """int64 values in [0, 2^bits) -> int32 words along `dim`, element i of a word at bit bits * i (auto_gptq's packing)"""
+    per = 32 // bits
+    v = vals.to(torch.int64).movedim(dim, 0)
+    word = torch.zeros((v.shape[0] // per, *v.shape[1:]), dtype=torch.int64)
+    for i in range(per):
+        word |= v[i::per] << (bits * i)
+    word = torch.where(word >= 2 ** 31, word - 2 ** 32, word)
+    return word.to(torch.int32).movedim(0, dim).contiguous()
+
+
+def gptq_checkpoint(case, *, v2, act_order, scale_dtype, seed):
+    """what an auto_gptq QuantLinear of the quantized-zeros case `case` (make_exact_case(..., mode="quantized")) holds, as a
+    namespace: qweight int32 [K*bits/32, N], qzeros int32 [K/g, N*bits/32] (v1 stores z - 1 modulo 2^bits, so z = 0 is stored as
+    2^bits - 1; v2 stores z), scales [K/g, N] and bias [N] in `scale_dtype` (+-2^e and quarter integers: exact in float16 and
+    bfloat16), g_idx int32 [K].  The case's K axis is the sorted one: with act_order, GPTQ's desc_act assignment of the checkpoint's
+    columns to groups (from `seed` alone, so modules built with one seed share a g_idx) puts sorted column j at checkpoint column
+    perm[j], perm = stable_argsort(g_idx); without it g_idx = k // g and perm is None.  Also returns A, the case's activations in
+    checkpoint column order (A[:, perm] is the case's), and perm."""
+    from types import SimpleNamespace
+    assert case["mode"] == "quantized" and case["fmt"] == "uint", (case["mode"], case["fmt"])
+    N, K, bits = case["N"], case["K"], case["bit"]
+    G = case["qz"].shape[0]
+    g = K // G
+    if act_order:
+        gen = torch.Generator().manual_seed(seed)
+        g_idx = torch.empty(K, dtype=torch.int32)
+        g_idx[torch.randperm(K, generator=gen)] = torch.arange(K, dtype=torch.int32) // g
+        perm = torch.sort(g_idx.long(), stable=True).indices
+        A = torch.empty_like(case["A"])
+        A[:, perm] = case["A"]
+        intw = torch.empty((K, N), dtype=torch.int64)
+        intw[perm] = case["fields"].T.to(torch.int64)
+    else:
+        g_idx = torch.arange(K, dtype=torch.int32) // g
+        perm, A, intw = None, case["A"], case["fields"].T.to(torch.int64)
+    z = case["qz"].to(torch.int64)
+    stored_z = z if v2 else (z - 1) % 2 ** bits
+    bias = None if case["bias"] is None else torch.nn.Parameter(case["bias"].double().to(scale_dtype), requires_grad=False)
+    return SimpleNamespace(qweight=_pack_int32(intw, bits, 0), qzeros=_pack_int32(stored_z, bits, 1),
+                           scales=case["scale"].double().T.contiguous().to(scale_dtype), bias=bias, g_idx=g_idx, A=A, perm=perm)
+
+
+def zeros_mode_case(case, mode):
+    """the quantized-zeros case with its integer zero points z expressed in `mode`: "original" zeros z, "rescale" zeros z s (exact:
+    s = +-2^e), or the case itself; every mode dequantises to the same (w - z) s"""
+    if mode == "quantized":
+        return case
+    adt = O.TORCH_DTYPE[case["cfg"]["A_dtype"]]
+    z = case["qz"].double().T
+    zeros = (z if mode == "original" else z * case["scale"].double()).to(adt)
+    assert torch.equal(zeros.double(), z if mode == "original" else z * case["scale"].double())
+    return dict(case, mode=mode, zeros=zeros, qz=None, cfg=dict(case["cfg"], zeros_mode=mode))
+
+
 # ---- the operands as float64 ---------------------------------------------------------------------------------------------------
 def _gidx(case, device):
     G = case["scale"].shape[1] if case["scale"] is not None else 1
