@@ -9,6 +9,8 @@ from __future__ import annotations
 import ctypes
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libbitblas_b200.so")
 
@@ -124,6 +126,52 @@ def ensure_init(device_index: int) -> None:
         return
     check(load().bb_init(int(device_index)), "bb_init")
     _inited.add(device_index)
+
+
+def device_stream(t: torch.Tensor):
+    """(device, ordinal, raw current stream) of a CUDA tensor; the library is initialised on that device on first use"""
+    dev = t.device
+    idx = dev.index if dev.index is not None else torch.cuda.current_device()
+    if idx not in _inited:
+        ensure_init(idx)
+    return dev, idx, torch.cuda.current_stream(idx).cuda_stream
+
+
+def call(name: str, device: int, *args) -> None:
+    """the library entry point `name` with the device of ordinal `device` current (the kernels launch on the calling thread's
+    current device); raises RuntimeError with the library's message when it fails"""
+    fn = getattr(_lib or load(), name)
+    if device != torch.cuda.current_device():
+        with torch.cuda.device(device):
+            rc = fn(*args)
+    else:
+        rc = fn(*args)
+    if rc != 0:   # tested here too: every decode step comes through this function, and the success path calls nothing more
+        check(rc, name)
+
+
+_TORCH_DTYPE_IDS = {getattr(torch, name): i for name, i in DTYPE_IDS.items()}
+
+
+def dtype_id(dtype: torch.dtype) -> int:
+    return _TORCH_DTYPE_IDS[dtype]
+
+
+def check_tensor(t, name: str, dtype: torch.dtype, dim: int = None, numel: int = None) -> None:
+    """a tensor argument of a library call: a contiguous CUDA torch.Tensor of `dtype`, `dim`-D and of `numel` elements where
+    given.  The type is checked before the device, so a CPU tensor of the wrong type reports its type."""
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"{name} must be a torch.Tensor")
+    if dim is not None and (t.dtype != dtype or t.dim() != dim):
+        raise TypeError(f"{name} must be a {dim}-D {dtype} tensor (got {t.dim()}-D {t.dtype})")
+    if t.dtype != dtype:
+        raise TypeError(f"{name} has dtype {t.dtype}, expected {dtype}")
+    if not t.is_cuda:
+        raise RuntimeError(f"{name} must be a CUDA tensor: bitblas_b200 has no CPU path")
+    if not t.is_contiguous():
+        raise ValueError(f"{name} must be contiguous")
+    if numel is not None and t.numel() != numel:
+        raise ValueError(f"{name} has {t.numel()} elements, expected {numel}")
 
 
 def kernel_name(kernel_id: int) -> str:

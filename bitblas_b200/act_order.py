@@ -16,7 +16,6 @@ from types import SimpleNamespace
 import torch
 
 from . import _lib
-from .moe import _check, _device_ready
 
 
 def perm_from_g_idx(g_idx, K: int, group_size: int):
@@ -92,33 +91,30 @@ def permute_cols(A: torch.Tensor, perm: torch.Tensor, offsets: torch.Tensor = No
     group claims are left unwritten.  Perm values are clamped to [0, K), offsets to [0, rows].  Returns output ([rows, K])."""
     if not isinstance(A, torch.Tensor) or A.dtype not in (torch.float16, torch.bfloat16):
         raise TypeError("A must be a float16 or bfloat16 torch.Tensor")
-    _check(A, "A", A.dtype, 2)
+    _lib.check_tensor(A, "A", A.dtype, 2)
     rows, K = A.shape
     if offsets is None:
-        _check(perm, "perm", torch.int32, 1)
+        _lib.check_tensor(perm, "perm", torch.int32, 1)
         if perm.numel() != K:
             raise ValueError(f"perm must be [K={K}] without offsets (got {tuple(perm.shape)})")
         E = 1
     else:
-        _check(offsets, "offsets", torch.int32, 1)
-        _check(perm, "perm", torch.int32, 2)
+        _lib.check_tensor(offsets, "offsets", torch.int32, 1)
+        _lib.check_tensor(perm, "perm", torch.int32, 2)
         E = offsets.numel() - 1
         if tuple(perm.shape) != (E, K):
             raise ValueError(f"perm must be [E={E}, K={K}] for {E + 1} offsets (got {tuple(perm.shape)})")
     if perm.device != A.device or (offsets is not None and offsets.device != A.device):
         raise ValueError("A, perm and offsets must be on the same device")
-    dev, stream = _device_ready(A)
+    dev, idx, stream = _lib.device_stream(A)
     if output is None:
         output = torch.empty_like(A)
     else:
-        _check(output, "output", A.dtype, 2)
+        _lib.check_tensor(output, "output", A.dtype, 2)
         if tuple(output.shape) != (rows, K) or output.device != dev:
             raise ValueError(f"output must be [{rows}, {K}] on {dev}")
-    with torch.cuda.device(dev):
-        rc = _lib.load().bb_permute_cols(A.data_ptr(), output.data_ptr(), perm.data_ptr(), rows, K,
-                                         _lib.DTYPE_IDS[str(A.dtype)[6:]], E, None if offsets is None else offsets.data_ptr(),
-                                         stream)
-    _lib.check(rc, "bb_permute_cols")
+    _lib.call("bb_permute_cols", idx, A.data_ptr(), output.data_ptr(), perm.data_ptr(), rows, K, _lib.dtype_id(A.dtype), E,
+              None if offsets is None else offsets.data_ptr(), stream)
     return output
 
 

@@ -3,14 +3,13 @@
 Same constructor, buffers (``qweight`` / ``scales`` / ``zeros`` / ``bias`` or ``weight``; shapes and dtypes as in
 module/__init__.py:164-205 so reference checkpoints load), ``forward``, ``load_and_transform_weight`` and the GPTQ
 repack entry points.  Differences that matter here: the output is ``torch.empty`` (the reference memsets with
-``torch.zeros`` on every call, :277), the pointer list is built once, and the GPTQ repack runs as device kernels
-(bb_repack_gptq_*_device) instead of Python column loops (:24-74).
+``torch.zeros`` on every call, :277), ``forward`` is ``Matmul.forward`` on the layer's buffers (checked once per distinct set)
+instead of a pointer list handed to ``lib.call``, and the GPTQ repack runs as device kernels (bb_repack_gptq_*_device) instead of
+Python column loops (:24-74).
 """
 from __future__ import annotations
 
 import ctypes
-import operator
-from functools import reduce
 from logging import getLogger
 from typing import List, Optional, Union
 
@@ -105,7 +104,6 @@ class Linear(nn.Module):
         # for every other layer
         self.register_buffer("perm", None)
         self.q_params = None
-        self._q_param_key = None
 
     # ---- construction helpers ------------------------------------------------------------------------
     def _buffer_specs(self, bias: bool):
@@ -137,29 +135,13 @@ class Linear(nn.Module):
             global_operator_cache.add(config, op)
         return op
 
-    def _live_params(self):
-        """tensors `lib.call` needs after the activations, in the reference's positional order."""
-        cfg = self.bitblas_matmul.config
-        if self.consistent:
-            named = [("weight", True), ("bias", cfg.with_bias)]
-        else:
-            named = [("qweight", True), ("scales", cfg.with_scaling), ("zeros", cfg.with_zeros), ("bias", cfg.with_bias)]
-        return [getattr(self, name) for name, used in named if used]
-
-    def _check_live_params(self, params, device):
-        """the operator's parameter checks (dtype, element count, contiguity, CUDA) on the live buffers, and all of them on
-        `device`, A's: `lib.call` hands the kernel bare pointers"""
-        cfg = self.bitblas_matmul.config
-        self.bitblas_matmul._check_params(self.qweight, self.scales if cfg.with_scaling else None,
-                                          self.zeros if cfg.with_zeros else None, self.bias if cfg.with_bias else None)
-        for t in params:
-            if t.device != device:
-                raise ValueError(f"the layer's buffers must be on A's device {device} (a buffer is on {t.device})")
-
     def init_params(self):
-        tensors = self._live_params()
-        self.q_params = [ctypes.c_void_p(t.data_ptr()) for t in tensors]
-        self._q_param_key = tuple(t.data_ptr() for t in tensors)
+        """``q_params``: the buffers' pointers in ``lib.call``'s positional order, for integrations that call it themselves after
+        loading (the reference's surface).  ``forward`` does not read them."""
+        cfg = self.bitblas_matmul.config
+        named = [("weight", True)] if self.consistent else [("qweight", True), ("scales", cfg.with_scaling), ("zeros", cfg.with_zeros)]
+        named.append(("bias", cfg.with_bias))
+        self.q_params = [ctypes.c_void_p(getattr(self, name).data_ptr()) for name, used in named if used]
 
     def warmup(self, topk=20):
         self.bitblas_matmul.hardware_aware_finetune(topk=topk)
@@ -168,30 +150,15 @@ class Linear(nn.Module):
         op = self.bitblas_matmul
         if self.consistent:
             return op.forward(A, self.weight, bias=self.bias, output=output)
-        if not A.is_cuda:
-            raise RuntimeError("A must be a CUDA tensor: bitblas_b200 has no CPU path")
         if not A.is_contiguous():
             A = A.contiguous()
-        if A.dtype != self.torch_dtype:
-            raise TypeError(f"A has dtype {A.dtype}, expected {self.torch_dtype}")
-        if A.shape[-1] != self.in_features:
-            raise ValueError(f"A has inner dimension {A.shape[-1]}, expected {self.in_features}")
-        stream = torch.cuda.current_stream(A.device)
-        # the reference rebuilds this list on every call (module/__init__.py:274); rebuild, and validate the buffers the kernel
-        # reads through raw pointers, only if a buffer moved
-        params = self._live_params()
-        if self.q_params is None or self._q_param_key != tuple(t.data_ptr() for t in params):
-            self._check_live_params(params, A.device)
-            self.init_params()
-        output = op._output_for(A, output)
+        cfg = op.config
+        # every check of Matmul.forward passes before the act-order gather: a refused call launches nothing
+        output, ptrs = op._check_forward(A, self.qweight, self.scales if cfg.with_scaling else None,
+                                         self.zeros if cfg.with_zeros else None, self.bias if cfg.with_bias else None, output)
         if self.perm is not None:   # act-order: the weight's K axis is sorted, so A's columns are gathered to match
             A = act_order.permute_cols(A.view(-1, self.in_features), self.perm).view(A.shape)
-        args = [ctypes.c_void_p(A.data_ptr()), *self.q_params, ctypes.c_void_p(output.data_ptr())]
-        if op.dynamic_range is not None:
-            args.append(reduce(operator.mul, A.shape[:-1], 1))
-        args.append(ctypes.c_void_p(stream.cuda_stream))
-        op.lib.call(*args)
-        return output
+        return op._launch(A, ptrs, output)
 
     def load_and_transform_weight(self, weight: torch.Tensor, scales: torch.Tensor = None, zeros: torch.Tensor = None,
                                   bias: torch.Tensor = None):
@@ -212,7 +179,6 @@ class Linear(nn.Module):
             if bias is not None:
                 self.bias = bias
             self.perm = None   # field values come in input-column order
-        self.q_params = None
 
     def _load_from_state_dict(self, state_dict, prefix, *args, **kwargs):
         if not self.consistent:
@@ -222,7 +188,6 @@ class Linear(nn.Module):
     def _repack(self, gptq_module, device, v2: bool):
         """module/__init__.py:315-363 as two device kernels (qweight transpose+permute, qzeros unpack).  An act-order module
         (g_idx, see act_order.py) has its qweight's K axis sorted first and keeps the order in `perm`."""
-        lib = _lib.load()
         dev = torch.device(device)
         if dev.type != "cuda":
             raise RuntimeError("repack_from_gptq needs a CUDA device: bitblas_b200 has no CPU path")
@@ -232,10 +197,9 @@ class Linear(nn.Module):
                              "stored in the activations' type")
         if self.bias is not None and getattr(gptq_module, "bias", None) is None:
             raise ValueError("the layer has bias=True but the GPTQ module has no bias")
-        _lib.ensure_init(dev.index if dev.index is not None else torch.cuda.current_device())
         bits = self.bits
-        stream = torch.cuda.current_stream(dev).cuda_stream
         qw = gptq_module.qweight.to(dev).contiguous().view(torch.int32)  # [K*bits/32, N]
+        _, idx, stream = _lib.device_stream(qw)
         K, N = self.in_features, self.out_features
         assert qw.shape == (K * bits // 32, N), f"unexpected GPTQ qweight shape {tuple(qw.shape)}"
         perm = act_order.perm_from_g_idx(getattr(gptq_module, "g_idx", None), K, self.group_size)
@@ -244,27 +208,23 @@ class Linear(nn.Module):
             qw = act_order.permute_gptq_qweight(qw, perm, bits)
         out = torch.empty(op.retrieve_weight_shape(), dtype=torch.int8, device=dev)
         tgt = op.weight_transform.interleave_target if op.weight_transform is not None else 0
-        with torch.cuda.device(dev):
-            _lib.check(lib.bb_repack_gptq_qweight_device(qw.data_ptr(), out.data_ptr(), K, N, bits, tgt, stream),
-                       "bb_repack_gptq_qweight_device")
-            self.qweight = op.tile_weight(out) if op.weight_tiled else out   # propagate_b: slab tiling of the packed rows
-            # converted, not reinterpreted: checkpoints usually store float16 scales, whatever the layer's type
-            self.scales = gptq_module.scales.to(dev).T.to(self.torch_dtype).contiguous()
-            qz = gptq_module.qzeros.to(dev).contiguous().view(torch.int32)  # [K/g, N*bits/32]
-            G = K // self.group_size
-            mode = op.config.zeros_mode
-            if mode == "quantized":
-                zeros = torch.empty((G, N * bits // 8), dtype=torch.int8, device=dev)
-            else:
-                zeros = torch.empty((N, G), dtype=self.torch_dtype, device=dev)
-            _lib.check(lib.bb_repack_gptq_qzeros_device(qz.data_ptr(), self.scales.data_ptr(), zeros.data_ptr(), G, N, bits,
-                                                        _lib.ZEROS_IDS[mode], _lib.DTYPE_IDS[op.A_dtype], int(v2), stream),
-                       "bb_repack_gptq_qzeros_device")
-            self.zeros = zeros
+        _lib.call("bb_repack_gptq_qweight_device", idx, qw.data_ptr(), out.data_ptr(), K, N, bits, tgt, stream)
+        self.qweight = op.tile_weight(out) if op.weight_tiled else out   # propagate_b: slab tiling of the packed rows
+        # converted, not reinterpreted: checkpoints usually store float16 scales, whatever the layer's type
+        self.scales = gptq_module.scales.to(dev).T.to(self.torch_dtype).contiguous()
+        qz = gptq_module.qzeros.to(dev).contiguous().view(torch.int32)  # [K/g, N*bits/32]
+        G = K // self.group_size
+        mode = op.config.zeros_mode
+        if mode == "quantized":
+            zeros = torch.empty((G, N * bits // 8), dtype=torch.int8, device=dev)
+        else:
+            zeros = torch.empty((N, G), dtype=self.torch_dtype, device=dev)
+        _lib.call("bb_repack_gptq_qzeros_device", idx, qz.data_ptr(), self.scales.data_ptr(), zeros.data_ptr(), G, N, bits,
+                  _lib.ZEROS_IDS[mode], _lib.DTYPE_IDS[op.A_dtype], int(v2), stream)
+        self.zeros = zeros
         if self.bias is not None:
             self.bias = gptq_module.bias.data.to(dev).to(self.torch_dtype).contiguous()
         self.perm = perm
-        self.q_params = None
 
     def repack_from_gptq(self, gptq_module, device="cuda"):
         self._repack(gptq_module, device, v2=False)

@@ -18,6 +18,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from .act_order import perm_from_g_idx, permute_cols, permute_gptq_rows
 
 INTERLEAVE_ROWS = 8
 # kind -> (axis holding the rows, rows per element along it: None = 1, "bits" = 8 / bits packed rows per byte)
@@ -64,48 +65,27 @@ def deinterleave_gate_up(fused: torch.Tensor, kind: str, bits: int = None):
     return gate, up
 
 
-def _device_ready(t: torch.Tensor):
-    dev = t.device
-    idx = dev.index if dev.index is not None else torch.cuda.current_device()
-    if idx not in _lib._inited:
-        _lib.ensure_init(idx)
-    return dev, torch.cuda.current_stream(dev).cuda_stream
-
-
-def _check(t, name, dtype, dim):
-    if not isinstance(t, torch.Tensor):
-        raise TypeError(f"{name} must be a torch.Tensor")
-    if t.dtype != dtype or t.dim() != dim:
-        raise TypeError(f"{name} must be a {dim}-D {dtype} tensor (got {t.dim()}-D {t.dtype})")
-    if not t.is_cuda:
-        raise RuntimeError(f"{name} must be a CUDA tensor: bitblas_b200 has no CPU path")
-    if not t.is_contiguous():
-        raise ValueError(f"{name} must be contiguous")
-
-
 def moe_route(topk_ids: torch.Tensor, x: torch.Tensor, num_experts: int):
     """Route the tokens of x [T, K] (fp16 / bf16) by topk_ids (int32 [T, k]) on the device, in one launch (bb_moe_route).
     Returns (offsets int32 [E + 1], slot_rows int32 [T*k], x_sorted [T*k, K]): slot t*k + j goes to sorted row slot_rows[t*k + j]
     of expert topk_ids[t, j]; rows are ordered by expert, then by slot.  Ids outside [0, E) are dropped (slot_rows = -1) and
     x_sorted rows offsets[E] .. T*k - 1 are left unwritten."""
-    _check(topk_ids, "topk_ids", torch.int32, 2)
+    _lib.check_tensor(topk_ids, "topk_ids", torch.int32, 2)
     if not isinstance(x, torch.Tensor) or x.dtype not in (torch.float16, torch.bfloat16):
         raise TypeError("x must be a float16 or bfloat16 torch.Tensor")
-    _check(x, "x", x.dtype, 2)
+    _lib.check_tensor(x, "x", x.dtype, 2)
     T, k = topk_ids.shape
     if x.shape[0] != T:
         raise ValueError(f"x has {x.shape[0]} rows, topk_ids {T}")
     if x.device != topk_ids.device:
         raise ValueError("x and topk_ids must be on the same device")
-    dev, stream = _device_ready(x)
+    dev, idx, stream = _lib.device_stream(x)
     E, K = int(num_experts), x.shape[1]
     offsets = torch.empty(max(E, 0) + 1, dtype=torch.int32, device=dev)
     slot_rows = torch.empty(T * k, dtype=torch.int32, device=dev)
     x_sorted = torch.empty((T * k, K), dtype=x.dtype, device=dev)
-    with torch.cuda.device(dev):
-        rc = _lib.load().bb_moe_route(topk_ids.data_ptr(), T, k, E, x.data_ptr(), _lib.DTYPE_IDS[str(x.dtype)[6:]], K,
-                                      offsets.data_ptr(), slot_rows.data_ptr(), x_sorted.data_ptr(), stream)
-    _lib.check(rc, "bb_moe_route")
+    _lib.call("bb_moe_route", idx, topk_ids.data_ptr(), T, k, E, x.data_ptr(), _lib.dtype_id(x.dtype), K,
+              offsets.data_ptr(), slot_rows.data_ptr(), x_sorted.data_ptr(), stream)
     return offsets, slot_rows, x_sorted
 
 
@@ -113,17 +93,15 @@ def moe_route_index(topk_ids: torch.Tensor, num_experts: int):
     """moe_route without the copy, in one launch (bb_moe_route_index).  Returns (offsets int32 [E + 1], slot_rows int32 [T*k],
     row_token int32 [T*k]): offsets and slot_rows are exactly moe_route's, and row_token[slot_rows[s]] = s // k for every kept
     slot s, so x[row_token] is moe_route's x_sorted.  Rows offsets[E] .. T*k - 1 of row_token are left unwritten."""
-    _check(topk_ids, "topk_ids", torch.int32, 2)
+    _lib.check_tensor(topk_ids, "topk_ids", torch.int32, 2)
     T, k = topk_ids.shape
-    dev, stream = _device_ready(topk_ids)
+    dev, idx, stream = _lib.device_stream(topk_ids)
     E = int(num_experts)
     offsets = torch.empty(max(E, 0) + 1, dtype=torch.int32, device=dev)
     slot_rows = torch.empty(T * k, dtype=torch.int32, device=dev)
     row_token = torch.empty(T * k, dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        rc = _lib.load().bb_moe_route_index(topk_ids.data_ptr(), T, k, E, offsets.data_ptr(), slot_rows.data_ptr(),
-                                            row_token.data_ptr(), stream)
-    _lib.check(rc, "bb_moe_route_index")
+    _lib.call("bb_moe_route_index", idx, topk_ids.data_ptr(), T, k, E, offsets.data_ptr(), slot_rows.data_ptr(),
+              row_token.data_ptr(), stream)
     return offsets, slot_rows, row_token
 
 
@@ -133,26 +111,24 @@ def moe_combine(y_sorted: torch.Tensor, slot_rows: torch.Tensor, topk_weights: t
     int32 [T*k], topk_weights float32 [T, k]; returns [T, N]."""
     if not isinstance(y_sorted, torch.Tensor) or y_sorted.dtype not in (torch.float16, torch.bfloat16, torch.float32):
         raise TypeError("y_sorted must be a float16, bfloat16 or float32 torch.Tensor")
-    _check(y_sorted, "y_sorted", y_sorted.dtype, 2)
-    _check(topk_weights, "topk_weights", torch.float32, 2)
-    _check(slot_rows, "slot_rows", torch.int32, 1)
+    _lib.check_tensor(y_sorted, "y_sorted", y_sorted.dtype, 2)
+    _lib.check_tensor(topk_weights, "topk_weights", torch.float32, 2)
+    _lib.check_tensor(slot_rows, "slot_rows", torch.int32, 1)
     T, k = topk_weights.shape
     N = y_sorted.shape[1]
     if slot_rows.numel() != T * k or y_sorted.shape[0] != T * k:
         raise ValueError(f"slot_rows and y_sorted need T*k = {T * k} rows (got {slot_rows.numel()} and {y_sorted.shape[0]})")
     if not (y_sorted.device == slot_rows.device == topk_weights.device):
         raise ValueError("y_sorted, slot_rows and topk_weights must be on the same device")
-    dev, stream = _device_ready(y_sorted)
+    dev, idx, stream = _lib.device_stream(y_sorted)
     if output is None:
         output = torch.empty((T, N), dtype=y_sorted.dtype, device=dev)
     else:
-        _check(output, "output", y_sorted.dtype, 2)
+        _lib.check_tensor(output, "output", y_sorted.dtype, 2)
         if tuple(output.shape) != (T, N) or output.device != dev:
             raise ValueError(f"output must be [T={T}, N={N}] on {dev}")
-    with torch.cuda.device(dev):
-        rc = _lib.load().bb_moe_combine(slot_rows.data_ptr(), topk_weights.data_ptr(), y_sorted.data_ptr(),
-                                        _lib.DTYPE_IDS[str(y_sorted.dtype)[6:]], output.data_ptr(), T, k, N, stream)
-    _lib.check(rc, "bb_moe_combine")
+    _lib.call("bb_moe_combine", idx, slot_rows.data_ptr(), topk_weights.data_ptr(), y_sorted.data_ptr(),
+              _lib.dtype_id(y_sorted.dtype), output.data_ptr(), T, k, N, stream)
     return output
 
 
@@ -205,19 +181,17 @@ def moe_topk(router_logits: torch.Tensor, top_k: int, scoring: str = "softmax", 
             raise TypeError(f"correction_bias must be a float32 tensor of shape [E={E}]")
         if correction_bias.device != router_logits.device:
             raise ValueError("router_logits and correction_bias must be on the same device")
-        _check(correction_bias, "correction_bias", torch.float32, 1)
-    _check(router_logits, "router_logits", router_logits.dtype, 2)
-    dev, stream = _device_ready(router_logits)
+        _lib.check_tensor(correction_bias, "correction_bias", torch.float32, 1)
+    _lib.check_tensor(router_logits, "router_logits", router_logits.dtype, 2)
+    dev, idx, stream = _lib.device_stream(router_logits)
     k = int(top_k)
     topk_ids = torch.empty((T, max(k, 0)), dtype=torch.int32, device=dev)
     topk_weights = torch.empty((T, max(k, 0)), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        rc = _lib.load().bb_moe_topk(router_logits.data_ptr(), _lib.DTYPE_IDS[str(router_logits.dtype)[6:]], T, E, k,
-                                     _SCORING[scoring], None if correction_bias is None else correction_bias.data_ptr(),
-                                     int(num_expert_group) if grouped else 0, int(topk_group) if grouped else 0,
-                                     _GROUP_SCORE[group_score], int(bool(renormalize)), float(routed_scaling_factor),
-                                     topk_ids.data_ptr(), topk_weights.data_ptr(), stream)
-    _lib.check(rc, "bb_moe_topk")
+    _lib.call("bb_moe_topk", idx, router_logits.data_ptr(), _lib.dtype_id(router_logits.dtype), T, E, k,
+              _SCORING[scoring], None if correction_bias is None else correction_bias.data_ptr(),
+              int(num_expert_group) if grouped else 0, int(topk_group) if grouped else 0,
+              _GROUP_SCORE[group_score], int(bool(renormalize)), float(routed_scaling_factor),
+              topk_ids.data_ptr(), topk_weights.data_ptr(), stream)
     return topk_ids, topk_weights
 
 
@@ -256,7 +230,6 @@ class MoEExperts(nn.Module):
         offsets, slot_rows, x_sorted = moe_route(topk_ids, x, self.num_experts)
         gu, cfg = self.gate_up, self.gate_up.bitblas_matmul.config
         if gu.perm is not None:
-            from .act_order import permute_cols
             x_sorted = permute_cols(x_sorted, gu.perm, offsets)
         h = gu.bitblas_matmul.forward_grouped_swiglu(x_sorted, gu.qweight, offsets, gu.scales if cfg.with_scaling else None,
                                                      gu.zeros if cfg.with_zeros else None, gu.bias)
@@ -278,7 +251,6 @@ class MoEExperts(nn.Module):
         self.down.load_and_transform_weight(*down)
 
     def _repack(self, gate_modules, up_modules, down_modules, device, v2):
-        from .act_order import perm_from_g_idx, permute_gptq_rows
         from .module import GroupedLinear
         E, H, I = self.num_experts, self.hidden_size, self.intermediate_size
         if not len(gate_modules) == len(up_modules) == len(down_modules) == E:

@@ -165,11 +165,9 @@ class WeightTransform:
             raise ValueError(f"K={cols} must be a multiple of {epw} for {self.bits}-bit storage")
         out = torch.empty(weight.shape[:-1] + (cols * self.bits // 8,), dtype=torch.int8, device=weight.device)
         if weight.is_cuda:
-            _lib.ensure_init(weight.device.index or 0)
-            stream = torch.cuda.current_stream(weight.device).cuda_stream
-            with torch.cuda.device(weight.device):
-                _lib.check(lib.bb_transform_weight_device(weight.data_ptr(), out.data_ptr(), rows, cols, self.bits,
-                                                          self.interleave_target, stream), "bb_transform_weight_device")
+            _, idx, stream = _lib.device_stream(weight)
+            _lib.call("bb_transform_weight_device", idx, weight.data_ptr(), out.data_ptr(), rows, cols, self.bits,
+                      self.interleave_target, stream)
             return out
         _lib.check(lib.bb_compress_host(weight.data_ptr(), out.data_ptr(), rows, cols, self.bits), "bb_compress_host")
         if self.interleave_target:
@@ -222,11 +220,8 @@ class _LibShim:
         scale = next(it) if op.with_scaling else 0
         zeros = next(it) if op.with_zeros else 0
         bias = next(it) if op.with_bias else 0
-        C = next(it)
-        ws_ptr, ws_bytes = op._workspace_for(m, torch.device("cuda", torch.cuda.current_device())) if torch.cuda.is_available() else (0, 0)
-        rc = self._c.bb_matmul(ctypes.byref(op._desc), A, W, lut, scale, zeros, bias, C, m, ws_ptr, ws_bytes, stream)
-        if rc != 0:
-            raise RuntimeError(f"bb_matmul failed (code {rc}): {_lib.last_error()}")
+        # bare pointers name no device: like the reference's generated `call`, this launches on the current one
+        op._launch_raw(A, W, lut, scale, zeros, bias, next(it), m, torch.cuda.current_device(), stream)
 
 
 class Matmul(Operator):
@@ -345,10 +340,8 @@ class Matmul(Operator):
             raise ValueError(f"slab tiling needs rows % {R} == 0 and row bytes % {B} == 0 (got {n} x {rb})")
         if w.is_cuda:
             out = torch.empty_like(w)
-            _lib.ensure_init(w.device.index or 0)
-            with torch.cuda.device(w.device):
-                _lib.check(_lib.load().bb_retile_weight_device(w.data_ptr(), out.data_ptr(), n, rb, int(inverse),
-                                                               torch.cuda.current_stream(w.device).cuda_stream), "bb_retile_weight_device")
+            _, idx, stream = _lib.device_stream(w)
+            _lib.call("bb_retile_weight_device", idx, w.data_ptr(), out.data_ptr(), n, rb, int(inverse), stream)
             return out
         b = w.view(torch.int8).reshape(n, rb)
         if inverse:
@@ -388,40 +381,32 @@ class Matmul(Operator):
         return input_tensor  # no ladder propagation on H100
 
     # ---- forward ------------------------------------------------------------------------------------
-    def _check_tensor(self, t: torch.Tensor, name: str, dtype: torch.dtype, numel: Optional[int] = None):
-        if not isinstance(t, torch.Tensor):
-            raise TypeError(f"{name} must be a torch.Tensor")
-        if not t.is_cuda:
-            raise RuntimeError(f"{name} must be a CUDA tensor: bitblas_b200 has no CPU path")
-        if t.dtype != dtype:
-            raise TypeError(f"{name} has dtype {t.dtype}, expected {dtype}")
-        if not t.is_contiguous():
-            raise ValueError(f"{name} must be contiguous")
-        if numel is not None and t.numel() != numel:
-            raise ValueError(f"{name} has {t.numel()} elements, expected {numel}")
-
-    def _check_params(self, W, scale, zeros, bias):
-        """full validation of the (static) parameter tensors; forward() runs it once per distinct set of tensors."""
+    def _check_params(self, W, scale, zeros, bias, device):
+        """full validation of the (static) parameter tensors, all of them on `device` (A's: the kernel gets bare pointers);
+        forward() runs it once per distinct set of tensors."""
         c = self.config
         adt = getattr(torch, c.A_dtype)
         wshape = self.retrieve_weight_shape()
-        self._check_tensor(W, "W", torch.int8 if W.dtype != torch.uint8 else torch.uint8, wshape[0] * wshape[1])
+        _lib.check_tensor(W, "W", torch.int8 if W.dtype != torch.uint8 else torch.uint8, numel=wshape[0] * wshape[1])
         G = c.K // (c.group_size if c.group_size and c.group_size > 0 else c.K)
         if c.with_scaling:
             if scale is None:
                 raise ValueError("with_scaling=True but scale is None")
-            self._check_tensor(scale, "scale", adt, c.N * G)
+            _lib.check_tensor(scale, "scale", adt, numel=c.N * G)
         if c.with_zeros:
             if zeros is None:
                 raise ValueError("with_zeros=True but zeros is None")
             if c.zeros_mode == "quantized":
-                self._check_tensor(zeros, "zeros", torch.int8, G * (c.N * self.bit // 8))
+                _lib.check_tensor(zeros, "zeros", torch.int8, numel=G * (c.N * self.bit // 8))
             else:
-                self._check_tensor(zeros, "zeros", adt, c.N * G)
+                _lib.check_tensor(zeros, "zeros", adt, numel=c.N * G)
         if c.with_bias:
             if bias is None:
                 raise ValueError("with_bias=True but bias is None")
-            self._check_tensor(bias, "bias", adt, c.N)
+            _lib.check_tensor(bias, "bias", adt, numel=c.N)
+        for t in (W, scale if c.with_scaling else None, zeros if c.with_zeros else None, bias if c.with_bias else None):
+            if t is not None and t.device != device:
+                raise ValueError(f"the layer's buffers must be on A's device {device} (a buffer is on {t.device})")
 
     def _output_for(self, A, output):
         """the output of A [.., K]: a new [.., N] tensor on A's device, or the caller's, checked to hold the m * N values"""
@@ -430,52 +415,54 @@ class Matmul(Operator):
             return torch.empty(A.shape[:-1] + (N,), dtype=self.torch_output_dtype, device=A.device)
         numel = A.numel() // self.config.K * N
         if not (output.is_cuda and output.dtype == self.torch_output_dtype and output.is_contiguous() and output.numel() == numel):
-            self._check_tensor(output, "output", self.torch_output_dtype, numel)
+            _lib.check_tensor(output, "output", self.torch_output_dtype, numel=numel)
         return output
 
     def forward(self, A, W, scale=None, zeros=None, bias=None, output=None) -> Any:
         if self.consistent:
             return self._forward_consistent(A, W, bias, output)
+        output, ptrs = self._check_forward(A, W, scale, zeros, bias, output)
+        return self._launch(A, ptrs, output)
+
+    def _check_forward(self, A, W, scale, zeros, bias, output):
+        """the checking half of forward(): validates every argument and launches nothing.  Returns the output and, for _launch,
+        the data pointers of W, scale, zeros and bias."""
         c = self.config
-        # the parameter tensors of a layer do not change between calls: validate each distinct set once (keyed on the storage
-        # pointers; a new tensor -- or a re-allocated one -- is validated again).  The activations are checked every call.
-        key = (W.data_ptr(), scale.data_ptr() if scale is not None else 0, zeros.data_ptr() if zeros is not None else 0,
-               bias.data_ptr() if bias is not None else 0)
-        if key != self._checked_key:
-            self._check_params(W, scale, zeros, bias)
-            self._checked_key = key
         if not (A.is_cuda and A.dtype == self._torch_a_dtype and A.is_contiguous()):
-            self._check_tensor(A, "A", self._torch_a_dtype)
+            _lib.check_tensor(A, "A", self._torch_a_dtype)
+        # the parameter tensors of a layer do not change between calls: validate each distinct set once (keyed on the storage
+        # pointers and A's device; a new tensor -- or a re-allocated one -- is validated again).  The activations are checked
+        # every call.
+        key = (W.data_ptr(), scale.data_ptr() if scale is not None else 0, zeros.data_ptr() if zeros is not None else 0,
+               bias.data_ptr() if bias is not None else 0, A.device)
+        if key != self._checked_key:
+            self._check_params(W, scale, zeros, bias, A.device)
+            self._checked_key = key
         K = c.K
         if A.shape[-1] != K:
             raise ValueError(f"A has inner dimension {A.shape[-1]}, expected K={K}")
-        m = A.numel() // K
-        if self.dynamic_range is None and m != int(c.M):
-            raise ValueError(f"operator was created for static M={c.M}, got {m} rows")
-        dev = A.device
-        output = self._output_for(A, output)
-        idx = dev.index if dev.index is not None else torch.cuda.current_device()
-        if idx not in _lib._inited:
-            _lib.ensure_init(idx)
-        stream = torch.cuda.current_stream(dev).cuda_stream
+        if self.dynamic_range is None and A.numel() // K != int(c.M):
+            raise ValueError(f"operator was created for static M={c.M}, got {A.numel() // K} rows")
+        return self._output_for(A, output), key
+
+    def _launch(self, A, ptrs, output):
+        """the launching half of forward(): A is the checked activations, or a column gather of them (Linear's act-order)"""
+        dev, idx, stream = _lib.device_stream(A)
         lut = self.lut
         if lut is not None and lut.device != dev:
             lut = self.lut = lut.to(dev)
-        ws_ptr, ws_bytes = self._workspace_for(m, dev, stream)
-        if idx != torch.cuda.current_device():
-            with torch.cuda.device(dev):   # the kernels launch on the calling thread's current device
-                rc = self.lib._c.bb_matmul(self._desc_ref, A.data_ptr(), key[0], lut.data_ptr() if lut is not None else 0,
-                                           key[1], key[2], key[3], output.data_ptr(), m, ws_ptr, ws_bytes, stream)
-        else:
-            rc = self.lib._c.bb_matmul(self._desc_ref, A.data_ptr(), key[0], lut.data_ptr() if lut is not None else 0,
-                                       key[1], key[2], key[3], output.data_ptr(), m, ws_ptr, ws_bytes, stream)
-        if rc != 0:
-            raise RuntimeError(f"bb_matmul failed (code {rc}): {_lib.last_error()}")
+        self._launch_raw(A.data_ptr(), ptrs[0], lut.data_ptr() if lut is not None else 0, ptrs[1], ptrs[2], ptrs[3],
+                        output.data_ptr(), A.numel() // self.config.K, idx, stream)
         return output
 
-    def _workspace_for(self, m: int, device, stream=None):
+    def _launch_raw(self, A, W, lut, scale, zeros, bias, C, m, device, stream):
+        """the package's one bb_matmul call: raw pointers (0 = absent), m rows, on the device of ordinal `device`"""
+        ws_ptr, ws_bytes = self._workspace_for(m, device, stream)
+        _lib.call("bb_matmul", device, self._desc_ref, A, W, lut, scale, zeros, bias, C, m, ws_ptr, ws_bytes, stream)
+
+    def _workspace_for(self, m: int, device: int, stream: int):
         """scratch the kernel picked for `m` needs (bb_workspace_bytes: split-K partials, stream-K exchange slots); one cached,
-        ZERO-INITIALISED buffer per operator, device and stream, grown on demand.  The m = 1 slab kernel leaves its slots
+        ZERO-INITIALISED buffer per operator, device (ordinal) and stream, grown on demand.  The m = 1 slab kernel leaves its slots
         zero-tagged, so the buffer is reused by later calls on the same stream without clearing (include/bitblas_b200.h)."""
         key = (int(m), _lib.OVERRIDE_GEN)
         need = self._ws_need.get(key)
@@ -483,10 +470,10 @@ class Matmul(Operator):
             need = self._ws_need[key] = int(self.lib._c.bb_workspace_bytes(ctypes.byref(self._desc), int(m)))
         if need == 0:
             return 0, 0
-        wkey = (device, stream if stream is not None else torch.cuda.current_stream(device).cuda_stream)
+        wkey = (device, stream)
         ws = self._ws.get(wkey)
         if ws is None or ws.numel() < need:
-            ws = torch.zeros(need, dtype=torch.uint8, device=device)
+            ws = torch.zeros(need, dtype=torch.uint8, device=torch.device("cuda", device))
             self._ws[wkey] = ws
         return ws.data_ptr(), ws.numel()
 
@@ -497,8 +484,7 @@ class Matmul(Operator):
         if self.consistent:
             raise NotImplementedError("forward_scatter needs a low-bit weight operator")
         c = self.config
-        adt = getattr(torch, c.A_dtype)
-        self._check_tensor(A, "A", adt)
+        _lib.check_tensor(A, "A", self._torch_a_dtype)
         if A.shape[-1] != c.K:
             raise ValueError(f"A has inner dimension {A.shape[-1]}, expected K={c.K}")
         m = reduce(_operator.mul, A.shape[:-1], 1)
@@ -507,20 +493,16 @@ class Matmul(Operator):
             arr = peer_ptrs
         else:
             arr = (ctypes.c_void_p * n)(*[ctypes.c_void_p(int(x)) for x in peer_ptrs])
-        dev = A.device.index if A.device.index is not None else torch.cuda.current_device()
-        _lib.ensure_init(dev)
-        stream = torch.cuda.current_stream(device=A.device).cuda_stream
+        dev, idx, stream = _lib.device_stream(A)
         lut = self.lut
-        if lut is not None and lut.device != A.device:
-            lut = self.lut = lut.to(A.device)
-        rc = self.lib._c.bb_matmul_scatter(ctypes.byref(self._desc), A.data_ptr(), W.data_ptr(),
-                                           lut.data_ptr() if lut is not None else 0,
-                                           scale.data_ptr() if c.with_scaling else 0,
-                                           zeros.data_ptr() if c.with_zeros else 0,
-                                           bias.data_ptr() if c.with_bias else 0,
-                                           arr, n, int(ldc), int(col_offset), int(m), *self._workspace_for(int(m), A.device), stream)
-        if rc != 0:
-            raise RuntimeError(f"bb_matmul_scatter failed (code {rc}): {_lib.last_error()}")
+        if lut is not None and lut.device != dev:
+            lut = self.lut = lut.to(dev)
+        _lib.call("bb_matmul_scatter", idx, self._desc_ref, A.data_ptr(), W.data_ptr(),
+                  lut.data_ptr() if lut is not None else 0,
+                  scale.data_ptr() if c.with_scaling else 0,
+                  zeros.data_ptr() if c.with_zeros else 0,
+                  bias.data_ptr() if c.with_bias else 0,
+                  arr, n, int(ldc), int(col_offset), int(m), *self._workspace_for(int(m), idx, stream), stream)
 
     # ---- grouped (mixture-of-experts) forward -----------------------------------------------------------------------------
     def check_grouped(self, num_groups: int, swiglu: bool = False) -> None:
@@ -553,7 +535,7 @@ class Matmul(Operator):
             if tuple(t.shape) != shape:
                 raise ValueError(f"{name} has shape {tuple(t.shape)}, expected the stacked shape {shape}")
         for name, t, dtype, shape, _ in specs:
-            self._check_tensor(t, name, dtype)
+            _lib.check_tensor(t, name, dtype)
 
     def forward_grouped(self, A, W, offsets, scale=None, zeros=None, bias=None, output=None, capturable=False):
         """Grouped matmul for mixture-of-experts layers (bb_matmul_grouped): E problems of this operator's config.  A [T, K] holds
@@ -573,12 +555,11 @@ class Matmul(Operator):
         if self.consistent:
             raise NotImplementedError("forward_grouped needs a low-bit weight operator")
         E, T, ptrs, output, dev, stream = self._grouped_prepare(A, W, offsets, scale, zeros, bias, output, self.config.N)
-        with torch.cuda.device(dev):   # the kernels launch on the calling thread's current device
-            if T <= GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E or capturable:
-                name = "bb_matmul_grouped" if self._grouped_single_launch(T, E) == "gemv" else "bb_matmul_grouped_gemm"
-                self._grouped_call(name, dev, E, offsets.data_ptr(), A.data_ptr(), *ptrs, output.data_ptr(), T, stream)
-            else:
-                self._forward_grouped_per_group(A, W, offsets, scale, zeros, bias, output, dev, stream)
+        if T <= GROUPED_SINGLE_LAUNCH_MAX_ROWS_PER_GROUP * E or capturable:
+            name = "bb_matmul_grouped" if self._grouped_single_launch(T, E) == "gemv" else "bb_matmul_grouped_gemm"
+            _lib.call(name, dev, self._desc_ref, E, offsets.data_ptr(), A.data_ptr(), *ptrs, output.data_ptr(), T, stream)
+        else:
+            self._forward_grouped_per_group(A, W, offsets, scale, zeros, bias, output, dev, stream)
         return output
 
     def forward_grouped_swiglu(self, A, W, offsets, scale=None, zeros=None, bias=None, output=None, row_index=None):
@@ -599,7 +580,7 @@ class Matmul(Operator):
         E, T, ptrs, output, dev, stream = self._grouped_prepare(A, W, offsets, scale, zeros, bias, output, self.config.N // 2,
                                                                 swiglu=True)
         name = "bb_matmul_grouped_swiglu" if self._grouped_single_launch(T, E) == "gemv" else "bb_matmul_grouped_gemm_swiglu"
-        self._grouped_call(name, dev, E, offsets.data_ptr(), A.data_ptr(), *ptrs, output.data_ptr(), T, stream)
+        _lib.call(name, dev, self._desc_ref, E, offsets.data_ptr(), A.data_ptr(), *ptrs, output.data_ptr(), T, stream)
         return output
 
     def _forward_grouped_swiglu_gather(self, A, W, offsets, scale, zeros, bias, output, row_index):
@@ -610,21 +591,14 @@ class Matmul(Operator):
                                                                 swiglu=True, rows=row_index.numel())
         if not self._grouped_gemm_ok:
             raise ValueError(f"{name} does not cover this configuration: {self._grouped_gemm_err}")
-        self._check_tensor(row_index, "row_index", torch.int32)
-        if row_index.device != dev:
+        _lib.check_tensor(row_index, "row_index", torch.int32)
+        if row_index.device != A.device:
             raise ValueError("row_index must be on A's device")
         if T > 0 and A.shape[0] < 1:
             raise ValueError("A must have at least one row to gather from")
-        self._grouped_call(name, dev, E, offsets.data_ptr(), row_index.data_ptr(), A.data_ptr(), A.shape[0], *ptrs,
-                           output.data_ptr(), T, stream)
+        _lib.call(name, dev, self._desc_ref, E, offsets.data_ptr(), row_index.data_ptr(), A.data_ptr(), A.shape[0], *ptrs,
+                  output.data_ptr(), T, stream)
         return output
-
-    def _grouped_call(self, name, dev, *args):
-        """the grouped library entry point `name` on this operator's descriptor, launched on `dev` (the kernels run on the calling
-        thread's current device); raises RuntimeError with the library's message when it fails"""
-        with torch.cuda.device(dev):
-            rc = getattr(self.lib._c, name)(self._desc_ref, *args)
-        _lib.check(rc, name)
 
     def _grouped_single_launch(self, T: int, E: int) -> str:
         """the kernel of the one capturable grouped launch for T rows over E groups: the grouped GEMV ("gemv") up to
@@ -634,7 +608,7 @@ class Matmul(Operator):
 
     def _grouped_prepare(self, A, W, offsets, scale, zeros, bias, output, out_cols, swiglu=False, rows=None):
         """argument checks of the grouped forwards (parameters once per distinct set); returns (E, T, parameter pointers, output
-        [T, out_cols], device, stream).  T is A's row count, or `rows` (the gathering call, whose A has any number of rows)."""
+        [T, out_cols], device ordinal, stream).  T is A's row count, or `rows` (the gathering call, whose A has any number of rows)."""
         c = self.config
         if not isinstance(offsets, torch.Tensor) or offsets.dtype != torch.int32:
             raise TypeError("offsets must be an int32 torch.Tensor of num_groups + 1 row offsets")
@@ -655,19 +629,16 @@ class Matmul(Operator):
         T = A.shape[0] if rows is None else rows
         if output is not None and (not isinstance(output, torch.Tensor) or tuple(output.shape) != (T, out_cols)):
             raise ValueError(f"output must be [T={T}, {out_cols}]")
-        self._check_tensor(A, "A", self._torch_a_dtype)
-        self._check_tensor(offsets, "offsets", torch.int32)
+        _lib.check_tensor(A, "A", self._torch_a_dtype)
+        _lib.check_tensor(offsets, "offsets", torch.int32)
         if offsets.device != A.device or W.device != A.device:
             raise ValueError("A, W and offsets must be on the same device")
-        dev = A.device
         if output is None:
-            output = torch.empty((T, out_cols), dtype=self.torch_output_dtype, device=dev)
+            output = torch.empty((T, out_cols), dtype=self.torch_output_dtype, device=A.device)
         else:
-            self._check_tensor(output, "output", self.torch_output_dtype)
-        idx = dev.index if dev.index is not None else torch.cuda.current_device()
-        if idx not in _lib._inited:
-            _lib.ensure_init(idx)
-        return E, T, key[1:5], output, dev, torch.cuda.current_stream(dev).cuda_stream
+            _lib.check_tensor(output, "output", self.torch_output_dtype)
+        _, idx, stream = _lib.device_stream(A)
+        return E, T, key[1:5], output, idx, stream
 
     def _forward_grouped_per_group(self, A, W, offsets, scale, zeros, bias, output, dev, stream):
         """prefill side of forward_grouped: one bb_matmul per non-empty group on its row slice, with the offsets clamped exactly as
@@ -678,15 +649,11 @@ class Matmul(Operator):
             r0, r1 = bounds[e], bounds[e + 1]
             if r1 <= r0:
                 continue
-            m = r1 - r0
-            ws_ptr, ws_bytes = self._workspace_for(m, dev, stream)
-            rc = self.lib._c.bb_matmul(self._desc_ref, A[r0:r1].data_ptr(), W[e].data_ptr(), 0,
-                                       scale[e].data_ptr() if self.with_scaling else 0,
-                                       zeros[e].data_ptr() if self.with_zeros else 0,
-                                       bias[e].data_ptr() if self.with_bias else 0,
-                                       output[r0:r1].data_ptr(), m, ws_ptr, ws_bytes, stream)
-            if rc != 0:
-                raise RuntimeError(f"bb_matmul failed (code {rc}): {_lib.last_error()}")
+            self._launch_raw(A[r0:r1].data_ptr(), W[e].data_ptr(), 0,
+                            scale[e].data_ptr() if self.with_scaling else 0,
+                            zeros[e].data_ptr() if self.with_zeros else 0,
+                            bias[e].data_ptr() if self.with_bias else 0,
+                            output[r0:r1].data_ptr(), r1 - r0, dev, stream)
 
     def _forward_consistent(self, A, W, bias, output):
         """A_dtype == W_dtype (no sub-byte decode; general_matmul/__init__.py:33-51,568-580): a plain library GEMM, outside the

@@ -20,6 +20,7 @@ import torch
 import torch.distributed as dist
 import torch.nn as nn
 
+from . import _lib
 from .module import Linear
 
 
@@ -31,8 +32,6 @@ class PeerBarrier:
 
     def __init__(self, device, group=None):
         import torch.distributed._symmetric_memory as symm_mem
-        from . import _lib
-        self._lib = _lib.load()
         self.group = group if group is not None else dist.group.WORLD
         self.rank = dist.get_rank(group)
         self.world = dist.get_world_size(group)
@@ -45,13 +44,11 @@ class PeerBarrier:
         self.handle.barrier(channel=0)          # every rank's flag block is zeroed before anyone signals into it
         torch.cuda.synchronize(device)
         self.device = device
+        self._ordinal = self.flags.device.index
 
     def __call__(self, stream=None):
         st = stream if stream is not None else torch.cuda.current_stream(self.device)
-        rc = self._lib.bb_peer_barrier(self._arr, self.world, self.rank, st.cuda_stream)
-        if rc != 0:
-            from . import _lib
-            raise RuntimeError(f"bb_peer_barrier failed (code {rc}): {_lib.last_error()}")
+        _lib.call("bb_peer_barrier", self._ordinal, self._arr, self.world, self.rank, st.cuda_stream)
 
 
 def shard_bounds(n: int, rank: int, world: int, multiple: int = 16):
@@ -130,7 +127,6 @@ class ColumnParallelLinear(nn.Module):
             self.local.zeros = sh["zeros"].to(dev)
         if "bias" in sh:
             self.local.bias = sh["bias"].to(dev)
-        self.local.q_params = None
 
     def _chunks_for(self, m: int) -> int:
         if self.pipeline_chunks is not None:
@@ -320,7 +316,6 @@ class RowParallelLinear(nn.Module):
             self.local.zeros = sh["zeros"].to(dev)
         if bias is not None and self.bias is not None:
             self.bias = bias.to(dev).to(self.final_dtype)
-        self.local.q_params = None
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         xs = x if self.input_is_parallel else x[..., self.k_lo:self.k_hi]
