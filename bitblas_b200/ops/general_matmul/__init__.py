@@ -111,16 +111,10 @@ class MatmulConfig(OperatorConfig):
         # propagate_b selects the slab tiling BB_TILE_SLAB (include/bitblas_b200.h: [N/32][row_bytes/512][32][512 B]; one
         # work unit of the decode GEMV = one contiguous 16 KB block).  Default (None / False): the reference's row-major
         # storage, byte-compatible with its checkpoints.  propagate_a never applies (activations are consumed as they are).
-        requested_b = self._legalize_propagate(self.propagate_b)
-        want_tile = requested_b not in (None, TransformKind.NonTransform)
-        if want_tile:
-            wbits = {"int4": 4, "uint4": 4, "int2": 2, "uint2": 2}.get(self.W_dtype)
-            ok = (wbits is not None and self.W_dtype != self.A_dtype and self.N % 128 == 0
-                  and (self.K * wbits // 8) % _lib.BB_TILE_ROW_BYTES == 0 and (self.K * wbits) % 8 == 0)
-            if not ok:
-                logger.warning("propagate_b: slab tiling needs a 4/2-bit integer weight, N %% 128 == 0 and K*bits/8 %% 512 == 0 "
-                               "(N=%s K=%s W_dtype=%s); keeping the row-major storage", self.N, self.K, self.W_dtype)
-                want_tile = False
+        want_tile = slab_tiled(self.propagate_b, self.N, self.K, self.W_dtype, self.A_dtype)
+        if not want_tile and self._legalize_propagate(self.propagate_b) not in (None, TransformKind.NonTransform):
+            logger.warning("propagate_b: slab tiling needs a 4/2-bit integer weight, N %% 128 == 0 and K*bits/8 %% 512 == 0 "
+                           "(N=%s K=%s W_dtype=%s); keeping the row-major storage", self.N, self.K, self.W_dtype)
         self._set("propagate_a", TransformKind.NonTransform)
         self._set("propagate_b", TransformKind.LDMatrixTransform if want_tile else TransformKind.NonTransform)
         if self.zeros_mode is None:
@@ -136,6 +130,18 @@ class MatmulConfig(OperatorConfig):
             self._set("with_zeros", False)
         if self.A_dtype == self.W_dtype and self.W_dtype in ["float16", "bfloat16", "int8", "e4m3_float8", "e5m2_float8"]:
             self._set("storage_dtype", self.W_dtype)
+
+
+def slab_tiled(propagate_b, N: int, K: int, W_dtype: str, A_dtype: str) -> bool:
+    """True when a requested propagate_b stores an [N, K] weight of W_dtype in the slab tiling BB_TILE_SLAB, False when it
+    legalises to (or asked for) row-major storage.  The tiling needs a 4/2-bit integer weight, N % 128 == 0 and
+    K*bits/8 % BB_TILE_ROW_BYTES == 0.  MatmulConfig legalises propagate_b with it, and the tensor-parallel loaders
+    (bitblas_b200.parallel) use it to tell whether a FULL layer's weight is tiled when only its shard has an operator."""
+    if MatmulConfig._legalize_propagate(propagate_b) in (None, TransformKind.NonTransform):
+        return False
+    wbits = {"int4": 4, "uint4": 4, "int2": 2, "uint2": 2}.get(W_dtype)
+    return (wbits is not None and W_dtype != A_dtype and N % 128 == 0 and (K * wbits // 8) % _lib.BB_TILE_ROW_BYTES == 0
+            and (K * wbits) % 8 == 0)
 
 
 class WeightTransform:
@@ -778,4 +784,4 @@ class Matmul(Operator):
         return self.weight_executors if (self.weight_executors is not None and self.weight_executors.size) else None
 
 
-__all__ = ["Matmul", "MatmulConfig", "WeightTransform", "is_native_compute"]
+__all__ = ["Matmul", "MatmulConfig", "WeightTransform", "is_native_compute", "slab_tiled"]

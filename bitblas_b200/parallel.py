@@ -22,6 +22,7 @@ import torch.nn as nn
 
 from . import _lib
 from .module import Linear
+from .ops.general_matmul import slab_tiled
 
 
 class PeerBarrier:
@@ -112,15 +113,22 @@ class ColumnParallelLinear(nn.Module):
         self.gather_output = gather_output
         self.pipeline_chunks = pipeline_chunks
         self.local = Linear(in_features, hi - lo, **linear_kwargs)
+        self._propagate_b = linear_kwargs.get("propagate_b", False)
         self._comm_stream = None
 
     def load_full_params(self, qweight, scales=None, zeros=None, bias=None):
-        """Take full-size (already transformed) parameters and keep this rank's shard."""
+        """full-size parameters in the storage of the FULL layer (as produced by Matmul.transform_weight of an operator with
+        this layer's out_features, in_features and propagate_b: slab-tiled where that layer legalises propagate_b to the tiling,
+        row-major otherwise) -> this rank's N shard, in its own operator's storage.  The two can differ: a shard of N/world
+        rows tiles only when N/world % 128 == 0."""
         op = self.local.bitblas_matmul
+        if slab_tiled(self._propagate_b, self.out_features, self.in_features, op.W_dtype, op.A_dtype):
+            qweight = op.tile_weight(qweight, inverse=True)
         sh = shard_quantized_params(qweight, scales, zeros, bias, rank=self.rank, world=self.world, bits=op.bit,
                                     zeros_mode=op.config.zeros_mode)
         dev = self.local.qweight.device
-        self.local.qweight = sh["qweight"].to(dev)
+        w = sh["qweight"].to(dev)
+        self.local.qweight = op.tile_weight(w) if op.weight_tiled else w
         if "scales" in sh:
             self.local.scales = sh["scales"].to(dev)
         if "zeros" in sh:
@@ -290,18 +298,23 @@ class RowParallelLinear(nn.Module):
         # partial sums leave the kernel in fp32 (the all-reduce must not round per rank); bias is added after the reduction
         self.local = Linear(self.k_per, out_features, bias=False, out_dtype="float32" if self.world > 1 else out_dtype, **linear_kwargs)
         self._whole_row_groups = gs in (-1, None)
+        self._propagate_b = linear_kwargs.get("propagate_b", False)
         self.register_buffer("bias", torch.zeros((out_features,), dtype=self.final_dtype) if bias else None)
 
     def load_full_params(self, qweight, scales=None, zeros=None, bias=None):
-        """full-size parameters in the operator's own storage (as produced by Matmul.transform_weight of the FULL layer, row-major
-        or slab-tiled per this layer's propagate_b) -> this rank's K shard."""
+        """full-size parameters in the storage of the FULL layer (as produced by Matmul.transform_weight of an operator with
+        this layer's out_features, in_features and propagate_b: slab-tiled where that layer legalises propagate_b to the tiling,
+        row-major otherwise) -> this rank's K shard, in its own operator's storage.  The two can differ: a shard of K/world
+        columns tiles only when (K/world)*bits/8 % 512 == 0."""
         op = self.local.bitblas_matmul
-        if op.weight_tiled:
+        if slab_tiled(self._propagate_b, self.out_features, self.in_features, op.W_dtype, op.A_dtype):
             qweight = op.tile_weight(qweight, inverse=True)
         g = self.in_features if self._whole_row_groups else op.config.group_size
-        if self._whole_row_groups and scales is not None and self.world > 1:
-            # one group spanning the full K: every shard multiplies by the same per-row scale (and zero point)
-            sh = {"qweight": qweight[:, self.k_lo * op.bit // 8:self.k_hi * op.bit // 8].contiguous(), "scales": scales.contiguous()}
+        if self._whole_row_groups and self.world > 1:
+            # one group spanning the full K: every shard multiplies by the same per-row scale (and zero point), if any
+            sh = {"qweight": qweight[:, self.k_lo * op.bit // 8:self.k_hi * op.bit // 8].contiguous()}
+            if scales is not None:
+                sh["scales"] = scales.contiguous()
             if zeros is not None:
                 sh["zeros"] = zeros.contiguous()
         else:

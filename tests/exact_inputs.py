@@ -65,6 +65,18 @@ def dyadic_activations(M, K, gen, density=0.25, group=None):
     return blk.reshape(M, K)
 
 
+def sharded_activations(M, K, shards, gen, density=0.25, group=None):
+    """[M, K] activations of a row-parallel layer: dyadic_activations per K shard of K / shards columns, so every shard's row sum
+    and every group sum inside a shard is nonzero (a shard is a problem of its own, and with whole-row groups its K range is one
+    group); a row whose shard sums cancel has its last shard negated, which keeps the full row's sum nonzero as well"""
+    per = K // shards
+    assert per * shards == K
+    group = K if group is None else group
+    A = torch.cat([dyadic_activations(M, per, gen, density, min(group, per)) for _ in range(shards)], 1)
+    A[A.sum(1) == 0, K - per:] *= -1
+    return A
+
+
 def _fp8_dyadic_codes(fmt):
     """8-bit float codes whose value is a multiple of 1/8 and at most 16 in magnitude"""
     u = torch.arange(256, dtype=torch.int32)
@@ -92,9 +104,10 @@ def _auto_density(K, mode, bit, scale, zeros, qz, fmt):
 
 
 def make_exact_case(M, N, K, *, A_dtype="float16", W_dtype="uint4", out_dtype="float16", group_size=-1, mode="none", bias=False,
-                    fast_decoding=None, seed=0, A=None, density=None, propagate_b=False):
+                    fast_decoding=None, seed=0, A=None, density=None, propagate_b=False, shards=1):
     """one case in the layout of test_gpu_kernel_grid.make_case (so helpers.product_operator / run_product take it), built from
-    the exact value sets of the module docstring.  A_dtype int8: integer activations, exact as before."""
+    the exact value sets of the module docstring.  A_dtype int8: integer activations, exact as before.  shards > 1: the
+    activations of sharded_activations, so each of `shards` equal K ranges is an exact case of its own too."""
     g = torch.Generator().manual_seed(seed)
     fmt, bit = O.W_DTYPE_MAP[W_dtype]
     adt = O.TORCH_DTYPE[A_dtype]
@@ -137,7 +150,10 @@ def make_exact_case(M, N, K, *, A_dtype="float16", W_dtype="uint4", out_dtype="f
         else:
             if density is None:
                 density = _auto_density(K, mode, bit, scale, zeros, qz, fmt)
-            A = dyadic_activations(M, K, g, density, gs).to(adt)
+            if shards > 1:
+                A = sharded_activations(M, K, shards, g, density, gs).to(adt)
+            else:
+                A = dyadic_activations(M, K, g, density, gs).to(adt)
     cfg = dict(A_dtype=A_dtype, W_dtype=W_dtype, accum_dtype="int32" if A_dtype == "int8" else "float32",
                out_dtype=out_dtype, group_size=group_size, with_scaling=with_scaling, with_zeros=with_zeros,
                zeros_mode=mode if with_zeros else "original", with_bias=bias, fast_decoding=fast_decoding)

@@ -26,14 +26,24 @@ def _worker(rank, world, port, chunks, ret):
         import helpers as H
         from bitblas_b200.parallel import ColumnParallelLinear, shard_quantized_params
         M, N, K, g = 12, 64, 256, 128
-        for mode in ("original", "quantized"):
+        for mode, tiled in (("original", False), ("quantized", False), ("quantized", True)):
+            if tiled:
+                N, K = 384, 2048  # propagate_b: the full weight is slab-tiled (N % 128 == 0, 1024 bytes per row), the 192-row shard is not
             case = H.make_case(M, N, K, W_dtype="uint4", group_size=g, with_scaling=True, with_zeros=True, zeros_mode=mode,
                                with_bias=True, seed=7)
             full_ref = H.oracle_output(case)
             layer = ColumnParallelLinear(K, N, bias=True, A_dtype="float16", W_dtype="uint4", group_size=g, with_scaling=True,
-                                         with_zeros=True, zeros_mode=mode, enable_tuning=False, pipeline_chunks=chunks)
-            stored = layer.local.bitblas_matmul.weight_transform(case["fields"].to(torch.int8))
+                                         with_zeros=True, zeros_mode=mode, enable_tuning=False, pipeline_chunks=chunks, propagate_b=tiled)
+            op = layer.local.bitblas_matmul
+            assert not op.weight_tiled
+            import bitblas_b200 as bitblas
+            full_op = bitblas.Matmul(bitblas.MatmulConfig(M=M, N=N, K=K, A_dtype="float16", W_dtype="uint4", group_size=g, with_scaling=True,
+                                                          with_zeros=True, zeros_mode=mode, propagate_b=tiled), enable_tuning=False)
+            assert full_op.weight_tiled == tiled
+            stored = full_op.transform_weight(case["fields"].to(torch.int8))        # full-size, in the full layer's own storage
             layer.load_full_params(stored, case["scale"], case["zeros"], case["bias"])
+            if tiled:
+                stored = full_op.tile_weight(stored, inverse=True)
             lo, hi = layer.n_lo, layer.n_hi
             assert (lo, hi) == (rank * N // world, (rank + 1) * N // world)
             assert torch.equal(layer.local.qweight, stored[lo:hi])
@@ -79,25 +89,28 @@ def _row_worker(rank, world, port, ret):
         import bitblas_oracle as O
         import helpers as H
         from bitblas_b200.parallel import RowParallelLinear
-        M, N, K, g = 6, 64, 2048, 128
-        for mode, tiled in (("original", False), ("quantized", False), ("quantized", True)):
+        M, N, g = 6, 64, 128
+        for mode, tiled, K in (("original", False, 2048), ("quantized", False, 2048), ("quantized", True, 2048), ("quantized", True, 3072)):
             if tiled:
                 N = 128          # slab tiling needs N % 128 == 0 and (K/world)/2 % 512 == 0
+            # K = 3072: the full weight is slab-tiled (1536 bytes per row), the world-2 shard (768 bytes per row) is not
+            shard_tiled = tiled and K == 2048
             case = H.make_case(M, N, K, W_dtype="uint4", group_size=g, with_scaling=True, with_zeros=True, zeros_mode=mode, with_bias=True,
                                seed=11)
             layer = RowParallelLinear(K, N, bias=True, input_is_parallel=False, A_dtype="float16", W_dtype="uint4", group_size=g,
                                       with_scaling=True, with_zeros=True, zeros_mode=mode, enable_tuning=False, propagate_b=tiled)
             op = layer.local.bitblas_matmul
-            assert op.weight_tiled == tiled and op.config.K == K // world and op.config.out_dtype == "float32"
+            assert op.weight_tiled == shard_tiled and op.config.K == K // world and op.config.out_dtype == "float32"
             import bitblas_b200 as bitblas
             full_op = bitblas.Matmul(bitblas.MatmulConfig(M=M, N=N, K=K, A_dtype="float16", W_dtype="uint4", group_size=g, with_scaling=True,
                                                           with_zeros=True, zeros_mode=mode, propagate_b=tiled), enable_tuning=False)
+            assert full_op.weight_tiled == tiled
             stored = full_op.transform_weight(case["fields"].to(torch.int8))        # full-size, in the full layer's own storage
             layer.load_full_params(stored, case["scale"], case["zeros"], case["bias"])
             lo, hi = layer.k_lo, layer.k_hi
             assert (lo, hi) == (rank * K // world, (rank + 1) * K // world)
             # the shard decodes to exactly this rank's K range of the original fields
-            w_local = op.tile_weight(layer.local.qweight, inverse=True) if tiled else layer.local.qweight
+            w_local = op.tile_weight(layer.local.qweight, inverse=True) if shard_tiled else layer.local.qweight
             shard_fields = torch.from_numpy(O.general_decompress(O.deinterleave_weight(w_local.numpy(), 4, "float16"), 4)).to(torch.int32)
             assert torch.equal(shard_fields, case["fields"][:, lo:hi])
             sc, zz = layer.local.scales, layer.local.zeros
