@@ -60,6 +60,20 @@ EncodeTiledFn tensor_map_encoder() {
   return fn;
 }
 
+int make_map_2d(CUtensorMap* map, CUtensorMapDataType dt, const void* base, uint64_t inner, uint64_t outer,
+                uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, CUtensorMapSwizzle sw) {
+  EncodeTiledFn enc = tensor_map_encoder();
+  if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return 4; }
+  cuuint64_t dims[2] = {inner, outer};
+  cuuint64_t strides[1] = {row_stride_bytes};
+  cuuint32_t box[2] = {box_inner, box_outer};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(map, dt, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with CUresult %d", int(r)); return 4; }
+  return 0;
+}
+
 static int validate(const bb_matmul_desc* d) {
   if (!d) { set_error("null descriptor"); return 1; }
   if (d->N <= 0 || d->K <= 0) { set_error("N and K must be positive (N=%d K=%d)", d->N, d->K); return 1; }
@@ -142,8 +156,8 @@ struct PeerBarrierArgs { uint32_t* flags[BB_MAX_PEERS]; int n, rank; };
 
 __global__ void peer_barrier_kernel(const PeerBarrierArgs a) {
   __shared__ uint32_t seq_s;
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  pdl_wait();
+  pdl_launch_dependents();
   uint32_t* mine = a.flags[a.rank];
   if (threadIdx.x == 0) {
     const uint32_t seq = mine[16] + 1u;

@@ -124,6 +124,26 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn tensor_map_encoder();
+// a 2-D TMA map: `outer` rows of `inner` elements, `row_stride_bytes` apart; box = box_inner x box_outer.  Returns 0, or 4 with the
+// error set
+int make_map_2d(CUtensorMap* map, CUtensorMapDataType dt, const void* base, uint64_t inner, uint64_t outer,
+                uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, CUtensorMapSwizzle sw);
+
+// The instance ladder of the kernels built for 16-bit activations x 4- / 2-bit weights x interleaved / compressed storage:
+// f(TypeTag<T>, BITS, IL) for d's a_dtype (float16, else bfloat16), w_bits (4, else 2) and w_layout, BITS and IL as
+// std::integral_constant / std::bool_constant.
+template <typename T>
+struct TypeTag { using type = T; };
+template <typename F>
+int dispatch_t_bits_il(const bb_matmul_desc& d, F&& f) {
+  const bool il = d.w_layout == BB_LAYOUT_INTERLEAVED_16;
+  auto bits_il = [&](auto t) {
+    using std::integral_constant;
+    if (d.w_bits == 4) return il ? f(t, integral_constant<int, 4>{}, std::true_type{}) : f(t, integral_constant<int, 4>{}, std::false_type{});
+    return il ? f(t, integral_constant<int, 2>{}, std::true_type{}) : f(t, integral_constant<int, 2>{}, std::false_type{});
+  };
+  return d.a_dtype == BB_F16 ? bits_il(TypeTag<__half>{}) : bits_il(TypeTag<__nv_bfloat16>{});
+}
 
 // kernel family entry points (each returns 0 / error code; *_supported says whether the family covers it)
 bool generic_supported(const bb_matmul_desc& d);
@@ -253,6 +273,44 @@ __device__ __forceinline__ uint2 ldg_nc_v2(const void* p) {
   return r;
 }
 
+// shared memory, mbarriers and TMA: each wrapper takes 32-bit shared-memory addresses; the pointer forms convert through smem_u32
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
+}
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) { mbar_init(smem_u32(bar), count); }
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) { mbar_arrive_expect_tx(smem_u32(bar), bytes); }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) { mbar_arrive(smem_u32(bar)); }
+__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// (`map` is a const void* here: typed as const CUtensorMap*, the slab GEMV's coordinate registers are assigned differently)
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* map, int c0, int c1, uint32_t bar) {
+  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
+               "l"(map), "r"(c0), "r"(c1), "r"(bar)
+               : "memory");
+}
+__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
+  tma_load_2d(smem_u32(dst), map, c0, c1, smem_u32(bar));
+}
+__device__ __forceinline__ uint4 lds128(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+
 template <typename T>
 struct TypeTraits;
 template <>
@@ -277,6 +335,28 @@ __device__ __forceinline__ uint32_t h2_as_u32(__half2 v) { return *reinterpret_c
 __device__ __forceinline__ __half2 u32_as_h2(uint32_t v) { return *reinterpret_cast<__half2*>(&v); }
 __device__ __forceinline__ uint32_t b2_as_u32(__nv_bfloat162 v) { return *reinterpret_cast<uint32_t*>(&v); }
 __device__ __forceinline__ __nv_bfloat162 u32_as_b2(uint32_t v) { return *reinterpret_cast<__nv_bfloat162*>(&v); }
+
+// the 16-bit pattern b as a T, widened to float
+template <typename T>
+__device__ __forceinline__ float raw_to_float(uint16_t b) {
+  return TypeTraits<T>::to_float(*reinterpret_cast<const T*>(&b));
+}
+
+// c += A (16 x 16, T) * B (16 x 8, T) with fp32 accumulators
+template <typename T>
+__device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1);
+template <>
+__device__ __forceinline__ void mma_16816<__half>(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+template <>
+__device__ __forceinline__ void mma_16816<__nv_bfloat16>(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
 
 // packed 16-bit x2 arithmetic on raw registers, dispatched on element type
 template <typename T>

@@ -1,5 +1,5 @@
 // bb_gemm_ts.cuh -- the per-tile pieces of the wgmma GEMM (bb_gemm_ts.cu): PTX wrappers, shared-memory layout, the LOP3
-// decode into wgmma A fragments, per-row group parameters and the 2-D TMA map.  gemm_ts_kernel (bb_gemm_ts.cu) runs one tile per
+// decode into wgmma A fragments and per-row group parameters.  gemm_ts_kernel (bb_gemm_ts.cu) runs one tile per
 // CTA; gemm_ts_grouped_kernel (bb_grouped_gemm.cu) runs every (expert, m-tile, n-tile) tile a persistent CTA takes.  Each kernel
 // keeps its own k-loop and epilogue: sharing them as device functions changes gemm_ts_kernel's register allocation.  The
 // design notes are at the top of bb_gemm_ts.cu.
@@ -17,19 +17,8 @@ constexpr int TS_CONSUMER_WARPS = 8;       // warps 0-7: two consumer warpgroups
 constexpr int TS_THREADS = (TS_CONSUMER_WARPS + 1) * 32;   // + warp 8: TMA producer
 
 // ---------------------------------------------------------------------------------------------
-// PTX wrappers
+// PTX wrappers (the shared-memory, mbarrier and 2-D TMA ones are in bb_common.cuh)
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
       "{\n"
@@ -41,15 +30,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "WAIT_DONE:\n"
       "}\n" ::"r"(smem_u32(bar)),
       "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-          smem_u32(dst)),
-      "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
       : "memory");
 }
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, uint64_t* bar) {
@@ -145,17 +125,6 @@ struct TsSmem {
   static constexpr int kBarBytes = 256;   // full[8] + empty[8]
   static constexpr int kTotal = kStages * kStageBytes + kBarBytes + 1024;  // + alignment slack
 };
-
-__device__ __forceinline__ uint4 lds128(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
-  return v;
-}
 
 // byte t of each of four words: (w0.t, w1.t, w2.t, w3.t)
 __device__ __forceinline__ uint32_t gather_byte(uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3, uint32_t sel) {
@@ -296,21 +265,6 @@ struct RowGroup {
     if constexpr (MODE == 4) c.mz_lo = magic + ((qz_raw >> qz_shift) & ((1u << BITS) - 1u)) * 0x00010001u;
   }
 };
-
-// a 2-D TMA map: `outer` rows of `inner` elements, `row_stride_bytes` apart; box = box_inner x box_outer
-int make_map_2d(CUtensorMap* map, CUtensorMapDataType dt, const void* base, uint64_t inner, uint64_t outer,
-                uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, CUtensorMapSwizzle sw) {
-  EncodeTiledFn enc = tensor_map_encoder();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return 4; }
-  cuuint64_t dims[2] = {inner, outer};
-  cuuint64_t strides[1] = {row_stride_bytes};
-  cuuint32_t box[2] = {box_inner, box_outer};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, dt, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with CUresult %d", int(r)); return 4; }
-  return 0;
-}
 
 }  // namespace
 

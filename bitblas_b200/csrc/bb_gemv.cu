@@ -33,7 +33,7 @@ __device__ __forceinline__ void mma_16832_u8s8(int (&c)[4], const uint32_t (&a)[
 }
 
 template <typename T, int BITS, bool IL, int NT, int ZK, bool SC>
-__global__ void __launch_bounds__(NT == 1 ? 128 : MAX_KS * 32) __maxnreg__(gemv_mma_maxnreg(NT, ZK))
+__global__ void __launch_bounds__(gemv_max_ks(NT) * 32) __maxnreg__(gemv_mma_maxnreg(NT, ZK))
 gemv_mma_kernel(const GemvParams p) {
   __shared__ float red[MAX_KS][16][8 * NT];
   gemv_mma_tile<T, BITS, IL, NT, ZK, SC, true>(p, blockIdx.x, red);
@@ -45,7 +45,7 @@ gemv_mma_kernel(const GemvParams p) {
 // produced on the tensor cores with an all-ones A fragment.
 // ---------------------------------------------------------------------------------------------
 template <int BITS, int NT>
-__global__ void __launch_bounds__(NT == 1 ? 128 : MAX_KS * 32) __maxnreg__(NT == 1 ? 96 : (NT == 2 ? 128 : 208))
+__global__ void __launch_bounds__(gemv_max_ks(NT) * 32) __maxnreg__(NT == 1 ? 96 : (NT == 2 ? 128 : 208))
 gemv_i8_kernel(const GemvParams p) {
   constexpr int WPS = BITS;            // words per thread per row per step (32 k)
   constexpr int STEP_BYTES = 16 * BITS;
@@ -158,27 +158,20 @@ gemv_i8_kernel(const GemvParams p) {
 }
 
 // one CTA per 16-row block, the K split from pick_ks
-#define BB_GEMV_GO(KERNEL, MAXKS)                                                 \
-  {                                                                               \
-    static KernelCache<MAX_KS + 1> cache;                                         \
-    p.ks = pick_ks(cache, KERNEL, MAXKS, nb, p.K / 128);                          \
-    return launch_pdl(KERNEL, nb, p.ks * 32, 0, a.stream, pdl_enabled(), p);      \
-  }
+template <int NT, typename Kernel>
+int launch_gemv_kernel(Kernel kernel, KernelCache<MAX_KS + 1>& cache, GemvParams p, cudaStream_t stream) {
+  const int nb = p.N / 16;
+  p.ks = pick_ks(cache, kernel, gemv_max_ks(NT), nb, p.K / 128);
+  return launch_pdl(kernel, nb, p.ks * 32, 0, stream, pdl_enabled(), p);
+}
 
 template <typename T, int BITS, bool IL>
-int launch_mma_nt(const MatmulArgs& a, GemvParams p) {
-  const int nb = p.N / 16;
-  const int nt = (p.M + 7) / 8;
-#define BB_GEMV_NT(ZKV, SCV)                                                             \
-  if (nt <= 1) BB_GEMV_GO((gemv_mma_kernel<T, BITS, IL, 1, ZKV, SCV>), 4) \
-  else if (nt == 2) BB_GEMV_GO((gemv_mma_kernel<T, BITS, IL, 2, ZKV, SCV>), MAX_KS) \
-  else BB_GEMV_GO((gemv_mma_kernel<T, BITS, IL, 4, ZKV, SCV>), MAX_KS)
-  if (!p.with_scaling) { BB_GEMV_NT(0, false) }
-  else if (p.zmode == 0) { BB_GEMV_NT(0, true) }
-  else if (p.zmode == 1) { BB_GEMV_NT(1, true) }
-  else if (p.zmode == 2) { BB_GEMV_NT(2, true) }
-  else { BB_GEMV_NT(3, true) }
-#undef BB_GEMV_NT
+int launch_mma_nt(const MatmulArgs& a, const GemvParams& p) {
+  return gemv_mma_instance(p, p.M, [&](auto nt, auto zk, auto sc) {
+    constexpr int NT = decltype(nt)::value;
+    static KernelCache<MAX_KS + 1> cache;
+    return launch_gemv_kernel<NT>(gemv_mma_kernel<T, BITS, IL, NT, decltype(zk)::value, decltype(sc)::value>, cache, p, a.stream);
+  });
 }
 
 GemvParams make_params(const MatmulArgs& a) { return make_params(a.d, a.A, a.W, a.scale, a.zeros, a.bias, make_outspec(a), a.m); }
@@ -208,15 +201,9 @@ int launch_gemv_mma(const MatmulArgs& a) {
     return 5;
   }
   const GemvParams p = make_params(a);
-  const bool il = a.d.w_layout == BB_LAYOUT_INTERLEAVED_16;
-  const bool f16 = a.d.a_dtype == BB_F16;
-  const int bits = a.d.w_bits;
-  if (f16) {
-    if (bits == 4) return il ? launch_mma_nt<__half, 4, true>(a, p) : launch_mma_nt<__half, 4, false>(a, p);
-    return il ? launch_mma_nt<__half, 2, true>(a, p) : launch_mma_nt<__half, 2, false>(a, p);
-  }
-  if (bits == 4) return il ? launch_mma_nt<__nv_bfloat16, 4, true>(a, p) : launch_mma_nt<__nv_bfloat16, 4, false>(a, p);
-  return il ? launch_mma_nt<__nv_bfloat16, 2, true>(a, p) : launch_mma_nt<__nv_bfloat16, 2, false>(a, p);
+  return dispatch_t_bits_il(a.d, [&](auto t, auto bits, auto il) {
+    return launch_mma_nt<typename decltype(t)::type, decltype(bits)::value, decltype(il)::value>(a, p);
+  });
 }
 
 bool gemv_i8_supported(const bb_matmul_desc& d, int m) {
@@ -236,18 +223,13 @@ int launch_gemv_i8(const MatmulArgs& a) {
     set_error("gemv: A and W must be 16-byte aligned");
     return 5;
   }
-  GemvParams p = make_params(a);
-  const int nb = p.N / 16;
-  const int nt = (p.M + 7) / 8;
-  if (a.d.w_bits == 2) {
-    if (nt <= 1) BB_GEMV_GO((gemv_i8_kernel<2, 1>), 4)
-    else if (nt == 2) BB_GEMV_GO((gemv_i8_kernel<2, 2>), MAX_KS)
-    else BB_GEMV_GO((gemv_i8_kernel<2, 4>), MAX_KS)
-  } else {
-    if (nt <= 1) BB_GEMV_GO((gemv_i8_kernel<4, 1>), 4)
-    else if (nt == 2) BB_GEMV_GO((gemv_i8_kernel<4, 2>), MAX_KS)
-    else BB_GEMV_GO((gemv_i8_kernel<4, 4>), MAX_KS)
-  }
+  const GemvParams p = make_params(a);
+  return gemv_nt(p.M, [&](auto nt) {
+    constexpr int NT = decltype(nt)::value;
+    static KernelCache<MAX_KS + 1> cache2, cache4;
+    return a.d.w_bits == 2 ? launch_gemv_kernel<NT>(gemv_i8_kernel<2, NT>, cache2, p, a.stream)
+                           : launch_gemv_kernel<NT>(gemv_i8_kernel<4, NT>, cache4, p, a.stream);
+  });
 }
 
 }  // namespace bb

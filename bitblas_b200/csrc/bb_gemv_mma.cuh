@@ -62,26 +62,6 @@ int pick_ks(KernelCache<MAX_KS + 1>& cache, Kernel kernel, int max_ks, int ctas,
   return full;
 }
 
-template <typename T>
-__device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1);
-template <>
-__device__ __forceinline__ void mma_16816<__half>(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-template <>
-__device__ __forceinline__ void mma_16816<__nv_bfloat16>(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-template <typename T>
-__device__ __forceinline__ float raw_to_float(uint16_t b) {
-  return TypeTraits<T>::to_float(*reinterpret_cast<const T*>(&b));
-}
-
 // Programmatic dependent launch (PDL).  A decode step is a chain of dependent GEMVs (qkv -> o -> gate_up -> down); the
 // weights, scales and zeros of the next one do not depend on the previous result, only its activations do.  Each streaming
 // kernel therefore (1) lets the next kernel in the stream start once every CTA of its own has finished its weight stream
@@ -114,6 +94,28 @@ __device__ __forceinline__ void split_range(int total, int parts, int idx, int& 
 // register budget of one gemv_mma instance (NT batch tiles of 8 rows; "original" / "rescale" zeros carry more per-group state)
 constexpr int gemv_mma_maxnreg(int nt, int zk) {
   return nt == 1 ? ((zk == 1 || zk == 2) ? 112 : 96) : (nt == 2 ? ((zk == 1 || zk == 2) ? 168 : 128) : ((zk == 1 || zk == 2) ? 232 : 192));
+}
+// most warps per CTA (K splits) of an instance with NT batch tiles: one batch tile splits K over at most 4 warps
+constexpr int gemv_max_ks(int nt) { return nt == 1 ? 4 : MAX_KS; }
+
+// The instance ladder of the streaming GEMV kernels.  gemv_nt: f(NT) with NT = 1, 2 or 4 batch tiles of 8 rows for `rows` rows of
+// A.  gemv_mma_instance: f(NT, ZK, SC) with (ZK, SC) from p's scale / zero-point mode.  All as std::integral_constant tags.
+template <typename F>
+int gemv_nt(int rows, F&& f) {
+  if (rows <= 8) return f(std::integral_constant<int, 1>{});
+  if (rows <= 16) return f(std::integral_constant<int, 2>{});
+  return f(std::integral_constant<int, 4>{});
+}
+template <typename F>
+int gemv_mma_instance(const GemvParams& p, int rows, F&& f) {
+  return gemv_nt(rows, [&](auto nt) {
+    using std::integral_constant;
+    if (!p.with_scaling) return f(nt, integral_constant<int, 0>{}, std::false_type{});
+    if (p.zmode == 0) return f(nt, integral_constant<int, 0>{}, std::true_type{});
+    if (p.zmode == 1) return f(nt, integral_constant<int, 1>{}, std::true_type{});
+    if (p.zmode == 2) return f(nt, integral_constant<int, 2>{}, std::true_type{});
+    return f(nt, integral_constant<int, 3>{}, std::true_type{});
+  });
 }
 
 // ---------------------------------------------------------------------------------------------

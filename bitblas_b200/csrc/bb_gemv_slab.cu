@@ -95,18 +95,9 @@ struct SlabParams {
   int fast_params;  // group size 128, 8-aligned group count, N % 32 == 0, aligned pointers: 16-byte async copies of the parameters
 };
 
-__device__ __forceinline__ uint32_t gs_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void gs_mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void gs_mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
+// the PTX wrappers only this kernel uses (the shared ones are in bb_common.cuh)
 __device__ __forceinline__ void gs_mbar_expect_tx_only(uint32_t bar, uint32_t bytes) {   // no arrival
   asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void gs_mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void gs_mbar_wait(uint32_t bar, uint32_t parity) {
   asm volatile(
@@ -121,28 +112,15 @@ __device__ __forceinline__ void gs_mbar_wait(uint32_t bar, uint32_t parity) {
 }
 // (No nanosleep back-off between the helper warps' barrier probes: the schedulers are not short of issue slots, the consumer warps
 //  are bound by their own dependent-instruction latency.)
-__device__ __forceinline__ void gs_tma_2d(uint32_t dst, const void* map, int c0, int c1, uint32_t bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
-               "l"(map), "r"(c0), "r"(c1), "r"(bar)
-               : "memory");
-}
 __device__ __forceinline__ void gs_bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src),
                "r"(bytes), "r"(bar)
                : "memory");
 }
-__device__ __forceinline__ uint4 gs_lds128(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-  return v;
-}
 __device__ __forceinline__ float2 gs_lds64f(uint32_t addr) {
   float2 v;
   asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
   return v;
-}
-__device__ __forceinline__ void gs_cp_async16(uint32_t dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
 // the mbarrier receives one arrival from this thread when all its cp.async issued so far have landed
 __device__ __forceinline__ void gs_cp_async_arrive_noinc(uint32_t bar) {
@@ -153,11 +131,6 @@ __device__ __forceinline__ uint32_t gs_lds8(uint32_t addr) {
   asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
   return v;
 }
-__device__ __forceinline__ uint32_t gs_lds32(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
-  return v;
-}
 __device__ __forceinline__ void gs_sts64f(uint32_t addr, float a, float b) {
   asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
@@ -166,27 +139,6 @@ __device__ __forceinline__ float gs_lds32f(uint32_t addr) {
   float v;
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
   return v;
-}
-
-template <typename T>
-__device__ __forceinline__ void gs_mma(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1);
-template <>
-__device__ __forceinline__ void gs_mma<__half>(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-template <>
-__device__ __forceinline__ void gs_mma<__nv_bfloat16>(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-template <typename T>
-__device__ __forceinline__ float gs_raw_to_float(uint32_t b) {
-  const uint16_t h = uint16_t(b);
-  return TypeTraits<T>::to_float(*reinterpret_cast<const T*>(&h));
 }
 
 template <typename T>
@@ -219,7 +171,7 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
   constexpr int NG = GS_NG, NF = GS_NF, S = GS_STAGES;
   constexpr int NCW = GS_GW * NG;            // consumer warps
   extern __shared__ uint8_t gs_raw[];
-  const uint32_t base = (gs_smem_u32(gs_raw) + 1023u) & ~1023u;
+  const uint32_t base = (smem_u32(gs_raw) + 1023u) & ~1023u;
   const uint32_t Wb = base;                                   // [S][32 rows][512 B]
   const uint32_t Ab = Wb + uint32_t(S) * GS_WBYTES;           // [S][1024 halves]
   const uint32_t Pb = Ab + uint32_t(S) * GS_ABYTES;           // [S][8 steps][32 rows] (c1, c2)
@@ -232,15 +184,15 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
-      gs_mbar_init(Bb + 8u * s, 1);             // wfull: the weight box and the activation slab have landed (issuer arrival + transaction bytes)
-      gs_mbar_init(Bb + 8u * (S + s), 1);       // pfull: the finisher has written the unit's sums and (c1, c2) pairs
-      gs_mbar_init(Bb + 8u * (2 * S + s), 32);  // praw: the 32 issuer lanes' parameter copies landed
-      gs_mbar_init(Bb + 8u * (3 * S + s), GS_GW);   // empty: the four warps of the group that consumed the unit
+      mbar_init(Bb + 8u * s, 1);             // wfull: the weight box and the activation slab have landed (issuer arrival + transaction bytes)
+      mbar_init(Bb + 8u * (S + s), 1);       // pfull: the finisher has written the unit's sums and (c1, c2) pairs
+      mbar_init(Bb + 8u * (2 * S + s), 32);  // praw: the 32 issuer lanes' parameter copies landed
+      mbar_init(Bb + 8u * (3 * S + s), GS_GW);   // empty: the four warps of the group that consumed the unit
     }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_barrier_init();
   }
   __syncthreads();
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  pdl_launch_dependents();
 
   const int R = gridDim.x;
   const int ri = R - 1 - int(blockIdx.x);   // ranges in reverse CTA order: an owner waits only for CTAs dispatched before it
@@ -270,20 +222,20 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
     // never stored / consumed; the transaction count is always the full box), the activation slab, the raw parameters
     auto unit_w = [&](int rb, int ku, int slot) {   // lane 0
       if (p.Wt) gs_bulk_g2s(Wb + uint32_t(slot) * GS_WBYTES, p.Wt + (size_t(rb) * UPR + ku) * GS_WBYTES, GS_WBYTES, Bb + 8u * slot);
-      else gs_tma_2d(Wb + uint32_t(slot) * GS_WBYTES, &tmW, ku * (GS_ROW_BYTES / 4), rb * GS_ROWS, Bb + 8u * slot);
+      else tma_load_2d(Wb + uint32_t(slot) * GS_WBYTES, &tmW, ku * (GS_ROW_BYTES / 4), rb * GS_ROWS, Bb + 8u * slot);
     };
     auto unit_params = [&](int rb, int ku, int slot) {   // all 32 lanes: lane = row of the unit
       const uint32_t bar = Bb + 8u * (2 * S + slot);
       if (unit_fast(rb, ku)) {
         const uint32_t raw = RAWb + uint32_t(slot) * GS_RAWBYTES;
         const size_t off = size_t(rb * GS_ROWS + lane) * p.G + ku * GS_STEPS;   // g = 128: group index = step index
-        if (p.with_scaling) gs_cp_async16(raw + uint32_t(lane) * 16u, scale16 + off);
-        if (p.zmode == 1 || p.zmode == 2) gs_cp_async16(raw + 512u + uint32_t(lane) * 16u, zeros16 + off);
+        if (p.with_scaling) cp_async16(raw + uint32_t(lane) * 16u, scale16 + off);
+        if (p.zmode == 1 || p.zmode == 2) cp_async16(raw + 512u + uint32_t(lane) * 16u, zeros16 + off);
         else if (p.zmode == 3 && lane < GS_STEPS)
-          gs_cp_async16(raw + 512u + uint32_t(lane) * 16u, zeros8 + size_t(ku * GS_STEPS + lane) * (p.N >> 1) + rb * (GS_ROWS / 2));
+          cp_async16(raw + 512u + uint32_t(lane) * 16u, zeros8 + size_t(ku * GS_STEPS + lane) * (p.N >> 1) + rb * (GS_ROWS / 2));
         gs_cp_async_arrive_noinc(bar);
       } else {
-        gs_mbar_arrive(bar);   // slow path: the finisher loads the parameters itself
+        mbar_arrive(bar);   // slow path: the finisher loads the parameters itself
       }
     };
     // weights and group parameters do not depend on the preceding kernel: request the first ring-full before waiting for it
@@ -304,7 +256,7 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
         next_unit(qq, kk, gg);
       }
     }
-    asm volatile("griddepcontrol.wait;" ::: "memory");   // the activations depend on the preceding kernel
+    pdl_wait();   // the activations depend on the preceding kernel
     int slot = 0, qq = q0, ku = ku0, gg = g0;
     uint32_t ephase = 1u;   // parity trick: the first pass over the ring finds every slot free
 #pragma unroll 1
@@ -317,7 +269,7 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
         // (the weight bytes of the first ring-full were registered with the pre-wait request; the padding units past the last
         //  row block -- they exist when NRB % NG != 0 -- carry no weights)
         const bool w_now = i >= npre && rb < p.NRB;
-        gs_mbar_expect_tx(Bb + 8u * slot, abytes + (w_now ? uint32_t(GS_WBYTES) : 0u));
+        mbar_arrive_expect_tx(Bb + 8u * slot, abytes + (w_now ? uint32_t(GS_WBYTES) : 0u));
         if (w_now) unit_w(rb, ku, slot);
         gs_bulk_g2s(Ab + uint32_t(slot) * GS_ABYTES, reinterpret_cast<const uint8_t*>(p.A) + size_t(k0) * 2, abytes, Bb + 8u * slot);
       }
@@ -327,7 +279,7 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
     }
     return;
   }
-  asm volatile("griddepcontrol.wait;" ::: "memory");   // (our stores and workspace traffic must follow the preceding kernel)
+  pdl_wait();   // (our stores and workspace traffic must follow the preceding kernel)
 
   if (warp > NCW) {
     // =========================== finisher warp f: units i = f, f + NF, ... of the range ===========================
@@ -363,14 +315,14 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
 #pragma unroll
       for (int ms = 0; ms < 8; ++ms) {
         const uint32_t a = abase + uint32_t(g8 * 128 + ((ms + g8) & 7) * 16 + 2 * t4) * 2u;
-        bf[ms][0] = gs_lds32(a);
-        bf[ms][1] = gs_lds32(a + 16u);
+        bf[ms][0] = lds32(a);
+        bf[ms][1] = lds32(a + 16u);
       }
       float c0[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
       for (int ms = 0; ms < 4; ++ms) {
-        gs_mma<T>(c0, sfrag, bf[ms][0], bf[ms][1]);
-        gs_mma<T>(c1, sfrag, bf[ms + 4][0], bf[ms + 4][1]);
+        mma_16816<T>(c0, sfrag, bf[ms][0], bf[ms][1]);
+        mma_16816<T>(c1, sfrag, bf[ms + 4][0], bf[ms + 4][1]);
       }
       if (g8 < 2) {   // row 0: S -> .y, row 1: SM -> .x
         const uint32_t d = Sb + uint32_t(slot) * GS_SBYTES + uint32_t(2 * t4) * 8u + (g8 == 0 ? 4u : 0u);
@@ -382,7 +334,7 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
       uint32_t sc[8], zc[8];   // raw 16-bit scales; raw fp16 zeros or (quantized) the byte holding this row's zero point
       if (unit_fast(rb, ku)) {
         const uint32_t raw = RAWb + uint32_t(slot) * GS_RAWBYTES;
-        const uint4 s4 = gs_lds128(raw + uint32_t(lane) * 16u);
+        const uint4 s4 = lds128(raw + uint32_t(lane) * 16u);
         const uint32_t sw[4] = {s4.x, s4.y, s4.z, s4.w};
 #pragma unroll
         for (int st = 0; st < 8; ++st) sc[st] = (st & 1) ? (sw[st >> 1] >> 16) : (sw[st >> 1] & 0xffffu);
@@ -390,7 +342,7 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
 #pragma unroll
           for (int st = 0; st < 8; ++st) zc[st] = gs_lds8(raw + 512u + uint32_t(st) * 16u + uint32_t(lane >> 1));
         } else {
-          const uint4 z4 = gs_lds128(raw + 512u + uint32_t(lane) * 16u);
+          const uint4 z4 = lds128(raw + 512u + uint32_t(lane) * 16u);
           const uint32_t zw[4] = {z4.x, z4.y, z4.z, z4.w};
 #pragma unroll
           for (int st = 0; st < 8; ++st) zc[st] = (st & 1) ? (zw[st >> 1] >> 16) : (zw[st >> 1] & 0xffffu);
@@ -418,11 +370,11 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
         constexpr bool SC = decltype(sc_tag)::value;
 #pragma unroll
         for (int st = 0; st < 8; ++st) {
-          const float c1 = SC ? gs_raw_to_float<T>(sc[st]) : 1.f;
+          const float c1 = SC ? raw_to_float<T>(sc[st]) : 1.f;
           float c2;
           if constexpr (ZM == 0) c2 = -c1 * float(p.zp_const);
-          else if constexpr (ZM == 1) c2 = -c1 * gs_raw_to_float<T>(zc[st]);
-          else if constexpr (ZM == 2) c2 = -gs_raw_to_float<T>(zc[st]);
+          else if constexpr (ZM == 1) c2 = -c1 * raw_to_float<T>(zc[st]);
+          else if constexpr (ZM == 2) c2 = -raw_to_float<T>(zc[st]);
           else c2 = -c1 * float((zc[st] >> zsh) & 15u);
           gs_sts64f(pbase + uint32_t(st) * (GS_ROWS * 8u), c1, c2);
         }
@@ -434,7 +386,7 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
       else if (p.zmode == 2) body(integral_constant<int, 2>{}, std::true_type{});
       else body(integral_constant<int, 3>{}, std::true_type{});
       __syncwarp();
-      if (lane == 0) gs_mbar_arrive(Bb + 8u * (S + slot));
+      if (lane == 0) mbar_arrive(Bb + 8u * (S + slot));
       slot += NF;                       // S % NF == 0: the slot sequence of this warp closes on itself
       if (slot >= S) { slot -= S; phase ^= 1u; }
       gg += NF; rb += NF;               // t -> t + NF
@@ -493,12 +445,12 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
       const uint32_t wst = Wb + uint32_t(slot) * GS_WBYTES + woff;
       uint4 wv[8];
 #pragma unroll
-      for (int x = 0; x < 8; ++x) wv[x] = gs_lds128(wst + uint32_t(x) * (4u * GS_ROW_BYTES));
+      for (int x = 0; x < 8; ++x) wv[x] = lds128(wst + uint32_t(x) * (4u * GS_ROW_BYTES));
       if (lane < 8) {   // one divergent region per unit
         const uint32_t ast = Ab + uint32_t(slot) * GS_ABYTES + aoff;
 #pragma unroll
         for (int x = 0; x < 4; ++x) {
-          const uint4 v = gs_lds128(ast + uint32_t(x) * 16u);
+          const uint4 v = lds128(ast + uint32_t(x) * 16u);
           Rv[x][0] = v.x; Rv[x][1] = v.y; Rv[x][2] = v.z; Rv[x][3] = v.w;
         }
       }
@@ -532,7 +484,7 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
             b0 = __byte_perm(Rv[wi][jj], Rv[wi][jj + 2], 0x5410);
             b1 = __byte_perm(Rv[wi][jj], Rv[wi][jj + 2], 0x7632);
           }
-          gs_mma<T>(c, af, b0, b1);
+          mma_16816<T>(c, af, b0, b1);
         }
       };
 #pragma unroll
@@ -571,7 +523,7 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
       }
     }
     __syncwarp();
-    if (lane == 0) gs_mbar_arrive(Bb + 8u * (3 * S + slot));
+    if (lane == 0) mbar_arrive(Bb + 8u * (3 * S + slot));
 
     if (closes || i + NG >= n_units) {
       // ---- end of this range's segment of row block rb: group reduction over 4 K-slices x 2 k-halves, then store / park / collect ----
@@ -648,16 +600,10 @@ bool get_w_map(CUtensorMap* tm, const void* W, int N, int K) {
   ++g_map_clock;
   for (int i = 0; i < g_map_count; ++i)
     if (g_maps[i].W == W && g_maps[i].N == N && g_maps[i].K == K) { g_maps[i].stamp = g_map_clock; *tm = g_maps[i].map; return true; }
-  EncodeTiledFn enc = tensor_map_encoder();
-  if (!enc) return false;
   CUtensorMap m;
-  const cuuint64_t Kb = cuuint64_t(K) / 2;
-  cuuint64_t dims[2] = {Kb / 4, cuuint64_t(N)};
-  cuuint64_t strides[1] = {Kb};
-  cuuint32_t box[2] = {GS_ROW_BYTES / 4, GS_ROWS};
-  cuuint32_t estr[2] = {1, 1};
-  if (enc(&m, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, const_cast<void*>(W), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-          CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+  const uint64_t Kb = uint64_t(K) / 2;
+  if (make_map_2d(&m, CU_TENSOR_MAP_DATA_TYPE_UINT32, W, Kb / 4, uint64_t(N), Kb, GS_ROW_BYTES / 4, GS_ROWS,
+                  CU_TENSOR_MAP_SWIZZLE_NONE))
     return false;
   int idx = g_map_count;
   if (g_map_count < GS_MAP_CACHE) ++g_map_count;

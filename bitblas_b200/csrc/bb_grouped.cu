@@ -40,7 +40,7 @@ struct GroupedParams {
 };
 
 template <typename T, int BITS, bool IL, int NT, int ZK, bool SC, bool SWIGLU = false>
-__global__ void __launch_bounds__(NT == 1 ? 128 : MAX_KS * 32) __maxnreg__(gemv_mma_maxnreg(NT, ZK))
+__global__ void __launch_bounds__(gemv_max_ks(NT) * 32) __maxnreg__(gemv_mma_maxnreg(NT, ZK))
 gemv_grouped_kernel(const GroupedParams g) {
   constexpr int R = 8 * NT;   // rows of A per pass over a 16-row block of W
   __shared__ float red[MAX_KS][16][8 * NT];
@@ -87,38 +87,23 @@ int launch_grouped_kernel(KernelT kernel, KernelCache<MAX_KS + 1>& cache, Groupe
 }
 
 template <typename T, int BITS, bool IL, bool SWIGLU>
-int launch_grouped_nt(const GroupedParams& g, int nt, const int (&max_items)[3], cudaStream_t s) {
-#define BB_GROUPED_GO(NTV, ZKV, SCV, MAXKS)                                                                   \
-  {                                                                                                          \
-    static KernelCache<MAX_KS + 1> cache;                                                                    \
-    return launch_grouped_kernel(gemv_grouped_kernel<T, BITS, IL, NTV, ZKV, SCV, SWIGLU>, cache, g,         \
-                                 max_items[NTV == 1 ? 0 : (NTV == 2 ? 1 : 2)], MAXKS, s);                    \
-  }
-#define BB_GROUPED_NT(ZKV, SCV)                     \
-  if (nt == 1) BB_GROUPED_GO(1, ZKV, SCV, 4)        \
-  if (nt == 2) BB_GROUPED_GO(2, ZKV, SCV, MAX_KS)   \
-  BB_GROUPED_GO(4, ZKV, SCV, MAX_KS)
-  if (!g.p.with_scaling) { BB_GROUPED_NT(0, false) }
-  if (g.p.zmode == 0) { BB_GROUPED_NT(0, true) }
-  if (g.p.zmode == 1) { BB_GROUPED_NT(1, true) }
-  if (g.p.zmode == 2) { BB_GROUPED_NT(2, true) }
-  BB_GROUPED_NT(3, true)
-#undef BB_GROUPED_NT
-#undef BB_GROUPED_GO
+int launch_grouped_nt(const GroupedParams& g, int rows, const int (&max_items)[3], cudaStream_t s) {
+  return gemv_mma_instance(g.p, rows, [&](auto nt, auto zk, auto sc) {
+    constexpr int NT = decltype(nt)::value;
+    static KernelCache<MAX_KS + 1> cache;
+    return launch_grouped_kernel(gemv_grouped_kernel<T, BITS, IL, NT, decltype(zk)::value, decltype(sc)::value, SWIGLU>, cache, g,
+                                 max_items[NT == 1 ? 0 : (NT == 2 ? 1 : 2)], gemv_max_ks(NT), s);
+  });
 }
 
 size_t elem_bytes(int dtype) { return dtype == BB_F32 ? 4 : 2; }
 
 template <bool SWIGLU>
-int launch_grouped_typed(const bb_matmul_desc& d, bool il, const GroupedParams& g, int nt, const int (&max_items)[3], cudaStream_t s) {
-  if (d.a_dtype == BB_F16) {
-    if (d.w_bits == 4) return il ? launch_grouped_nt<__half, 4, true, SWIGLU>(g, nt, max_items, s) : launch_grouped_nt<__half, 4, false, SWIGLU>(g, nt, max_items, s);
-    return il ? launch_grouped_nt<__half, 2, true, SWIGLU>(g, nt, max_items, s) : launch_grouped_nt<__half, 2, false, SWIGLU>(g, nt, max_items, s);
-  }
-  if (d.w_bits == 4) return il ? launch_grouped_nt<__nv_bfloat16, 4, true, SWIGLU>(g, nt, max_items, s) : launch_grouped_nt<__nv_bfloat16, 4, false, SWIGLU>(g, nt, max_items, s);
-  return il ? launch_grouped_nt<__nv_bfloat16, 2, true, SWIGLU>(g, nt, max_items, s) : launch_grouped_nt<__nv_bfloat16, 2, false, SWIGLU>(g, nt, max_items, s);
+int launch_grouped_typed(const bb_matmul_desc& d, const GroupedParams& g, int rows, const int (&max_items)[3], cudaStream_t s) {
+  return dispatch_t_bits_il(d, [&](auto t, auto bits, auto il) {
+    return launch_grouped_nt<typename decltype(t)::type, decltype(bits)::value, decltype(il)::value, SWIGLU>(g, rows, max_items, s);
+  });
 }
-
 
 }  // namespace
 
@@ -149,11 +134,10 @@ int launch_grouped(const GroupedArgs& a) {
   g.offsets = a.offsets; g.E = a.num_groups; g.T = a.total_rows;
   g.w_stride = a.w_stride; g.s_stride = a.s_stride; g.z_stride = a.z_stride; g.b_stride = a.b_stride;
   g.out_bytes = int(elem_bytes(d.out_dtype));
-  // rows per pass: 8, 16 or 32, from the mean rows per active group (T rows over at most min(E, T) groups)
+  // rows per pass: 8, 16 or 32 (gemv_nt), from the mean rows per active group (T rows over at most min(E, T) groups)
   const int total_rows = a.total_rows;
   const int active = std::min(a.num_groups, total_rows);
   const int mean_rows = (total_rows + active - 1) / active;
-  const int nt = mean_rows <= 8 ? 1 : (mean_rows <= 16 ? 2 : 4);
   // work items: sum_e ceil(m_e / R) row chunks per 16-row block <= T / R + (groups with rows)
   const long long nb = d.N / 16;
   int max_items[3];
@@ -163,9 +147,8 @@ int launch_grouped(const GroupedArgs& a) {
     if (items > INT_MAX) { set_error("grouped matmul: N/16 x (T/rows + groups) exceeds 2^31 work items"); return 1; }
     max_items[i] = int(items);
   }
-  const bool il = d.w_layout == BB_LAYOUT_INTERLEAVED_16;
-  return a.swiglu ? launch_grouped_typed<true>(d, il, g, nt, max_items, a.stream)
-                  : launch_grouped_typed<false>(d, il, g, nt, max_items, a.stream);
+  return a.swiglu ? launch_grouped_typed<true>(d, g, mean_rows, max_items, a.stream)
+                  : launch_grouped_typed<false>(d, g, mean_rows, max_items, a.stream);
 }
 
 }  // namespace bb

@@ -52,9 +52,6 @@ struct GroupedTsParams {
   int a_rows;
 };
 
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
 // the mbarrier's phase also waits for this thread's earlier cp.async copies (net-zero on its pending count)
 __device__ __forceinline__ void cp_async_mbar_arrive(uint64_t* bar) {
   asm volatile("cp.async.mbarrier.arrive.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -367,14 +364,10 @@ int launch_grouped_gemm_bm(const GroupedTsParams& g, const void* A, const void* 
 }
 
 template <bool SWIGLU, bool GATHER = false>
-int launch_grouped_gemm_typed(const bb_matmul_desc& d, bool il, const GroupedTsParams& g, const void* A, const void* W,
-                              cudaStream_t s) {
-  if (d.a_dtype == BB_F16) {
-    if (d.w_bits == 4) return il ? launch_grouped_gemm_bm<__half, 4, true, SWIGLU, GATHER>(g, A, W, s) : launch_grouped_gemm_bm<__half, 4, false, SWIGLU, GATHER>(g, A, W, s);
-    return il ? launch_grouped_gemm_bm<__half, 2, true, SWIGLU, GATHER>(g, A, W, s) : launch_grouped_gemm_bm<__half, 2, false, SWIGLU, GATHER>(g, A, W, s);
-  }
-  if (d.w_bits == 4) return il ? launch_grouped_gemm_bm<__nv_bfloat16, 4, true, SWIGLU, GATHER>(g, A, W, s) : launch_grouped_gemm_bm<__nv_bfloat16, 4, false, SWIGLU, GATHER>(g, A, W, s);
-  return il ? launch_grouped_gemm_bm<__nv_bfloat16, 2, true, SWIGLU, GATHER>(g, A, W, s) : launch_grouped_gemm_bm<__nv_bfloat16, 2, false, SWIGLU, GATHER>(g, A, W, s);
+int launch_grouped_gemm_typed(const bb_matmul_desc& d, const GroupedTsParams& g, const void* A, const void* W, cudaStream_t s) {
+  return dispatch_t_bits_il(d, [&](auto t, auto bits, auto il) {
+    return launch_grouped_gemm_bm<typename decltype(t)::type, decltype(bits)::value, decltype(il)::value, SWIGLU, GATHER>(g, A, W, s);
+  });
 }
 
 }  // namespace
@@ -401,10 +394,9 @@ int launch_grouped_gemm(const GroupedArgs& a) {
     set_error("grouped GEMM: N/128 x (T/32 + groups) exceeds 2^31 tiles");
     return 1;
   }
-  const bool il = d.w_layout == BB_LAYOUT_INTERLEAVED_16;
-  if (a.row_index) return launch_grouped_gemm_typed<true, true>(d, il, g, a.A, a.W, a.stream);
-  return a.swiglu ? launch_grouped_gemm_typed<true>(d, il, g, a.A, a.W, a.stream)
-                  : launch_grouped_gemm_typed<false>(d, il, g, a.A, a.W, a.stream);
+  if (a.row_index) return launch_grouped_gemm_typed<true, true>(d, g, a.A, a.W, a.stream);
+  return a.swiglu ? launch_grouped_gemm_typed<true>(d, g, a.A, a.W, a.stream)
+                  : launch_grouped_gemm_typed<false>(d, g, a.A, a.W, a.stream);
 }
 
 }  // namespace bb

@@ -36,11 +36,6 @@ struct PermuteParams {
   int T, K, E, R;             // rows, columns, groups, rows per tile
 };
 
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-  const uint32_t s = static_cast<uint32_t>(__cvta_generic_to_shared(smem));
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(s), "l"(gmem) : "memory");
-}
-
 __global__ void __launch_bounds__(PERMUTE_THREADS) permute_cols_kernel(const PermuteParams p) {
   extern __shared__ __align__(16) uint16_t tile_s[];   // [R, K]
   __shared__ int row0_s[BB_GROUPED_MAX_GROUPS], rows_s[BB_GROUPED_MAX_GROUPS], item0_s[BB_GROUPED_MAX_GROUPS + 1];
@@ -67,7 +62,7 @@ __global__ void __launch_bounds__(PERMUTE_THREADS) permute_cols_kernel(const Per
     }
     const uint4* src = reinterpret_cast<const uint4*>(p.A + size_t(r0) * p.K);
     uint4* tile4 = reinterpret_cast<uint4*>(tile_s);
-    for (int v = tid; v < n * vecs; v += PERMUTE_THREADS) cp_async16(tile4 + v, src + v);
+    for (int v = tid; v < n * vecs; v += PERMUTE_THREADS) cp_async16(smem_u32(tile4 + v), src + v);
     asm volatile("cp.async.wait_all;" ::: "memory");
     __syncthreads();
     const int32_t* pe = p.perm + size_t(e) * p.K;
