@@ -35,7 +35,7 @@ EXPORTS = [
     "bb_init", "bb_matmul", "bb_matmul_scatter", "bb_matmul_grouped", "bb_matmul_grouped_gemm", "bb_matmul_grouped_swiglu",
     "bb_matmul_grouped_gemm_swiglu", "bb_matmul_grouped_gemm_swiglu_gather", "bb_moe_route", "bb_moe_route_index",
     "bb_moe_combine", "bb_moe_topk", "bb_permute_cols", "bb_peer_barrier", "bb_workspace_bytes", "bb_select_kernel", "bb_kernel_name", "bb_set_kernel_override",
-    "bb_launch_count", "bb_last_error", "bb_version", "bb_compress_host", "bb_interleave_host",
+    "bb_set_sm_count_cap", "bb_launch_count", "bb_last_error", "bb_version", "bb_compress_host", "bb_interleave_host",
     "bb_transform_weight_device", "bb_repack_gptq_qweight_device", "bb_repack_gptq_qzeros_device",
     "bb_retile_weight_device", "bb_debug_decode", "bb_debug_dequant",
 ]
@@ -52,7 +52,7 @@ class MatmulDesc(ctypes.Structure):
 
 
 _lib = None
-OVERRIDE_GEN = 0   # bumped by every bb_set_kernel_override call (testing hook)
+OVERRIDE_GEN = 0   # bumped by every bb_set_kernel_override and bb_set_sm_count_cap call (testing hooks)
 
 
 def load() -> ctypes.CDLL:
@@ -86,14 +86,16 @@ def load() -> ctypes.CDLL:
     lib.bb_workspace_bytes.argtypes = [dp, i32]; lib.bb_workspace_bytes.restype = sz
     lib.bb_select_kernel.argtypes = [dp, i32]; lib.bb_select_kernel.restype = i32
     lib.bb_kernel_name.argtypes = [i32]; lib.bb_kernel_name.restype = ctypes.c_char_p
-    lib.bb_set_kernel_override.argtypes = [i32]; lib.bb_set_kernel_override.restype = i32
-    _c_override = lib.bb_set_kernel_override
+    def _bumps_generation(c_fn):   # operators cache bb_workspace_bytes per (m, override generation); both hooks change it
+        c_fn.argtypes = [i32]; c_fn.restype = i32
 
-    def _set_override(kernel_id):   # operators cache bb_workspace_bytes per (m, override generation)
-        global OVERRIDE_GEN
-        OVERRIDE_GEN += 1
-        return _c_override(int(kernel_id))
-    lib.bb_set_kernel_override = _set_override
+        def call(value):
+            global OVERRIDE_GEN
+            OVERRIDE_GEN += 1
+            return c_fn(int(value))
+        return call
+    lib.bb_set_kernel_override = _bumps_generation(lib.bb_set_kernel_override)
+    lib.bb_set_sm_count_cap = _bumps_generation(lib.bb_set_sm_count_cap)
     lib.bb_launch_count.argtypes = []; lib.bb_launch_count.restype = ctypes.c_uint64
     lib.bb_last_error.argtypes = []; lib.bb_last_error.restype = ctypes.c_char_p
     lib.bb_version.argtypes = []; lib.bb_version.restype = i32

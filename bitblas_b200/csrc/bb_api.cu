@@ -21,6 +21,7 @@ static thread_local char g_err[512] = "";
 std::atomic<uint64_t> g_launches{0};
 static std::atomic<int> g_override{BB_KERNEL_AUTO};
 static std::atomic<int> g_sm_count[BB_MAX_DEVICES];   // 0 = not queried yet; per-device state is keyed on the ordinal
+static std::atomic<int> g_sm_cap{0};                  // bb_set_sm_count_cap; 0 = no cap
 
 void set_error(const char* fmt, ...) {
   va_list ap;
@@ -35,7 +36,7 @@ int current_device() {
   return (dev < 0 || dev >= BB_MAX_DEVICES) ? 0 : dev;
 }
 
-int device_sm_count() {
+int device_sm_count_uncapped() {
   const int dev = current_device();
   int n = g_sm_count[dev].load(std::memory_order_relaxed);
   if (n == 0) {
@@ -43,6 +44,12 @@ int device_sm_count() {
     g_sm_count[dev].store(n, std::memory_order_relaxed);
   }
   return n;
+}
+
+int device_sm_count() {
+  const int n = device_sm_count_uncapped();
+  const int cap = g_sm_cap.load(std::memory_order_relaxed);
+  return cap > 0 && cap < n ? cap : n;
 }
 
 bool pdl_enabled() {
@@ -231,6 +238,17 @@ const char* bb_kernel_name(int id) {
 }
 
 int bb_set_kernel_override(int id) { return g_override.exchange(id); }
+
+int bb_set_sm_count_cap(int cap) {
+  // a cap above the real count would launch grids larger than what is resident at once, and the slab kernel's collectors spin on
+  // slots written by other CTAs of their own grid
+  const int n = device_sm_count_uncapped();
+  if (cap < 0 || cap > n) {
+    set_error("bb_set_sm_count_cap: cap must be in [0, %d] (0 removes the cap; %d is this device's SM count), got %d", n, n, cap);
+    return -1;
+  }
+  return g_sm_cap.exchange(cap);
+}
 
 size_t bb_workspace_bytes(const bb_matmul_desc* desc, int m) {
   if (validate(desc)) return 0;

@@ -63,7 +63,8 @@ struct MatmulArgs {
 
 constexpr int BB_MAX_DEVICES = 64;
 int current_device();     // ordinal of the calling thread's current CUDA device, clamped to [0, BB_MAX_DEVICES)
-int device_sm_count();    // SM count of the current device (cached per device)
+int device_sm_count();    // SM count of the current device (cached per device), at most the bb_set_sm_count_cap cap
+int device_sm_count_uncapped();   // the same without the cap
 // whether the streaming kernels launch with programmatic dependent launch (default on; BB_PDL=0 restores plain stream order)
 bool pdl_enabled();
 
@@ -153,6 +154,7 @@ int launch_gemv_mma(const MatmulArgs& a);
 bool gemv_slab_supported(const bb_matmul_desc& d, int m);
 int launch_gemv_slab(const MatmulArgs& a);
 size_t gemv_slab_workspace_bytes();     // tagged partial slots (must be zero-initialised once by the caller)
+size_t gemv_slab_slot_bytes(int sms);   // the slot region of a launch on `sms` SMs (gemv_slab_workspace_bytes at device_sm_count)
 bool gemv_i8_supported(const bb_matmul_desc& d, int m);
 int launch_gemv_i8(const MatmulArgs& a);
 bool gemm_ts_supported(const bb_matmul_desc& d, int m);

@@ -338,6 +338,10 @@ int choose_splits(int tiles, int num_kb, int sms) {
   return best;
 }
 
+// Byte offset of the split-K partials in the workspace: past the m = 1 slab kernel's slot region, sized at the device's full SM
+// count whatever bb_set_sm_count_cap says.  An operator hands one buffer to every m, and the slab requires its slots zero on entry.
+size_t splitk_partials_offset() { return gemv_slab_slot_bytes(device_sm_count_uncapped()); }
+
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
@@ -373,9 +377,10 @@ int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
   const int num_kb_total = a.d.K / EI::kKB;
   const int tiles = p.m_tiles * (a.d.N / TS_ROWS);
   p.splits = a.m <= 128 ? choose_splits(tiles, num_kb_total, device_sm_count()) : 1;
-  if (p.splits > 1 && a.workspace_bytes < size_t(p.splits) * a.m * a.d.N * 4) p.splits = 1;  // no scratch given
+  const size_t ws_off = splitk_partials_offset();
+  if (p.splits > 1 && a.workspace_bytes < ws_off + size_t(p.splits) * a.m * a.d.N * 4) p.splits = 1;  // no scratch given
   p.kb_per_split = num_kb_total / p.splits;
-  p.ws = a.workspace;
+  p.ws = p.splits > 1 ? static_cast<char*>(a.workspace) + ws_off : a.workspace;
   const size_t smem_bytes = SM::kTotal;
   CUtensorMap tmA, tmW;
   const CUtensorMapDataType adt = EI::kInt8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
@@ -453,7 +458,7 @@ size_t gemm_ts_workspace_bytes(const bb_matmul_desc& d, int m) {
   const int bm = m <= 32 ? 32 : (m <= 64 ? 64 : 128);
   const int tiles = ((m + bm - 1) / bm) * (d.N / TS_ROWS);
   const int sp = choose_splits(tiles, d.K / kb, device_sm_count());
-  return sp > 1 ? size_t(sp) * m * d.N * 4 : 0;
+  return sp > 1 ? splitk_partials_offset() + size_t(sp) * m * d.N * 4 : 0;
 }
 
 int launch_gemm_ts(const MatmulArgs& a) {

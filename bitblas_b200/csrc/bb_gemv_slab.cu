@@ -630,7 +630,8 @@ int launch_slab(const MatmulArgs& a, const CUtensorMap& tm, const SlabParams& p)
 }  // namespace
 
 // tagged exchange slots: [CTAs][consumer groups][32 rows], at most GS_MINB CTAs per SM
-size_t gemv_slab_workspace_bytes() { return size_t(GS_MINB * GS_NG) * size_t(device_sm_count()) * GS_ROWS * 8 + 256; }
+size_t gemv_slab_slot_bytes(int sms) { return size_t(GS_MINB * GS_NG) * size_t(sms) * GS_ROWS * 8 + 256; }
+size_t gemv_slab_workspace_bytes() { return gemv_slab_slot_bytes(device_sm_count()); }
 
 bool gemv_slab_supported(const bb_matmul_desc& d, int m) {
   if (m != 1) return false;

@@ -268,7 +268,8 @@ int bb_peer_barrier(void* const* peer_flags, int n_peers, int rank, void* stream
  * The buffer must be ZERO-INITIALISED once by the caller before its first use (cudaMemset / torch.zeros): the slab kernel
  * exchanges partial sums through tagged slots and leaves every slot zero-tagged again when it finishes, so the same
  * buffer can then be reused by later calls ON THE SAME STREAM without clearing (calls that may run concurrently need their
- * own buffers).  The split-K partials of the wgmma kernel carry no such requirement. */
+ * own buffers).  The wgmma kernel's split-K partials need no clearing; they start past the slab kernel's slot region (sized
+ * at the device's full SM count), so one buffer can serve every m: a split-K call never dirties the slots an m = 1 call reads. */
 size_t bb_workspace_bytes(const bb_matmul_desc* desc, int m);
 
 /* which kernel family bb_matmul would run for (desc, m) -- bb_kernel_id; <0 on invalid desc. */
@@ -276,6 +277,12 @@ int bb_select_kernel(const bb_matmul_desc* desc, int m);
 const char* bb_kernel_name(int kernel_id);
 /* testing hook: force a kernel family (BB_KERNEL_AUTO restores dispatch). Returns previous value. */
 int bb_set_kernel_override(int kernel_id);
+/* testing hook: every kernel sizes its work decomposition (grids, split-K, stream-K ranges, bb_workspace_bytes) as if the device
+ * had min(real SM count, cap) SMs, so one device runs the partitions of smaller parts (an H100 PCIe, a MIG slice).  Kernel choice
+ * (bb_select_kernel) does not depend on it.  cap = 0 removes the cap.  A cap below 0 or above the current device's SM count is
+ * refused (-1, bb_last_error set, cap unchanged): a capped grid must stay resident at once.  Returns the previous cap.  Global
+ * to the process; set it while no call is in flight and size workspaces after setting it. */
+int bb_set_sm_count_cap(int cap);
 /* number of kernel launches issued by this library since load (bench.py's gpu_launches counter). */
 uint64_t bb_launch_count(void);
 

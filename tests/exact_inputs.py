@@ -427,6 +427,11 @@ def slab_geometry(N, K, sms):
     return UPR, NRB, T, R
 
 
+def slab_slot_bytes(sms):
+    """bb_workspace_bytes of an m = 1 slab call on `sms` SMs: [2 CTAs per SM][NG groups][32 rows] 8-byte slots, + 256 for alignment"""
+    return 2 * NG * ROWS * 8 * sms + 256
+
+
 def range_begin(ri, T, R):
     return ri * T // R
 
@@ -470,6 +475,8 @@ def slab_coverage(N, K, sms):
             props.add("padding_only_range")
         for grp in range(NG):
             segs = _segments(t0, t1, grp, UPR)
+            if sum(1 for rb, kus in segs if rb < NRB and kus == list(range(UPR))) >= 2:
+                props.add("group_closes_2_blocks")   # several owner fix-ups of one group in one CTA (small SM counts only)
             for j, (rb, kus) in enumerate(segs):
                 if rb >= NRB:
                     continue

@@ -114,6 +114,43 @@ def test_c_abi_validation_without_gpu():
         assert lib.bb_init(0) != 0 and b"CUDA" in lib.bb_last_error()
 
 
+def test_sm_count_cap_hook():
+    """bb_set_sm_count_cap: negative caps and caps above the device's SM count are refused and leave the cap as it was; every
+    accepted call returns the previous cap and starts a new workspace generation; kernel choice does not depend on the cap"""
+    lib = _lib.load()
+    descs = []
+    for a, w, bits, accum, out, layout in [(_lib.BB_F16, _lib.BB_W_UINT, 4, _lib.BB_F32, _lib.BB_F16, 0),
+                                           (_lib.BB_BF16, _lib.BB_W_INT, 4, _lib.BB_F32, _lib.BB_BF16, 1),
+                                           (_lib.BB_F16, _lib.BB_W_UINT, 2, _lib.BB_F32, _lib.BB_F32, 1),
+                                           (_lib.BB_I8, _lib.BB_W_INT, 2, _lib.BB_I32, _lib.BB_I32, 2),
+                                           (_lib.BB_F16, _lib.BB_W_FP4, 4, _lib.BB_F32, _lib.BB_F16, 0)]:
+        for N, K in [(4096, 4096), (1024, 3584), (48, 2304), (12288, 12288)]:
+            d = _lib.MatmulDesc()
+            d.N, d.K, d.a_dtype, d.w_fmt, d.w_bits, d.accum_dtype, d.out_dtype, d.w_layout = N, K, a, w, bits, accum, out, layout
+            d.group_size, d.with_scaling = (128, 1) if a != _lib.BB_I8 else (-1, 0)
+            descs.append(d)
+    ms = (1, 2, 8, 9, 16, 32, 100, 128, 4096)
+    dispatch = lambda: [lib.bb_select_kernel(ctypes.byref(d), m) for d in descs for m in ms]   # noqa: E731
+    plain = dispatch()
+    assert {_lib.BB_KERNEL_GEMV_SLAB, _lib.BB_KERNEL_GEMV_MMA, _lib.BB_KERNEL_GEMM_TS, _lib.BB_KERNEL_GEMM_TS_I8} <= set(plain)
+    prev = lib.bb_set_sm_count_cap(0)
+    try:
+        for bad in (-1, -132, 1 << 20):
+            gen = _lib.OVERRIDE_GEN
+            assert lib.bb_set_sm_count_cap(bad) < 0
+            assert b"bb_set_sm_count_cap" in lib.bb_last_error()
+            assert _lib.OVERRIDE_GEN == gen + 1
+            assert lib.bb_set_sm_count_cap(0) == 0, f"the refused cap {bad} was applied"
+        for cap in (1, 7, 33, 66):
+            gen = _lib.OVERRIDE_GEN
+            assert lib.bb_set_sm_count_cap(cap) == 0
+            assert _lib.OVERRIDE_GEN == gen + 1
+            assert dispatch() == plain, cap
+            assert lib.bb_set_sm_count_cap(0) == cap
+    finally:
+        lib.bb_set_sm_count_cap(prev)
+
+
 def test_forward_refuses_cpu_tensors():
     op = bitblas.Matmul(bitblas.MatmulConfig(M=1, N=16, K=128, W_dtype="uint4"), enable_tuning=False)
     with pytest.raises(RuntimeError, match="no CPU path"):

@@ -12,7 +12,19 @@ SLAB_SHAPES = [(8192, 8192), (28672, 8192), (8192, 28672), (12288, 12288),      
                (1024, 8192), (1024, 3584), (16, 4096), (48, 2304), (2064, 3840), (4112, 6144)]   # shards, padding, ragged, N % 32 = 16
 SLAB_PROPERTIES = {"block_over_3_ranges", "range_inside_block", "owner_stops_mid_block", "one_unit_per_cta", "odd_NRB",
                    "padding_only_range", "ragged_last_unit_1_slices", "ragged_last_unit_2_slices", "ragged_last_unit_3_slices",
-                   "N%32=16"}
+                   "N%32=16", "group_closes_2_blocks"}
+SMALL_SM_PROPERTIES = {"group_closes_2_blocks"}   # at these shapes only below 120 SMs: tested at capped SM counts
+# the SM counts test_gpu_sm_counts.py runs SLAB_SHAPES at, besides the device's own (1: R = 2 ranges; 114: H100 PCIe)
+SLAB_CAPS = (1, 2, 3, 5, 33, 114)
+
+
+def slab_cap_coverage(device_sms):
+    """{property: the caps of SLAB_CAPS + (device_sms,) at which one of SLAB_SHAPES reaches it}"""
+    hit = {}
+    for cap in sorted(set(SLAB_CAPS) | {device_sms}):
+        for p in set().union(*(X.slab_coverage(N, K, cap) for N, K in SLAB_SHAPES)):
+            hit.setdefault(p, []).append(cap)
+    return hit
 
 
 # ---- the checker ----------------------------------------------------------------------------------------------------------------
@@ -124,7 +136,25 @@ def test_slab_shapes_cover_every_stream_k_property():
     hit = set()
     for N, K in SLAB_SHAPES:
         hit |= X.slab_coverage(N, K, 132)
-    assert SLAB_PROPERTIES <= hit, SLAB_PROPERTIES - hit
+    assert SLAB_PROPERTIES - SMALL_SM_PROPERTIES <= hit, SLAB_PROPERTIES - SMALL_SM_PROPERTIES - hit
+    assert not SMALL_SM_PROPERTIES & hit, "reached on a full H100: not a small-SM-count property"
+
+
+def test_slab_caps_cover_every_property_three_times():
+    """the capped SM counts of test_gpu_sm_counts.py reach every property at three or more caps, one of them below 8"""
+    hit = slab_cap_coverage(132)
+    for p in sorted(SLAB_PROPERTIES):
+        caps = hit.get(p, [])
+        assert len(caps) >= 3 and min(caps) < 8, (p, caps)
+
+
+def test_group_closes_2_blocks_property():
+    """one group of one range closes two whole row blocks only when the range is long enough: two ranges over 896 row blocks
+    do, 264 ranges do not, and a shape with one block per group never does"""
+    N, K = 28672, 8192
+    assert "group_closes_2_blocks" in X.slab_coverage(N, K, 1)           # R = 2: every group closes hundreds of blocks
+    assert "group_closes_2_blocks" not in X.slab_coverage(N, K, 132)
+    assert "group_closes_2_blocks" not in X.slab_coverage(48, 2304, 1)   # NRB = 2: one block per group
 
 
 # ---- gemv_mma / gemv_i8 K split ---------------------------------------------------------------------------------------------------

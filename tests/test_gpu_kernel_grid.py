@@ -410,13 +410,16 @@ def _sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-def _check_split(op, m, split, kb):
+def _check_split(op, m, split, kb, sms=None):
+    """the split-K factor of the launch on `sms` SMs (default: the device's), read from bb_workspace_bytes: 0 without split-K,
+    else the slab's slot region at the device's full SM count followed by f [m, N] fp32 partials"""
     from bitblas_b200 import _lib
+    from exact_inputs import slab_slot_bytes
     ws = _lib.load().bb_workspace_bytes(ctypes.byref(op._desc), m)
-    expect = ts_splits(m, op.N, op.K, kb, _sms()) > 1
-    assert (ws > 0) == expect, (m, ws, expect)
+    f = ts_splits(m, op.N, op.K, kb, sms or _sms())
+    assert ws == (slab_slot_bytes(_sms()) + f * m * op.N * 4 if f > 1 else 0), (m, ws, f)
     if m <= 128:
-        assert expect == split
+        assert (f > 1) == split
 
 
 @pytest.mark.parametrize("c", TS_CELLS, ids=[_id(c) for c in TS_CELLS])

@@ -294,6 +294,7 @@ def test_block_graph_replay_matches_eager():
 CHAIN = r"""
 import sys, torch
 sys.path[:0] = [{root!r}, {tests!r}, {oracle!r}]
+{prologue}
 from test_gpu_moe import _make_block, _routing
 m, _ = _make_block(seed=21)
 outs = []
@@ -310,20 +311,27 @@ torch.save([o.cpu() for o in outs], {path!r})
 """
 
 
-def test_block_pdl_chain_matches_plain_stream_order(tmp_path):
-    """16 blocks back to back, each fed by the previous one's output, without synchronisation: the launches chained with PDL give
-    the same bits as BB_PDL=0 (plain stream order), which the library reads once per process"""
+def pdl_chain_matches_plain_stream_order(chain, tmp_path, prologue=""):
+    """runs the script `chain` (a template with the keys root, tests, oracle, path and prologue: code run before the chain) once
+    with BB_PDL=1 and once with BB_PDL=0, which the library reads once per process, and asserts bit-identical step outputs"""
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     res = {}
     for pdl in ("1", "0"):
         path = str(tmp_path / f"chain{pdl}.pt")
-        env = dict(os.environ, BB_PDL=pdl)
-        code = CHAIN.format(root=root, tests=os.path.join(root, "tests"), oracle=os.path.join(root, "oracle"), path=path)
-        r = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=600)
+        code = chain.format(root=root, tests=os.path.join(root, "tests"), oracle=os.path.join(root, "oracle"), path=path,
+                            prologue=prologue)
+        r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, BB_PDL=pdl), capture_output=True, text=True,
+                           timeout=600)
         assert r.returncode == 0, r.stderr[-2000:]
         res[pdl] = torch.load(path)
     for i, (a, b) in enumerate(zip(res["1"], res["0"])):
         assert torch.equal(a, b), f"step {i}"
+
+
+def test_block_pdl_chain_matches_plain_stream_order(tmp_path):
+    """16 blocks back to back, each fed by the previous one's output, without synchronisation: the launches chained with PDL give
+    the same bits as BB_PDL=0 (plain stream order)"""
+    pdl_chain_matches_plain_stream_order(CHAIN, tmp_path)
 
 
 @pytest.mark.parametrize("v2", [False, True])

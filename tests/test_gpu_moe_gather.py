@@ -4,9 +4,6 @@ including malformed indices with guard rows; and the copy-free block (moe_route_
 bit-identical to MoEExperts wherever its gate/up call runs the grouped GEMM, with its launch count, graph replay, a PDL chain and
 its peak memory."""
 import itertools
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -14,7 +11,7 @@ import torch
 from test_gpu_grouped_gemm import ROUTINGS as GEMM_ROUTINGS
 from test_gpu_grouped_gemm import _build, grouped_bm
 from test_gpu_kernel_grid import MODES, OUTS
-from test_gpu_moe import _launches, _make_block, _routing
+from test_gpu_moe import _launches, _make_block, _routing, pdl_chain_matches_plain_stream_order
 
 pytestmark = pytest.mark.gpu
 
@@ -231,6 +228,7 @@ def test_gathering_block_graph_replay_matches_eager():
 CHAIN = r"""
 import sys, torch
 sys.path[:0] = [{root!r}, {tests!r}, {oracle!r}]
+{prologue}
 from test_gpu_moe import _make_block, _routing
 from test_gpu_moe_gather import _gathering
 m, _ = _make_block(E=8, seed=23)
@@ -249,17 +247,7 @@ torch.save([o.cpu() for o in outs], {path!r})
 
 def test_gathering_block_pdl_chain_matches_plain_stream_order(tmp_path):
     """8 copy-free blocks (2048 rows over 8 experts) back to back without synchronisation: PDL gives the bits of BB_PDL=0"""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    res = {}
-    for pdl in ("1", "0"):
-        path = str(tmp_path / f"chain{pdl}.pt")
-        code = CHAIN.format(root=root, tests=os.path.join(root, "tests"), oracle=os.path.join(root, "oracle"), path=path)
-        r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, BB_PDL=pdl), capture_output=True, text=True,
-                           timeout=600)
-        assert r.returncode == 0, r.stderr[-2000:]
-        res[pdl] = torch.load(path)
-    for i, (a, b) in enumerate(zip(res["1"], res["0"])):
-        assert torch.equal(a, b), f"step {i}"
+    pdl_chain_matches_plain_stream_order(CHAIN, tmp_path)
 
 
 def test_gathering_block_peak_memory_drops_by_the_copy():
