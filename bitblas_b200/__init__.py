@@ -27,4 +27,5 @@ from . import cache, quantization, testing  # noqa: E402,F401
 from .parallel import ColumnParallelLinear  # noqa: E402,F401
 from .graph import CapturedStep  # noqa: E402,F401
 from .moe import MoEExperts, moe_topk  # noqa: E402,F401
+from .mlp import SwiGLUMLP  # noqa: E402,F401
 from .act_order import permute_cols  # noqa: E402,F401

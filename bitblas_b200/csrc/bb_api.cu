@@ -258,10 +258,23 @@ size_t bb_workspace_bytes(const bb_matmul_desc* desc, int m) {
   return 0;
 }
 
-static int matmul_impl(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
+// the gate/up interleave pairs 8 gate rows with 8 up rows in every 16-row block of W: N = 2I with I % 8 == 0
+static bool swiglu_shape_ok(const bb_matmul_desc* desc) {
+  if (desc && desc->N % 16) {
+    set_error("SwiGLU: desc->N = 2I needs I %% 8 == 0 (gate/up interleave in blocks of 8 rows; N=%d)", desc->N);
+    return false;
+  }
+  return true;
+}
+
+static int matmul_impl(bool swiglu, const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
                        const void* zeros, const void* bias, void* C, void* const* peer_C, int n_peers, long long ldc,
                        long long col_offset, int m, void* workspace, size_t workspace_bytes, void* stream) {
   if (validate(desc)) return 1;
+  if (swiglu) {
+    if (desc->a_dtype == BB_I8) { set_error("bb_matmul_swiglu: int8 activations are not supported (float16 | bfloat16)"); return 1; }
+    if (!swiglu_shape_ok(desc)) return 1;
+  }
   if (m == 0) return 0;  // wrapper/tl.py:156-157
   if (m < 0) { set_error("m must be >= 0 (got %d)", m); return 1; }
   if (!A || !W || (!C && n_peers == 0)) { set_error("A, W and C must be non-null"); return 1; }
@@ -280,6 +293,7 @@ static int matmul_impl(const bb_matmul_desc* desc, const void* A, const void* W,
   a.n_peers = n_peers; a.ldc = n_peers ? ldc : desc->N; a.col_offset = n_peers ? col_offset : 0;
   for (int i = 0; i < BB_MAX_PEERS; ++i) a.peer_C[i] = (i < n_peers) ? peer_C[i] : nullptr;
   a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.stream = (cudaStream_t)stream;
+  a.swiglu = swiglu;
   const int k = select(a.d, m);
   if (n_peers > 0 && k == BB_KERNEL_GENERIC) {
     set_error("the column-parallel scatter epilogue needs a fast kernel (gemv_mma / gemv_i8 / gemm_ts); this configuration dispatches to generic_simt");
@@ -300,24 +314,21 @@ static int matmul_impl(const bb_matmul_desc* desc, const void* A, const void* W,
 int bb_matmul(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
               const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes,
               void* stream) {
-  return matmul_impl(desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes, stream);
+  return matmul_impl(false, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes, stream);
+}
+
+int bb_matmul_swiglu(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
+                     const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes,
+                     void* stream) {
+  return matmul_impl(true, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes, stream);
 }
 
 int bb_matmul_scatter(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
                       const void* zeros, const void* bias, void* const* peer_C, int n_peers, int64_t ldc,
                       int64_t col_offset, int m, void* workspace, size_t workspace_bytes, void* stream) {
   if (n_peers < 1) { set_error("bb_matmul_scatter needs n_peers >= 1"); return 1; }
-  return matmul_impl(desc, A, W, lut, scale, zeros, bias, nullptr, peer_C, n_peers, ldc, col_offset, m, workspace,
+  return matmul_impl(false, desc, A, W, lut, scale, zeros, bias, nullptr, peer_C, n_peers, ldc, col_offset, m, workspace,
                      workspace_bytes, stream);
-}
-
-// the gate/up interleave pairs 8 gate rows with 8 up rows in every 16-row block of W: N = 2I with I % 8 == 0
-static bool swiglu_shape_ok(const bb_matmul_desc* desc) {
-  if (desc && desc->N % 16) {
-    set_error("SwiGLU: desc->N = 2I needs I %% 8 == 0 (gate/up interleave in blocks of 8 rows; N=%d)", desc->N);
-    return false;
-  }
-  return true;
 }
 
 // the grouped entry points: gemm picks the grouped wgmma GEMM instead of the grouped GEMV, swiglu the fused gate/up epilogue,

@@ -57,6 +57,7 @@ struct MatmulArgs {
   void* workspace;
   size_t workspace_bytes;
   cudaStream_t stream;
+  bool swiglu;           // bb_matmul_swiglu: W holds gate/up interleaved (d.N = 2I rows), C is [m, d.N / 2] = silu(gate) * up
   int groups() const { return d.K / (d.group_size <= 0 ? d.K : d.group_size); }
   int gsize() const { return d.group_size <= 0 ? d.K : d.group_size; }
 };
@@ -246,7 +247,7 @@ inline OutSpec make_outspec(void* C, long long ld) {   // the single output C
   return o;
 }
 inline OutSpec make_outspec(const MatmulArgs& a) {
-  if (a.n_peers == 0) return make_outspec(a.C, a.d.N);
+  if (a.n_peers == 0) return make_outspec(a.C, a.swiglu ? a.d.N / 2 : a.d.N);
   OutSpec o;
   o.n = a.n_peers;
   for (int i = 0; i < BB_MAX_PEERS; ++i) o.ptr[i] = i < a.n_peers ? a.peer_C[i] : nullptr;
@@ -589,9 +590,9 @@ __device__ __forceinline__ void store_out_i32(void* C, size_t o, int v, int b, i
   }
 }
 
-// ---- SwiGLU epilogue of the grouped kernels (gate/up interleave: weight row 16b + i is gate row 8b + i for i < 8, up row 8b + i - 8
-// for i >= 8; both halves of a 16-row block are owned by the same thread) ----------------------------------------------------------
-// one pre-activation as the plain grouped epilogue stores it
+// ---- SwiGLU epilogue of bb_matmul_swiglu and the grouped SwiGLU calls (gate/up interleave: weight row 16b + i is gate row 8b + i for
+// i < 8, up row 8b + i - 8 for i >= 8) ----------------------------------------------------------------------------------------------
+// one pre-activation as the plain epilogue stores it
 __device__ __forceinline__ float swiglu_operand(float v, bool has_bias, float bias, int out_dtype) {
   if (out_dtype == BB_F16) return __half2float(round_out<__half>(v, has_bias, bias));
   if (out_dtype == BB_BF16) return __bfloat162float(round_out<__nv_bfloat16>(v, has_bias, bias));

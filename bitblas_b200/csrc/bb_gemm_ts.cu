@@ -27,8 +27,10 @@ namespace bb {
 namespace {
 
 // FMT: 0 = integer formats (LOP3 magic-number decode), 1 = 16-entry table formats (NF4 / fp4; BITS = 4, compressed storage),
-//      2 = 8-bit float weights (e4m3 / e5m2; BITS = 8)
-template <typename T, int BITS, int BM, bool IL, int FMT = 0>
+//      2 = 8-bit float weights (e4m3 / e5m2; BITS = 8).  SWIGLU (16-bit activations only): bb_matmul_swiglu -- without split-K the
+//      epilogue is store_tile_swiglu; with it the raw partials are written as in the plain instance and splitk_reduce_kernel forms
+//      silu(gate) * up
+template <typename T, int BITS, int BM, bool IL, int FMT = 0, bool SWIGLU = false>
 __global__ void __launch_bounds__(TS_THREADS, 1)
 gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const TsParams p) {
   using SM = TsSmem<T, BITS, BM>;
@@ -190,6 +192,12 @@ gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 
   // ----- epilogue: acc[4i + 2h + j] = C^T[row rA + 8h][column 8i + 2t + j] -> C[m, n] -----
+  if constexpr (SWIGLU) {
+    if (p.splits == 1) {
+      store_tile_swiglu<T, BM>(acc, p, reinterpret_cast<const T*>(p.bias), m0, p.M, nA, nB, t);
+      return;
+    }
+  }
   float bias_f[2] = {0.f, 0.f};
   if (p.bias) {
 #pragma unroll
@@ -247,10 +255,52 @@ gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 }
 
+// splitk_reduce_kernel of the SWIGLU instances: out[m, c] = silu(g) * u for the output columns c = 8b + i, with g and u the plain
+// reduce's values of rows 16b + i and 16b + i + 8 (the same split order and rounding).  One thread = 4 consecutive c, which never
+// straddle a block of 8 (N / 2 % 4 == 0): one 128-bit load of gate and one of up partials per split.
+__device__ __forceinline__ void splitk_reduce_swiglu(const TsParams& p) {
+  const unsigned n4 = unsigned(p.N) >> 3;                 // output quads per row (N / 2 columns)
+  const unsigned total4 = unsigned(p.M) * n4;
+  const size_t split_stride4 = size_t(p.M) * (unsigned(p.N) >> 2);
+  for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < total4; i += gridDim.x * blockDim.x) {
+    const unsigned m = i / n4, c = (i - m * n4) * 4u;
+    const unsigned ng = (c >> 3) * 16u + (c & 7u);       // first gate row of the quad; its up rows are 8 further
+    const size_t q = (size_t(m) * p.N + ng) >> 2;        // the gate quad's float4 index in one split's [M][N] partials
+    float g[4] = {0.f, 0.f, 0.f, 0.f}, u[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int sp = 0; sp < p.splits; ++sp) {
+      const float4* ws = reinterpret_cast<const float4*>(p.ws) + size_t(sp) * split_stride4 + q;
+      const float4 vg = __ldcs(ws), vu = __ldcs(ws + 2);
+      g[0] += vg.x; g[1] += vg.y; g[2] += vg.z; g[3] += vg.w;
+      u[0] += vu.x; u[1] += vu.y; u[2] += vu.z; u[3] += vu.w;
+    }
+    const size_t o = size_t(m) * (p.N / 2) + c;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float bg = 0.f, bu = 0.f;
+      if (p.bias) {
+        if (p.a_dtype == BB_F16) {
+          bg = __half2float(reinterpret_cast<const __half*>(p.bias)[ng + j]);
+          bu = __half2float(reinterpret_cast<const __half*>(p.bias)[ng + 8 + j]);
+        } else {
+          bg = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.bias)[ng + j]);
+          bu = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(p.bias)[ng + 8 + j]);
+        }
+      }
+      store_swiglu(p.out.ptr[0], o + j, swiglu_operand(g[j], p.bias != nullptr, bg, p.out_dtype),
+                   swiglu_operand(u[j], p.bias != nullptr, bu, p.out_dtype), p.out_dtype);
+    }
+  }
+}
+
 // out[m, n] = cast(sum_s ws[s][m][n]) (+ bias), stored to every destination of the OutSpec.  One thread = 4 consecutive n
 // (N is a multiple of 128 here): 128-bit loads of the partials, 32-bit index arithmetic, one vector store per destination.
-template <bool INT8>
+// SWIGLU: splitk_reduce_swiglu.
+template <bool INT8, bool SWIGLU = false>
 __global__ void splitk_reduce_kernel(const TsParams p) {
+  if constexpr (SWIGLU) {
+    splitk_reduce_swiglu(p);
+    return;
+  }
   const unsigned n4 = unsigned(p.N) >> 2;                 // quads per row
   const unsigned total4 = unsigned(p.M) * n4;             // m * N / 4 < 2^31 (m <= 128 on this path)
   const size_t split_stride4 = size_t(p.M) * n4;          // quads per split
@@ -362,11 +412,11 @@ int make_map_w_tiled(CUtensorMap* map, const void* base, uint64_t row_bytes, uin
   return 0;
 }
 
-template <typename T, int BITS, int BM, bool IL, int FMT = 0>
+template <typename T, int BITS, int BM, bool IL, int FMT, bool SWIGLU>
 int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
   using SM = TsSmem<T, BITS, BM>;
   using EI = ElemInfo<T>;
-  auto kernel = gemm_ts_kernel<T, BITS, BM, IL, FMT>;
+  auto kernel = gemm_ts_kernel<T, BITS, BM, IL, FMT, SWIGLU>;
   static KernelCache<> cache;
   if (!kernel_setup(cache, kernel, SM::kTotal)) {
     set_error("gemm_ts: cannot raise the kernel's dynamic shared memory to %d bytes on this device", SM::kTotal);
@@ -399,10 +449,11 @@ int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
   kernel<<<grid, TS_THREADS, smem_bytes, a.stream>>>(tmA, tmW, p);
   BB_LAUNCH_CHECK();
   if (p.splits > 1) {
-    const size_t total = size_t(a.m) * a.d.N / 4;   // one thread per 4 consecutive n
+    const size_t total = size_t(a.m) * a.d.N / (SWIGLU ? 8 : 4);   // one thread per 4 consecutive output columns
     const int rthreads = 256;
     const int rblocks = int(std::min<size_t>((total + rthreads - 1) / rthreads, size_t(device_sm_count()) * 8));
     if (EI::kInt8) splitk_reduce_kernel<true><<<rblocks, rthreads, 0, a.stream>>>(p);
+    else if (SWIGLU) splitk_reduce_kernel<false, true><<<rblocks, rthreads, 0, a.stream>>>(p);
     else splitk_reduce_kernel<false><<<rblocks, rthreads, 0, a.stream>>>(p);
     BB_LAUNCH_CHECK();
   }
@@ -410,11 +461,19 @@ int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
 }
 
 // activation rows per CTA: the wgmma N extent (m > 128 runs several 128-row tiles)
+template <typename T, int BITS, bool IL, int FMT, bool SWIGLU>
+int launch_ts_bm_sw(const MatmulArgs& a, const TsParams& p) {
+  if (a.m <= 32) return launch_ts_inst<T, BITS, 32, IL, FMT, SWIGLU>(a, p);
+  if (a.m <= 64) return launch_ts_inst<T, BITS, 64, IL, FMT, SWIGLU>(a, p);
+  return launch_ts_inst<T, BITS, 128, IL, FMT, SWIGLU>(a, p);
+}
+// (the int8 instances have no SWIGLU form: bb_matmul_swiglu rejects int8 activations)
 template <typename T, int BITS, bool IL, int FMT>
 int launch_ts_bm(const MatmulArgs& a, const TsParams& p) {
-  if (a.m <= 32) return launch_ts_inst<T, BITS, 32, IL, FMT>(a, p);
-  if (a.m <= 64) return launch_ts_inst<T, BITS, 64, IL, FMT>(a, p);
-  return launch_ts_inst<T, BITS, 128, IL, FMT>(a, p);
+  if constexpr (!std::is_same<T, int8_t>::value) {
+    if (a.swiglu) return launch_ts_bm_sw<T, BITS, IL, FMT, true>(a, p);
+  }
+  return launch_ts_bm_sw<T, BITS, IL, FMT, false>(a, p);
 }
 template <typename T, int BITS>
 int launch_ts_layout(const MatmulArgs& a, const TsParams& p) {

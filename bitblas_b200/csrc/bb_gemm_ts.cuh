@@ -266,6 +266,27 @@ struct RowGroup {
   }
 };
 
+// The SwiGLU epilogue of the wgmma GEMMs (gemm_ts_kernel without split-K, gemm_ts_grouped_kernel): acc[4i + 2h + j] = C^T[row
+// rA + 8h][column 8i + 2t + j], and the thread's rows nA = 16b + i and nB = nA + 8 (i < 8) are gate and up of
+// C[m, 8b + i] = silu(gate) * up (row stride N / 2), for the rows m < m_end; bias is A_dtype [N] or null
+template <typename T, int BM>
+__device__ __forceinline__ void store_tile_swiglu(const float (&acc)[BM / 2], const TsParams& p, const T* bias, int m0, int m_end,
+                                                  int nA, int nB, int t) {
+  const float bg = bias ? TypeTraits<T>::to_float(bias[nA]) : 0.f, bu = bias ? TypeTraits<T>::to_float(bias[nB]) : 0.f;
+  const size_t col = size_t(nA >> 4) * 8 + size_t(nA & 7);
+#pragma unroll
+  for (int i = 0; i < BM / 8; ++i) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int m = m0 + 8 * i + 2 * t + j;
+      if (m >= m_end) continue;
+      const float g = swiglu_operand(acc[4 * i + j], bias != nullptr, bg, p.out_dtype);
+      const float u = swiglu_operand(acc[4 * i + 2 + j], bias != nullptr, bu, p.out_dtype);
+      store_swiglu(p.out.ptr[0], size_t(m) * size_t(p.N / 2) + col, g, u, p.out_dtype);
+    }
+  }
+}
+
 }  // namespace
 
 }  // namespace bb

@@ -32,11 +32,12 @@ __device__ __forceinline__ void mma_16832_u8s8(int (&c)[4], const uint32_t (&a)[
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-template <typename T, int BITS, bool IL, int NT, int ZK, bool SC>
+// SWIGLU: bb_matmul_swiglu (gate/up interleaved W, p.out = C [M, N / 2])
+template <typename T, int BITS, bool IL, int NT, int ZK, bool SC, bool SWIGLU = false>
 __global__ void __launch_bounds__(gemv_max_ks(NT) * 32) __maxnreg__(gemv_mma_maxnreg(NT, ZK))
 gemv_mma_kernel(const GemvParams p) {
   __shared__ float red[MAX_KS][16][8 * NT];
-  gemv_mma_tile<T, BITS, IL, NT, ZK, SC, true>(p, blockIdx.x, red);
+  gemv_mma_tile<T, BITS, IL, NT, ZK, SC, true, SWIGLU>(p, blockIdx.x, red);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -165,12 +166,13 @@ int launch_gemv_kernel(Kernel kernel, KernelCache<MAX_KS + 1>& cache, GemvParams
   return launch_pdl(kernel, nb, p.ks * 32, 0, stream, pdl_enabled(), p);
 }
 
-template <typename T, int BITS, bool IL>
+template <typename T, int BITS, bool IL, bool SWIGLU>
 int launch_mma_nt(const MatmulArgs& a, const GemvParams& p) {
   return gemv_mma_instance(p, p.M, [&](auto nt, auto zk, auto sc) {
     constexpr int NT = decltype(nt)::value;
     static KernelCache<MAX_KS + 1> cache;
-    return launch_gemv_kernel<NT>(gemv_mma_kernel<T, BITS, IL, NT, decltype(zk)::value, decltype(sc)::value>, cache, p, a.stream);
+    return launch_gemv_kernel<NT>(gemv_mma_kernel<T, BITS, IL, NT, decltype(zk)::value, decltype(sc)::value, SWIGLU>, cache, p,
+                                  a.stream);
   });
 }
 
@@ -202,7 +204,10 @@ int launch_gemv_mma(const MatmulArgs& a) {
   }
   const GemvParams p = make_params(a);
   return dispatch_t_bits_il(a.d, [&](auto t, auto bits, auto il) {
-    return launch_mma_nt<typename decltype(t)::type, decltype(bits)::value, decltype(il)::value>(a, p);
+    using T = typename decltype(t)::type;
+    constexpr int BITS = decltype(bits)::value;
+    constexpr bool IL = decltype(il)::value;
+    return a.swiglu ? launch_mma_nt<T, BITS, IL, true>(a, p) : launch_mma_nt<T, BITS, IL, false>(a, p);
   });
 }
 

@@ -156,12 +156,22 @@ __device__ __forceinline__ void gs_store(const SlabParams& p, int n, float v) {
   }
 }
 
+// bb_matmul_swiglu: C[0, col] = silu(g) * u of gate row n and up row n + 8, each rounded as gs_store rounds it (row stride N / 2)
+template <typename T>
+__device__ __forceinline__ void gs_store_swiglu(const SlabParams& p, int n, int col, float vg, float vu) {
+  const T* bias = reinterpret_cast<const T*>(p.bias);
+  const float g = swiglu_operand(vg, bias != nullptr, bias ? TypeTraits<T>::to_float(bias[n]) : 0.f, p.out_dtype);
+  const float u = swiglu_operand(vu, bias != nullptr, bias ? TypeTraits<T>::to_float(bias[n + 8]) : 0.f, p.out_dtype);
+  store_swiglu(p.out.ptr[0], size_t(col), g, u, p.out_dtype);
+}
+
 __device__ __forceinline__ int gs_range_begin(int ri, int T, int R) { return int((long long)ri * T / R); }
 
 
 // FMT: 0 = uint4 / int4 (LOP3 magic decode, magic and zero point removed through the activation sums), 1 = 16-entry table formats
-// (NF4 / fp4, compressed storage: PRMT table decode to exact A_dtype values, scale only -- the sums are not needed)
-template <typename T, bool IL, int FMT>
+// (NF4 / fp4, compressed storage: PRMT table decode to exact A_dtype values, scale only -- the sums are not needed).
+// SWIGLU: bb_matmul_swiglu (gate/up interleaved W, p.out = C [1, N / 2]); only the final store differs
+template <typename T, bool IL, int FMT, bool SWIGLU = false>
 __global__ void __launch_bounds__(GS_THREADS, GS_MINB)
 gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
   constexpr bool F16 = std::is_same<T, __half>::value;
@@ -570,7 +580,15 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
               if (ej > t_last) break;
             }
           }
-          if (n < p.N) gs_store<T>(p, n, v);
+          if constexpr (SWIGLU) {
+            // lane l holds row rb * 32 + l: the gate rows of the block's two 16-row halves are lanes 0-7 and 16-23, their up rows
+            // the lanes 8 above.  The whole warp takes this branch (seg_from0 and closes are uniform over the group), so all 32
+            // lanes join the shuffle; a gate row below N has its up row below N too (N % 16 == 0)
+            const float vu = __shfl_down_sync(0xffffffffu, v, 8);
+            if ((lane & 8) == 0 && n < p.N) gs_store_swiglu<T>(p, n, rb * 16 + 8 * (lane >> 4) + (lane & 7), v, vu);
+          } else {
+            if (n < p.N) gs_store<T>(p, n, v);
+          }
         }
       }
 #pragma unroll
@@ -617,14 +635,18 @@ bool get_w_map(CUtensorMap* tm, const void* W, int N, int K) {
 }
 
 
-template <typename T, bool IL, int FMT>
-int launch_slab(const MatmulArgs& a, const CUtensorMap& tm, const SlabParams& p) {
-  auto kernel = gemv_slab_kernel<T, IL, FMT>;
+template <typename T, bool IL, int FMT, bool SWIGLU>
+int launch_slab_inst(const MatmulArgs& a, const CUtensorMap& tm, const SlabParams& p) {
+  auto kernel = gemv_slab_kernel<T, IL, FMT, SWIGLU>;
   static KernelCache<> cache;
   const int occ = kernel_setup(cache, kernel, kSmemOptinMax, GS_THREADS, GS_SMEM_BYTES);
   if (occ < 1) { set_error("gemv_slab: kernel does not fit on this device"); return 4; }
   const int grid = std::max(1, std::min(p.T, std::min(occ, GS_MINB) * device_sm_count()));
   return launch_pdl(kernel, grid, GS_THREADS, GS_SMEM_BYTES, a.stream, pdl_enabled(), tm, p);
+}
+template <typename T, bool IL, int FMT>
+int launch_slab(const MatmulArgs& a, const CUtensorMap& tm, const SlabParams& p) {
+  return a.swiglu ? launch_slab_inst<T, IL, FMT, true>(a, tm, p) : launch_slab_inst<T, IL, FMT, false>(a, tm, p);
 }
 
 }  // namespace

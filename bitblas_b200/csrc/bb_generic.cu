@@ -108,7 +108,9 @@ __device__ __forceinline__ void store_float_out(void* C, int out_dtype, size_t i
   }
 }
 
-template <typename T>
+// SWIGLU: bb_matmul_swiglu -- warp n computes output column n of C [M, N / 2] from the gate / up weight rows 16 (n / 8) + n % 8
+// and that + 8, each with the plain instance's arithmetic
+template <typename T, bool SWIGLU = false>
 __global__ void __launch_bounds__(WARPS * 32)
 generic_float_kernel(const bb_matmul_desc d, const T* __restrict__ A, const uint8_t* __restrict__ W,
                      const T* __restrict__ lut, const T* __restrict__ scale, const void* __restrict__ zeros,
@@ -116,60 +118,80 @@ generic_float_kernel(const bb_matmul_desc d, const T* __restrict__ A, const uint
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n = blockIdx.x * WARPS + warp;
   const int m0 = blockIdx.y * MT;
-  if (n >= d.N) return;
+  if (n >= (SWIGLU ? d.N / 2 : d.N)) return;
   const int K = d.K, bits = d.w_bits;
   const int g = d.group_size <= 0 ? K : d.group_size;
   const int G = K / g;
   const size_t row_bytes = size_t(K) * bits / 8;
   const int tiled = d.w_tile == BB_TILE_SLAB;
-  const uint8_t* Wrow = W + (tiled ? tiled_byte_offset(n, 0, (long long)row_bytes) : size_t(n) * row_bytes);
   // "rescale" w * s - z: the reference's LOP3 decode (fp16, interleaved integer weights) uses one fma for 4- and 1-bit weights
   // (lop3.py:256,269; decode_i1b_to_f16_scale_zeros_rescale) but multiplies then subtracts for 2-bit ones (:633-635); every
   // other case is its TE definition, two roundings (bf16 has no fast decode in the reference)
   const bool use_fma = d.w_layout != BB_LAYOUT_COMPRESSED && (d.w_fmt == BB_W_UINT || d.w_fmt == BB_W_INT) &&
                        std::is_same<T, __half>::value && bits != 2;
-  float acc[MT];
+  // acc[i] = the dot product of row m0 + i of A with weight row `n`, in every lane
+  auto row_dot = [&](const int n, float (&acc)[MT]) {
+    const uint8_t* Wrow = W + (tiled ? tiled_byte_offset(n, 0, (long long)row_bytes) : size_t(n) * row_bytes);
 #pragma unroll
-  for (int i = 0; i < MT; ++i) acc[i] = 0.f;
+    for (int i = 0; i < MT; ++i) acc[i] = 0.f;
 
-  for (int k = lane; k < K; k += 32) {
-    const uint32_t u = load_field(Wrow, k, bits, d.w_layout, tiled);
-    const int gi = k / g;
-    T w;
-    if (d.with_zeros && d.zeros_mode == BB_ZEROS_QUANTIZED) {
-      const uint8_t* qz = reinterpret_cast<const uint8_t*>(zeros);
-      const int epb = 8 / bits;
-      const uint32_t z = (qz[size_t(gi) * (size_t(d.N) * bits / 8) + n / epb] >> (bits * (n % epb))) & ((1u << bits) - 1u);
-      w = cvt_int<T>(int(u) - int(z));
-    } else {
-      w = decode_value<T>(u, d.w_fmt, bits, lut);
-    }
-    if (d.with_scaling) {
-      const T s = scale[size_t(n) * G + gi];
-      if (!d.with_zeros || d.zeros_mode == BB_ZEROS_QUANTIZED) {
-        w = t_mul(w, s);
+    for (int k = lane; k < K; k += 32) {
+      const uint32_t u = load_field(Wrow, k, bits, d.w_layout, tiled);
+      const int gi = k / g;
+      T w;
+      if (d.with_zeros && d.zeros_mode == BB_ZEROS_QUANTIZED) {
+        const uint8_t* qz = reinterpret_cast<const uint8_t*>(zeros);
+        const int epb = 8 / bits;
+        const uint32_t z = (qz[size_t(gi) * (size_t(d.N) * bits / 8) + n / epb] >> (bits * (n % epb))) & ((1u << bits) - 1u);
+        w = cvt_int<T>(int(u) - int(z));
       } else {
-        const T z = reinterpret_cast<const T*>(zeros)[size_t(n) * G + gi];
-        if (d.zeros_mode == BB_ZEROS_ORIGINAL) w = t_mul(t_sub(w, z), s);
-        else if (use_fma) w = t_fma(w, s, __hneg(z));
-        else w = t_sub(t_mul(w, s), z);
+        w = decode_value<T>(u, d.w_fmt, bits, lut);
+      }
+      if (d.with_scaling) {
+        const T s = scale[size_t(n) * G + gi];
+        if (!d.with_zeros || d.zeros_mode == BB_ZEROS_QUANTIZED) {
+          w = t_mul(w, s);
+        } else {
+          const T z = reinterpret_cast<const T*>(zeros)[size_t(n) * G + gi];
+          if (d.zeros_mode == BB_ZEROS_ORIGINAL) w = t_mul(t_sub(w, z), s);
+          else if (use_fma) w = t_fma(w, s, __hneg(z));
+          else w = t_sub(t_mul(w, s), z);
+        }
+      }
+      const float wf = TypeTraits<T>::to_float(w);
+#pragma unroll
+      for (int i = 0; i < MT; ++i) {
+        if (m0 + i < M) acc[i] = fmaf(TypeTraits<T>::to_float(A[size_t(m0 + i) * K + k]), wf, acc[i]);
       }
     }
-    const float wf = TypeTraits<T>::to_float(w);
 #pragma unroll
     for (int i = 0; i < MT; ++i) {
-      if (m0 + i < M) acc[i] = fmaf(TypeTraits<T>::to_float(A[size_t(m0 + i) * K + k]), wf, acc[i]);
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], off);
     }
-  }
+  };
+  if constexpr (SWIGLU) {
+    const int ng = (n >> 3) * 16 + (n & 7), nu = ng + 8;
+    float ag[MT], au[MT];
+    row_dot(ng, ag);
+    row_dot(nu, au);
+    if (lane == 0) {
+      const bool hb = d.with_bias != 0;
+      const float bg = hb ? bias_as_float<T>(bias, ng) : 0.f, bu = hb ? bias_as_float<T>(bias, nu) : 0.f;
 #pragma unroll
-  for (int i = 0; i < MT; ++i) {
+      for (int i = 0; i < MT; ++i)
+        if (m0 + i < M)
+          store_swiglu(C, size_t(m0 + i) * (d.N / 2) + n, swiglu_operand(ag[i], hb, bg, d.out_dtype),
+                       swiglu_operand(au[i], hb, bu, d.out_dtype), d.out_dtype);
+    }
+  } else {
+    float acc[MT];
+    row_dot(n, acc);
+    if (lane == 0) {
 #pragma unroll
-    for (int off = 16; off > 0; off >>= 1) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], off);
-  }
-  if (lane == 0) {
-#pragma unroll
-    for (int i = 0; i < MT; ++i)
-      if (m0 + i < M) store_float_out<T>(C, d.out_dtype, size_t(m0 + i) * d.N + n, acc[i], d.with_bias ? bias : nullptr, n);
+      for (int i = 0; i < MT; ++i)
+        if (m0 + i < M) store_float_out<T>(C, d.out_dtype, size_t(m0 + i) * d.N + n, acc[i], d.with_bias ? bias : nullptr, n);
+    }
   }
 }
 
@@ -249,15 +271,18 @@ bool generic_supported(const bb_matmul_desc& d) {
 
 int launch_generic(const MatmulArgs& a) {
   const bb_matmul_desc& d = a.d;
-  dim3 grid((d.N + WARPS - 1) / WARPS, (a.m + MT - 1) / MT);
+  dim3 grid(((a.swiglu ? d.N / 2 : d.N) + WARPS - 1) / WARPS, (a.m + MT - 1) / MT);
   dim3 block(WARPS * 32);
+  auto run_float = [&](auto t) {
+    using T = typename decltype(t)::type;
+    auto kernel = a.swiglu ? generic_float_kernel<T, true> : generic_float_kernel<T, false>;
+    kernel<<<grid, block, 0, a.stream>>>(d, (const T*)a.A, (const uint8_t*)a.W, (const T*)a.lut, (const T*)a.scale, a.zeros, a.bias,
+                                         a.C, a.m);
+  };
   if (d.a_dtype == BB_F16) {
-    generic_float_kernel<__half><<<grid, block, 0, a.stream>>>(
-        d, (const __half*)a.A, (const uint8_t*)a.W, (const __half*)a.lut, (const __half*)a.scale, a.zeros, a.bias, a.C, a.m);
+    run_float(TypeTag<__half>{});
   } else if (d.a_dtype == BB_BF16) {
-    generic_float_kernel<__nv_bfloat16><<<grid, block, 0, a.stream>>>(
-        d, (const __nv_bfloat16*)a.A, (const uint8_t*)a.W, (const __nv_bfloat16*)a.lut, (const __nv_bfloat16*)a.scale,
-        a.zeros, a.bias, a.C, a.m);
+    run_float(TypeTag<__nv_bfloat16>{});
   } else {
     generic_int_kernel<<<grid, block, 0, a.stream>>>(d, (const int8_t*)a.A, (const uint8_t*)a.W, (const int8_t*)a.scale,
                                                       a.zeros, (const int8_t*)a.bias, a.C, a.m);

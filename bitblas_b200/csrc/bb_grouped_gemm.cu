@@ -60,24 +60,12 @@ __device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence
 
 // gemm_ts_kernel's epilogue for one destination and no split-K: acc[4i + 2h + j] = C^T[row rA + 8h][column 8i + 2t + j] ->
 // C[m, n] for the rows m < m_end, cast to out_dtype, then bias[e][n] added in out_dtype (fp32: in one sum), as bb_matmul rounds.
-// SWIGLU: rows nA = 16b + i and nB = nA + 8 (i < 8) are gate and up of C[m, 8b + i] = silu(gate) * up, row stride N / 2
+// SWIGLU: store_tile_swiglu (bb_gemm_ts.cuh)
 template <typename T, int BM, bool SWIGLU>
 __device__ __forceinline__ void store_tile(const float (&acc)[BM / 2], const TsParams& p, const T* bias, int m0, int m_end,
                                            int nA, int nB, int t) {
   if constexpr (SWIGLU) {
-    const float bg = bias ? TypeTraits<T>::to_float(bias[nA]) : 0.f, bu = bias ? TypeTraits<T>::to_float(bias[nB]) : 0.f;
-    const size_t col = size_t(nA >> 4) * 8 + size_t(nA & 7);
-#pragma unroll
-    for (int i = 0; i < BM / 8; ++i) {
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const int m = m0 + 8 * i + 2 * t + j;
-        if (m >= m_end) continue;
-        const float g = swiglu_operand(acc[4 * i + j], bias != nullptr, bg, p.out_dtype);
-        const float u = swiglu_operand(acc[4 * i + 2 + j], bias != nullptr, bu, p.out_dtype);
-        store_swiglu(p.out.ptr[0], size_t(m) * size_t(p.N / 2) + col, g, u, p.out_dtype);
-      }
-    }
+    store_tile_swiglu<T, BM>(acc, p, bias, m0, m_end, nA, nB, t);
   } else {
     float bias_f[2] = {0.f, 0.f};
     if (bias) {

@@ -65,6 +65,22 @@ def deinterleave_gate_up(fused: torch.Tensor, kind: str, bits: int = None):
     return gate, up
 
 
+def gate_up_act_order(gate, up, down, H: int, I: int, gate_up_group_size: int, down_group_size: int, bits: int, where: str = ""):
+    """The act-order rule of a SwiGLU gate/up/down triple of GPTQ modules (MoEExperts per expert, SwiGLUMLP): gate and up read
+    the same input, so they must carry the same g_idx (ValueError otherwise; `where` prefixes the message) and keep it as the
+    gate/up projection's column order.  The down projection's column order is absorbed: gate and up are returned with their
+    output rows in down's sorted K order (permute_gptq_rows), so silu(gate) * up arrives in the order down's sorted weight reads and
+    down needs no gather.  Returns (gate, up), the modules themselves when down is not act-order."""
+    pg, pu = (perm_from_g_idx(getattr(m, "g_idx", None), H, gate_up_group_size) for m in (gate, up))
+    if (pg is None) != (pu is None) or (pg is not None and not torch.equal(pg.cpu(), pu.cpu())):
+        raise ValueError(f"{where}gate and up have different g_idx; they read the same input, so act-order "
+                         "checkpoints must give them the same column order")
+    pd = perm_from_g_idx(getattr(down, "g_idx", None), I, down_group_size)
+    if pd is None:
+        return gate, up
+    return permute_gptq_rows(gate, pd, bits), permute_gptq_rows(up, pd, bits)
+
+
 def moe_route(topk_ids: torch.Tensor, x: torch.Tensor, num_experts: int):
     """Route the tokens of x [T, K] (fp16 / bf16) by topk_ids (int32 [T, k]) on the device, in one launch (bb_moe_route).
     Returns (offsets int32 [E + 1], slot_rows int32 [T*k], x_sorted [T*k, K]): slot t*k + j goes to sorted row slot_rows[t*k + j]
@@ -257,16 +273,9 @@ class MoEExperts(nn.Module):
             raise ValueError(f"expected {E} GPTQ modules per projection, got {len(gate_modules)}, {len(up_modules)}, {len(down_modules)}")
         gate_modules, up_modules = list(gate_modules), list(up_modules)
         for e in range(E):
-            pg, pu = (perm_from_g_idx(getattr(m[e], "g_idx", None), H, self.gate_up.group_size) for m in (gate_modules, up_modules))
-            if (pg is None) != (pu is None) or (pg is not None and not torch.equal(pg.cpu(), pu.cpu())):
-                raise ValueError(f"expert {e}: gate and up have different g_idx; they read the same input, so act-order "
-                                 "checkpoints must give them the same column order")
-            # the down projection's column order, absorbed into the gate/up output rows: h comes out in its sorted K order
-            pd = perm_from_g_idx(getattr(down_modules[e], "g_idx", None), I, self.down.group_size)
-            if pd is not None:
-                bits = self.gate_up.bits
-                gate_modules[e] = permute_gptq_rows(gate_modules[e], pd, bits)
-                up_modules[e] = permute_gptq_rows(up_modules[e], pd, bits)
+            gate_modules[e], up_modules[e] = gate_up_act_order(gate_modules[e], up_modules[e], down_modules[e], H, I,
+                                                               self.gate_up.group_size, self.down.group_size,
+                                                               self.gate_up.bits, f"expert {e}: ")
         kw = dict(self._linear_kwargs)
         bias = kw.pop("bias")
         halves = []
@@ -293,4 +302,5 @@ class MoEExperts(nn.Module):
         self._repack(gate_modules, up_modules, down_modules, device, v2=True)
 
 
-__all__ = ["MoEExperts", "moe_topk", "moe_route", "moe_route_index", "moe_combine", "interleave_gate_up", "deinterleave_gate_up"]
+__all__ = ["MoEExperts", "moe_topk", "moe_route", "moe_route_index", "moe_combine", "interleave_gate_up", "deinterleave_gate_up",
+           "gate_up_act_order"]

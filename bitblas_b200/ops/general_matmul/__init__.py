@@ -414,9 +414,8 @@ class Matmul(Operator):
             if t is not None and t.device != device:
                 raise ValueError(f"the layer's buffers must be on A's device {device} (a buffer is on {t.device})")
 
-    def _output_for(self, A, output):
+    def _output_for(self, A, output, N):
         """the output of A [.., K]: a new [.., N] tensor on A's device, or the caller's, checked to hold the m * N values"""
-        N = self.config.N
         if output is None:
             return torch.empty(A.shape[:-1] + (N,), dtype=self.torch_output_dtype, device=A.device)
         numel = A.numel() // self.config.K * N
@@ -430,9 +429,9 @@ class Matmul(Operator):
         output, ptrs = self._check_forward(A, W, scale, zeros, bias, output)
         return self._launch(A, ptrs, output)
 
-    def _check_forward(self, A, W, scale, zeros, bias, output):
-        """the checking half of forward(): validates every argument and launches nothing.  Returns the output and, for _launch,
-        the data pointers of W, scale, zeros and bias."""
+    def _check_forward(self, A, W, scale, zeros, bias, output, swiglu=False):
+        """the checking half of forward() (swiglu: of forward_swiglu, whose output has N / 2 columns): validates every argument
+        and launches nothing.  Returns the output and, for _launch, the data pointers of W, scale, zeros and bias."""
         c = self.config
         if not (A.is_cuda and A.dtype == self._torch_a_dtype and A.is_contiguous()):
             _lib.check_tensor(A, "A", self._torch_a_dtype)
@@ -449,22 +448,45 @@ class Matmul(Operator):
             raise ValueError(f"A has inner dimension {A.shape[-1]}, expected K={K}")
         if self.dynamic_range is None and A.numel() // K != int(c.M):
             raise ValueError(f"operator was created for static M={c.M}, got {A.numel() // K} rows")
-        return self._output_for(A, output), key
+        return self._output_for(A, output, c.N // 2 if swiglu else c.N), key
 
-    def _launch(self, A, ptrs, output):
-        """the launching half of forward(): A is the checked activations, or a column gather of them (Linear's act-order)"""
+    def _launch(self, A, ptrs, output, swiglu=False):
+        """the launching half of forward() (swiglu: of forward_swiglu): A is the checked activations, or a column gather of them
+        (Linear's and SwiGLUMLP's act-order)"""
         dev, idx, stream = _lib.device_stream(A)
         lut = self.lut
         if lut is not None and lut.device != dev:
             lut = self.lut = lut.to(dev)
         self._launch_raw(A.data_ptr(), ptrs[0], lut.data_ptr() if lut is not None else 0, ptrs[1], ptrs[2], ptrs[3],
-                        output.data_ptr(), A.numel() // self.config.K, idx, stream)
+                        output.data_ptr(), A.numel() // self.config.K, idx, stream, swiglu)
         return output
 
-    def _launch_raw(self, A, W, lut, scale, zeros, bias, C, m, device, stream):
-        """the package's one bb_matmul call: raw pointers (0 = absent), m rows, on the device of ordinal `device`"""
+    def _launch_raw(self, A, W, lut, scale, zeros, bias, C, m, device, stream, swiglu=False):
+        """the package's one bb_matmul (swiglu: bb_matmul_swiglu) call: raw pointers (0 = absent), m rows, on the device of
+        ordinal `device`"""
         ws_ptr, ws_bytes = self._workspace_for(m, device, stream)
-        _lib.call("bb_matmul", device, self._desc_ref, A, W, lut, scale, zeros, bias, C, m, ws_ptr, ws_bytes, stream)
+        _lib.call("bb_matmul_swiglu" if swiglu else "bb_matmul", device, self._desc_ref, A, W, lut, scale, zeros, bias, C, m,
+                  ws_ptr, ws_bytes, stream)
+
+    def check_swiglu(self) -> None:
+        """raise unless forward_swiglu covers this operator: NotImplementedError for a consistent (A_dtype == W_dtype) operator,
+        ValueError for int8 activations or N % 16 != 0 (the gate/up interleave moves blocks of 8 gate and 8 up rows)"""
+        if self.consistent:
+            raise NotImplementedError("forward_swiglu needs a low-bit weight operator")
+        c = self.config
+        if c.A_dtype == "int8":
+            raise ValueError("forward_swiglu needs float16 or bfloat16 activations (int8 is not supported)")
+        if c.N % 16:
+            raise ValueError(f"forward_swiglu needs N = 2I with I % 8 == 0 (gate/up interleave; N={c.N})")
+
+    def forward_swiglu(self, A, W, scale=None, zeros=None, bias=None, output=None):
+        """The gate/up projection of a dense SwiGLU MLP in one launch (bb_matmul_swiglu): this operator's N = 2I rows hold gate and
+        up in the gate/up interleave (bitblas_b200.moe.interleave_gate_up; scale, zeros and bias rows follow it), and the output
+        [.., I] is silu(gate) * up, formed in the kernel epilogue from exactly the values forward() would store for the two rows.
+        The kernel is the one forward() picks for the same m, with the same workspace.  Arguments as in forward()."""
+        self.check_swiglu()
+        output, ptrs = self._check_forward(A, W, scale, zeros, bias, output, swiglu=True)
+        return self._launch(A, ptrs, output, swiglu=True)
 
     def _workspace_for(self, m: int, device: int, stream: int):
         """scratch the kernel picked for `m` needs (bb_workspace_bytes: split-K partials, stream-K exchange slots); one cached,

@@ -134,6 +134,18 @@ int bb_matmul_scatter(const bb_matmul_desc* desc, const void* A, const void* W, 
                       const void* zeros, const void* bias, void* const* peer_C, int n_peers, int64_t ldc,
                       int64_t col_offset, int m, void* workspace, size_t workspace_bytes, void* stream);
 
+/* The gate/up projection of a dense SwiGLU MLP in one call: the operands, workspace, kernel choice (bb_select_kernel, the kernel
+ * override and the SM-count cap apply unchanged), launch count and stream semantics of bb_matmul, with desc->N = 2I fused gate/up
+ * rows stored in the gate/up interleave of the grouped SwiGLU calls below (stored row 16b + i is gate row 8b + i for i < 8 and up
+ * row 8b + i - 8 for i >= 8; scale, zeros and bias rows follow it, quantized zeros in whole bytes).  C is [m, I]:
+ *     C[r, 8b + i] = round_out(silu(g) * u),   silu(g) = g / (1 + exp(-g)) in fp32, one rounding,
+ * where g and u are exactly what bb_matmul stores for rows 16b + i and 16b + i + 8 (cast to out_dtype, bias added in out_dtype;
+ * fp32 output stays fp32).  Covers every desc bb_matmul accepts with fp16 / bf16 activations and N % 16 == 0; int8 activations
+ * and N % 16 != 0 are rejected.  m == 0 returns 0 and launches nothing. */
+int bb_matmul_swiglu(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
+                     const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes,
+                     void* stream);
+
 /* Grouped matmul for mixture-of-experts layers (no reference counterpart; the contract of torch._grouped_mm with offsets).
  * `num_groups` problems share `desc` and run as ONE kernel launch.  A[total_rows, K] holds the rows of every group, sorted so
  * that group e owns rows [offsets[e], offsets[e+1]); `offsets` is a DEVICE int32 array of num_groups + 1 entries, read by the
