@@ -267,17 +267,44 @@ static bool swiglu_shape_ok(const bb_matmul_desc* desc) {
   return true;
 }
 
-static int matmul_impl(bool swiglu, const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
-                       const void* zeros, const void* bias, void* C, void* const* peer_C, int n_peers, long long ldc,
-                       long long col_offset, int m, void* workspace, size_t workspace_bytes, void* stream) {
+// the descriptor checks of bb_matmul_scaled on top of validate(): int8 activations, a 16- or 32-bit float output, no group scales or
+// zeros (the weight's scale is w_scale)
+static bool scaled_desc_ok(const bb_matmul_desc* desc) {
+  if (desc->a_dtype != BB_I8) {
+    set_error("bb_matmul_scaled: needs int8 activations (a_dtype=%d; quantize 16-bit ones with bb_quantize_act_int8)", desc->a_dtype);
+    return false;
+  }
+  if (desc->out_dtype != BB_F16 && desc->out_dtype != BB_BF16 && desc->out_dtype != BB_F32) {
+    set_error("bb_matmul_scaled: out_dtype must be float16, bfloat16 or float32 (got %d)", desc->out_dtype);
+    return false;
+  }
+  if (desc->with_scaling) { set_error("bb_matmul_scaled: group scales are not supported (with_scaling must be 0; pass w_scale)"); return false; }
+  if (desc->with_zeros) { set_error("bb_matmul_scaled: zero points are not supported (with_zeros must be 0)"); return false; }
+  return true;
+}
+
+// scaled: bb_matmul_scaled's two scales (null for every other entry point)
+static int matmul_impl(bool swiglu, const ScaledArgs* scaled, const bb_matmul_desc* desc, const void* A, const void* W,
+                       const void* lut, const void* scale, const void* zeros, const void* bias, void* C, void* const* peer_C,
+                       int n_peers, long long ldc, long long col_offset, int m, void* workspace, size_t workspace_bytes,
+                       void* stream) {
   if (validate(desc)) return 1;
   if (swiglu) {
     if (desc->a_dtype == BB_I8) { set_error("bb_matmul_swiglu: int8 activations are not supported (float16 | bfloat16)"); return 1; }
     if (!swiglu_shape_ok(desc)) return 1;
   }
+  if (scaled && !scaled_desc_ok(desc)) return 1;
   if (m == 0) return 0;  // wrapper/tl.py:156-157
   if (m < 0) { set_error("m must be >= 0 (got %d)", m); return 1; }
   if (!A || !W || (!C && n_peers == 0)) { set_error("A, W and C must be non-null"); return 1; }
+  if (scaled) {
+    if (!scaled->a_scale) { set_error("bb_matmul_scaled: a_scale must be non-null (fp32 [m], one scale per row of A)"); return 1; }
+    if (!scaled->w_scale) { set_error("bb_matmul_scaled: w_scale must be non-null (fp32 [N], one scale per output column)"); return 1; }
+    if ((reinterpret_cast<uintptr_t>(scaled->a_scale) & 3) || (reinterpret_cast<uintptr_t>(scaled->w_scale) & 3)) {
+      set_error("bb_matmul_scaled: a_scale and w_scale must be 4-byte aligned");
+      return 5;
+    }
+  }
   if (n_peers < 0 || n_peers > BB_MAX_PEERS) { set_error("n_peers must be in [0, %d]", BB_MAX_PEERS); return 1; }
   if (n_peers > 0) {
     if (!peer_C) { set_error("peer_C is null"); return 1; }
@@ -294,6 +321,7 @@ static int matmul_impl(bool swiglu, const bb_matmul_desc* desc, const void* A, c
   for (int i = 0; i < BB_MAX_PEERS; ++i) a.peer_C[i] = (i < n_peers) ? peer_C[i] : nullptr;
   a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.stream = (cudaStream_t)stream;
   a.swiglu = swiglu;
+  if (scaled) a.scaled = *scaled;
   const int k = select(a.d, m);
   if (n_peers > 0 && k == BB_KERNEL_GENERIC) {
     set_error("the column-parallel scatter epilogue needs a fast kernel (gemv_mma / gemv_i8 / gemm_ts); this configuration dispatches to generic_simt");
@@ -314,20 +342,30 @@ static int matmul_impl(bool swiglu, const bb_matmul_desc* desc, const void* A, c
 int bb_matmul(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
               const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes,
               void* stream) {
-  return matmul_impl(false, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes, stream);
+  return matmul_impl(false, nullptr, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
+                     stream);
 }
 
 int bb_matmul_swiglu(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
                      const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes,
                      void* stream) {
-  return matmul_impl(true, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes, stream);
+  return matmul_impl(true, nullptr, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
+                     stream);
+}
+
+int bb_matmul_scaled(const bb_matmul_desc* desc, const void* A, const void* W, const float* a_scale, const float* w_scale,
+                     const void* bias, void* C, int m, void* workspace, size_t workspace_bytes, void* stream) {
+  ScaledArgs sc;
+  sc.a_scale = a_scale; sc.w_scale = w_scale;
+  return matmul_impl(false, &sc, desc, A, W, nullptr, nullptr, nullptr, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
+                     stream);
 }
 
 int bb_matmul_scatter(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
                       const void* zeros, const void* bias, void* const* peer_C, int n_peers, int64_t ldc,
                       int64_t col_offset, int m, void* workspace, size_t workspace_bytes, void* stream) {
   if (n_peers < 1) { set_error("bb_matmul_scatter needs n_peers >= 1"); return 1; }
-  return matmul_impl(false, desc, A, W, lut, scale, zeros, bias, nullptr, peer_C, n_peers, ldc, col_offset, m, workspace,
+  return matmul_impl(false, nullptr, desc, A, W, lut, scale, zeros, bias, nullptr, peer_C, n_peers, ldc, col_offset, m, workspace,
                      workspace_bytes, stream);
 }
 
@@ -560,6 +598,20 @@ int bb_permute_cols(const void* A, void* out, const int32_t* perm, int rows, int
     return 5;
   }
   return launch_permute_cols(A, out, perm, rows, K, num_groups, offsets, (cudaStream_t)stream);
+}
+
+int bb_quantize_act_int8(const void* x, int a_dtype, int rows, int K, int8_t* q, float* scale, void* stream) {
+  if (a_dtype != BB_F16 && a_dtype != BB_BF16) { set_error("quantize act int8: x must be float16 or bfloat16 (a_dtype=%d)", a_dtype); return 1; }
+  if (K <= 0 || K % 8) { set_error("quantize act int8: needs K > 0 and K %% 8 == 0 (K=%d)", K); return 1; }
+  if (rows < 0) { set_error("quantize act int8: rows must be >= 0 (got %d)", rows); return 1; }
+  if (rows == 0) return 0;
+  if (!x) { set_error("quantize act int8: x must be non-null"); return 1; }
+  if (!q) { set_error("quantize act int8: q must be non-null"); return 1; }
+  if (!scale) { set_error("quantize act int8: scale must be non-null"); return 1; }
+  if (reinterpret_cast<uintptr_t>(x) & 15) { set_error("quantize act int8: x must be 16-byte aligned"); return 5; }
+  if (reinterpret_cast<uintptr_t>(q) & 15) { set_error("quantize act int8: q must be 16-byte aligned"); return 5; }
+  if (reinterpret_cast<uintptr_t>(scale) & 3) { set_error("quantize act int8: scale must be 4-byte aligned"); return 5; }
+  return launch_quantize_act_int8(x, a_dtype, rows, K, q, scale, (cudaStream_t)stream);
 }
 
 int bb_peer_barrier(void* const* peer_flags, int n_peers, int rank, void* stream) {

@@ -39,6 +39,13 @@ extern std::atomic<uint64_t> g_launches;
     }                                                                                        \
   } while (0)
 
+// the two fp32 quantization scales of bb_matmul_scaled: a_scale [m] (the preceding kernel's output, read after the PDL wait) and
+// w_scale [N]; both null for every other call
+struct ScaledArgs {
+  const float* a_scale = nullptr;
+  const float* w_scale = nullptr;
+};
+
 struct MatmulArgs {
   bb_matmul_desc d;
   const void* A;
@@ -58,6 +65,8 @@ struct MatmulArgs {
   size_t workspace_bytes;
   cudaStream_t stream;
   bool swiglu;           // bb_matmul_swiglu: W holds gate/up interleaved (d.N = 2I rows), C is [m, d.N / 2] = silu(gate) * up
+  ScaledArgs scaled;     // bb_matmul_scaled (int8 activations): the dequantizing epilogue store_out_scaled
+  bool is_scaled() const { return scaled.a_scale != nullptr; }
   int groups() const { return d.K / (d.group_size <= 0 ? d.K : d.group_size); }
   int gsize() const { return d.group_size <= 0 ? d.K : d.group_size; }
 };
@@ -201,6 +210,8 @@ int launch_moe_topk(const void* logits, int logits_dtype, int num_tokens, int nu
 constexpr int PERMUTE_MAX_K = 112640;
 int launch_permute_cols(const void* A, void* out, const int32_t* perm, int rows, int K, int num_groups, const int32_t* offsets,
                         cudaStream_t stream);
+// per-token int8 quantization of the activations, bb_quant.cu (validated by bb_quantize_act_int8 in bb_api.cu)
+int launch_quantize_act_int8(const void* x, int a_dtype, int rows, int K, int8_t* q, float* scale, cudaStream_t stream);
 
 // bit position of logical element `o` (0 .. 32/bits-1) inside its 32-bit storage word, for each weight
 // layout (restates bitblas/quantization/utils.py:73-110 + testing/cpp/lop3_type_conversion/fast_decoding.hpp:30-95,607-668)
@@ -587,6 +598,22 @@ __device__ __forceinline__ void store_out_i32(void* C, size_t o, int v, int b, i
     case BB_F32: reinterpret_cast<float*>(C)[o] = float(v) + float(b); break;
     case BB_F16: reinterpret_cast<__half*>(C)[o] = __hadd(__int2half_rn(v), __int2half_rn(b)); break;
     default: reinterpret_cast<__nv_bfloat16*>(C)[o] = __hadd(__int2bfloat16_rn(v), __int2bfloat16_rn(b));
+  }
+}
+// The dequantizing epilogue of bb_matmul_scaled: C[o] = round_out((float(acc) / s_a) / s_w) with the bias element n (out_dtype, null:
+// none) added in out_dtype after the rounding; an fp32 output is one sum.  The scales are quantization scales (value x scale = the
+// integer grid), so both steps divide, in BitNet's order; __fdiv_rn keeps them correctly rounded whatever the compiler flags.
+__device__ __forceinline__ void store_out_scaled(void* C, size_t o, int acc, float s_a, float s_w, const void* bias, int n,
+                                                 int out_dtype) {
+  const float y = __fdiv_rn(__fdiv_rn(__int2float_rn(acc), s_a), s_w);
+  const bool hb = bias != nullptr;
+  if (out_dtype == BB_F16) {
+    reinterpret_cast<__half*>(C)[o] = round_out<__half>(y, hb, hb ? __half2float(reinterpret_cast<const __half*>(bias)[n]) : 0.f);
+  } else if (out_dtype == BB_BF16) {
+    reinterpret_cast<__nv_bfloat16*>(C)[o] =
+        round_out<__nv_bfloat16>(y, hb, hb ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(bias)[n]) : 0.f);
+  } else {
+    reinterpret_cast<float*>(C)[o] = round_out<float>(y, hb, hb ? reinterpret_cast<const float*>(bias)[n] : 0.f);
   }
 }
 

@@ -29,10 +29,13 @@ namespace {
 // FMT: 0 = integer formats (LOP3 magic-number decode), 1 = 16-entry table formats (NF4 / fp4; BITS = 4, compressed storage),
 //      2 = 8-bit float weights (e4m3 / e5m2; BITS = 8).  SWIGLU (16-bit activations only): bb_matmul_swiglu -- without split-K the
 //      epilogue is store_tile_swiglu; with it the raw partials are written as in the plain instance and splitk_reduce_kernel forms
-//      silu(gate) * up
-template <typename T, int BITS, int BM, bool IL, int FMT = 0, bool SWIGLU = false>
+//      silu(gate) * up.  SCALED (int8 activations only): bb_matmul_scaled -- without split-K the tile is stored through
+//      store_out_scaled; with it the raw int32 partials are written as in the plain instance and splitk_reduce_kernel scales them.
+//      The scales are a parameter of their own (null in every other instance): TsParams is also the grouped GEMM's.
+template <typename T, int BITS, int BM, bool IL, int FMT = 0, bool SWIGLU = false, bool SCALED = false>
 __global__ void __launch_bounds__(TS_THREADS, 1)
-gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const TsParams p) {
+gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const TsParams p,
+               const ScaledArgs sc) {
   using SM = TsSmem<T, BITS, BM>;
   using EI = ElemInfo<T>;
   constexpr int S = SM::kStages;
@@ -198,8 +201,25 @@ gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       return;
     }
   }
+  if constexpr (SCALED) {
+    if (p.splits == 1) {
+      const float swA = sc.w_scale[nA], swB = sc.w_scale[nB];
+#pragma unroll
+      for (int i = 0; i < BM / 8; ++i) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const int m = m0 + 8 * i + 2 * t + j;
+          if (m >= p.M) continue;
+          const float sa = sc.a_scale[m];
+          store_out_scaled(p.out.ptr[0], size_t(m) * p.N + nA, int(acc[4 * i + j]), sa, swA, p.bias, nA, p.out_dtype);
+          store_out_scaled(p.out.ptr[0], size_t(m) * p.N + nB, int(acc[4 * i + 2 + j]), sa, swB, p.bias, nB, p.out_dtype);
+        }
+      }
+      return;
+    }
+  }
   float bias_f[2] = {0.f, 0.f};
-  if (p.bias) {
+  if (!SCALED && p.bias) {   // (a scaled call's bias is out_dtype, read by splitk_reduce_scaled)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int n = h ? nB : nA;
@@ -292,13 +312,37 @@ __device__ __forceinline__ void splitk_reduce_swiglu(const TsParams& p) {
   }
 }
 
+// splitk_reduce_kernel of the SCALED int8 instances: the exact int32 sum of the partials through store_out_scaled, so split and
+// unsplit calls store the same bits
+__device__ __forceinline__ void splitk_reduce_scaled(const TsParams& p, const ScaledArgs& sc) {
+  const unsigned n4 = unsigned(p.N) >> 2;
+  const unsigned total4 = unsigned(p.M) * n4;
+  const size_t split_stride4 = size_t(p.M) * n4;
+  for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < total4; i += gridDim.x * blockDim.x) {
+    const unsigned m = i / n4, n = (i - m * n4) * 4u;
+    int acc[4] = {0, 0, 0, 0};
+    for (int sp = 0; sp < p.splits; ++sp) {
+      const int4 v = __ldcs(reinterpret_cast<const int4*>(p.ws) + size_t(sp) * split_stride4 + i);
+      acc[0] += v.x; acc[1] += v.y; acc[2] += v.z; acc[3] += v.w;
+    }
+    const float sa = sc.a_scale[m];
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      store_out_scaled(p.out.ptr[0], size_t(m) * p.N + n + j, acc[j], sa, sc.w_scale[n + j], p.bias, n + j, p.out_dtype);
+  }
+}
+
 // out[m, n] = cast(sum_s ws[s][m][n]) (+ bias), stored to every destination of the OutSpec.  One thread = 4 consecutive n
 // (N is a multiple of 128 here): 128-bit loads of the partials, 32-bit index arithmetic, one vector store per destination.
-// SWIGLU: splitk_reduce_swiglu.
-template <bool INT8, bool SWIGLU = false>
-__global__ void splitk_reduce_kernel(const TsParams p) {
+// SWIGLU: splitk_reduce_swiglu; SCALED: splitk_reduce_scaled.
+template <bool INT8, bool SWIGLU = false, bool SCALED = false>
+__global__ void splitk_reduce_kernel(const TsParams p, const ScaledArgs sc) {
   if constexpr (SWIGLU) {
     splitk_reduce_swiglu(p);
+    return;
+  }
+  if constexpr (SCALED) {
+    splitk_reduce_scaled(p, sc);
     return;
   }
   const unsigned n4 = unsigned(p.N) >> 2;                 // quads per row
@@ -412,11 +456,11 @@ int make_map_w_tiled(CUtensorMap* map, const void* base, uint64_t row_bytes, uin
   return 0;
 }
 
-template <typename T, int BITS, int BM, bool IL, int FMT, bool SWIGLU>
+template <typename T, int BITS, int BM, bool IL, int FMT, bool SWIGLU, bool SCALED>
 int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
   using SM = TsSmem<T, BITS, BM>;
   using EI = ElemInfo<T>;
-  auto kernel = gemm_ts_kernel<T, BITS, BM, IL, FMT, SWIGLU>;
+  auto kernel = gemm_ts_kernel<T, BITS, BM, IL, FMT, SWIGLU, SCALED>;
   static KernelCache<> cache;
   if (!kernel_setup(cache, kernel, SM::kTotal)) {
     set_error("gemm_ts: cannot raise the kernel's dynamic shared memory to %d bytes on this device", SM::kTotal);
@@ -446,34 +490,38 @@ int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
                         CU_TENSOR_MAP_SWIZZLE_NONE);
   if (rc) return rc;
   const int grid = tiles * p.splits;
-  kernel<<<grid, TS_THREADS, smem_bytes, a.stream>>>(tmA, tmW, p);
+  kernel<<<grid, TS_THREADS, smem_bytes, a.stream>>>(tmA, tmW, p, a.scaled);
   BB_LAUNCH_CHECK();
   if (p.splits > 1) {
     const size_t total = size_t(a.m) * a.d.N / (SWIGLU ? 8 : 4);   // one thread per 4 consecutive output columns
     const int rthreads = 256;
     const int rblocks = int(std::min<size_t>((total + rthreads - 1) / rthreads, size_t(device_sm_count()) * 8));
-    if (EI::kInt8) splitk_reduce_kernel<true><<<rblocks, rthreads, 0, a.stream>>>(p);
-    else if (SWIGLU) splitk_reduce_kernel<false, true><<<rblocks, rthreads, 0, a.stream>>>(p);
-    else splitk_reduce_kernel<false><<<rblocks, rthreads, 0, a.stream>>>(p);
+    if constexpr (SCALED) splitk_reduce_kernel<true, false, true><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
+    else if (EI::kInt8) splitk_reduce_kernel<true><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
+    else if (SWIGLU) splitk_reduce_kernel<false, true><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
+    else splitk_reduce_kernel<false><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
     BB_LAUNCH_CHECK();
   }
   return 0;
 }
 
 // activation rows per CTA: the wgmma N extent (m > 128 runs several 128-row tiles)
-template <typename T, int BITS, bool IL, int FMT, bool SWIGLU>
+template <typename T, int BITS, bool IL, int FMT, bool SWIGLU, bool SCALED>
 int launch_ts_bm_sw(const MatmulArgs& a, const TsParams& p) {
-  if (a.m <= 32) return launch_ts_inst<T, BITS, 32, IL, FMT, SWIGLU>(a, p);
-  if (a.m <= 64) return launch_ts_inst<T, BITS, 64, IL, FMT, SWIGLU>(a, p);
-  return launch_ts_inst<T, BITS, 128, IL, FMT, SWIGLU>(a, p);
+  if (a.m <= 32) return launch_ts_inst<T, BITS, 32, IL, FMT, SWIGLU, SCALED>(a, p);
+  if (a.m <= 64) return launch_ts_inst<T, BITS, 64, IL, FMT, SWIGLU, SCALED>(a, p);
+  return launch_ts_inst<T, BITS, 128, IL, FMT, SWIGLU, SCALED>(a, p);
 }
-// (the int8 instances have no SWIGLU form: bb_matmul_swiglu rejects int8 activations)
+// (the int8 instances have no SWIGLU form: bb_matmul_swiglu rejects int8 activations; only they have a SCALED form:
+// bb_matmul_scaled rejects 16-bit ones)
 template <typename T, int BITS, bool IL, int FMT>
 int launch_ts_bm(const MatmulArgs& a, const TsParams& p) {
   if constexpr (!std::is_same<T, int8_t>::value) {
-    if (a.swiglu) return launch_ts_bm_sw<T, BITS, IL, FMT, true>(a, p);
+    if (a.swiglu) return launch_ts_bm_sw<T, BITS, IL, FMT, true, false>(a, p);
+  } else {
+    if (a.is_scaled()) return launch_ts_bm_sw<T, BITS, IL, FMT, false, true>(a, p);
   }
-  return launch_ts_bm_sw<T, BITS, IL, FMT, false>(a, p);
+  return launch_ts_bm_sw<T, BITS, IL, FMT, false, false>(a, p);
 }
 template <typename T, int BITS>
 int launch_ts_layout(const MatmulArgs& a, const TsParams& p) {

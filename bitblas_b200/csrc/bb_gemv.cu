@@ -44,10 +44,12 @@ gemv_mma_kernel(const GemvParams p) {
 // int8 activations (W2A8 / W4A8), exact int32 accumulation.  Weights are used as raw unsigned fields
 // (mma .u8.s8); the constant zero point of the signed formats is removed with zp * sum_k(a), the sum
 // produced on the tensor cores with an all-ones A fragment.
+// SCALED: bb_matmul_scaled -- the epilogue divides by sc.a_scale[m] (read after the PDL wait) and sc.w_scale[n] (store_out_scaled;
+// bias in out_dtype).  The scales are a parameter of their own: GemvParams is also the grouped GEMV's, whose layout stays put.
 // ---------------------------------------------------------------------------------------------
-template <int BITS, int NT>
+template <int BITS, int NT, bool SCALED = false>
 __global__ void __launch_bounds__(gemv_max_ks(NT) * 32) __maxnreg__(NT == 1 ? 96 : (NT == 2 ? 128 : 208))
-gemv_i8_kernel(const GemvParams p) {
+gemv_i8_kernel(const GemvParams p, const ScaledArgs sc) {
   constexpr int WPS = BITS;            // words per thread per row per step (32 k)
   constexpr int STEP_BYTES = 16 * BITS;
   __shared__ int red[MAX_KS][16][8 * NT];
@@ -152,18 +154,23 @@ gemv_i8_kernel(const GemvParams p) {
     int v = 0;
     for (int w = 0; w < p.ks; ++w) v += red[w][row][m];
     const int n = rb * 16 + row;
+    if constexpr (SCALED) {
+      store_out_scaled(p.out.ptr[0], size_t(m) * size_t(p.out.ld) + n, v, sc.a_scale[m], sc.w_scale[n], p.bias, n,
+                       p.out_dtype);
+      continue;
+    }
     const int b = p.bias ? int(reinterpret_cast<const int8_t*>(p.bias)[n]) : 0;
     const size_t o = size_t(m) * size_t(p.out.ld) + size_t(p.out.col0) + n;
     for (int d = 0; d < p.out.n; ++d) store_out_i32(p.out.ptr[d], o, v, b, p.out_dtype);
   }
 }
 
-// one CTA per 16-row block, the K split from pick_ks
-template <int NT, typename Kernel>
-int launch_gemv_kernel(Kernel kernel, KernelCache<MAX_KS + 1>& cache, GemvParams p, cudaStream_t stream) {
+// one CTA per 16-row block, the K split from pick_ks; `extra` follows p in the kernel's parameters
+template <int NT, typename Kernel, typename... Extra>
+int launch_gemv_kernel(Kernel kernel, KernelCache<MAX_KS + 1>& cache, GemvParams p, cudaStream_t stream, const Extra&... extra) {
   const int nb = p.N / 16;
   p.ks = pick_ks(cache, kernel, gemv_max_ks(NT), nb, p.K / 128);
-  return launch_pdl(kernel, nb, p.ks * 32, 0, stream, pdl_enabled(), p);
+  return launch_pdl(kernel, nb, p.ks * 32, 0, stream, pdl_enabled(), p, extra...);
 }
 
 template <typename T, int BITS, bool IL, bool SWIGLU>
@@ -231,9 +238,12 @@ int launch_gemv_i8(const MatmulArgs& a) {
   const GemvParams p = make_params(a);
   return gemv_nt(p.M, [&](auto nt) {
     constexpr int NT = decltype(nt)::value;
-    static KernelCache<MAX_KS + 1> cache2, cache4;
-    return a.d.w_bits == 2 ? launch_gemv_kernel<NT>(gemv_i8_kernel<2, NT>, cache2, p, a.stream)
-                           : launch_gemv_kernel<NT>(gemv_i8_kernel<4, NT>, cache4, p, a.stream);
+    static KernelCache<MAX_KS + 1> cache2, cache4, cache2s, cache4s;
+    if (a.is_scaled())
+      return a.d.w_bits == 2 ? launch_gemv_kernel<NT>(gemv_i8_kernel<2, NT, true>, cache2s, p, a.stream, a.scaled)
+                             : launch_gemv_kernel<NT>(gemv_i8_kernel<4, NT, true>, cache4s, p, a.stream, a.scaled);
+    return a.d.w_bits == 2 ? launch_gemv_kernel<NT>(gemv_i8_kernel<2, NT>, cache2, p, a.stream, a.scaled)
+                           : launch_gemv_kernel<NT>(gemv_i8_kernel<4, NT>, cache4, p, a.stream, a.scaled);
   });
 }
 

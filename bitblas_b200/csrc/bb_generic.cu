@@ -195,11 +195,13 @@ generic_float_kernel(const bb_matmul_desc d, const T* __restrict__ A, const uint
   }
 }
 
-// int8 activations, exact int32 accumulate
+// int8 activations, exact int32 accumulate.  SCALED: bb_matmul_scaled -- store_out_scaled with a_scale [M], w_scale [N] and a bias
+// in out_dtype
+template <bool SCALED = false>
 __global__ void __launch_bounds__(WARPS * 32)
 generic_int_kernel(const bb_matmul_desc d, const int8_t* __restrict__ A, const uint8_t* __restrict__ W,
                    const int8_t* __restrict__ scale, const void* __restrict__ zeros,
-                   const int8_t* __restrict__ bias, void* __restrict__ C, int M) {
+                   const int8_t* __restrict__ bias, void* __restrict__ C, int M, const ScaledArgs sc) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n = blockIdx.x * WARPS + warp;
   const int m0 = blockIdx.y * MT;
@@ -248,6 +250,10 @@ generic_int_kernel(const bb_matmul_desc d, const int8_t* __restrict__ A, const u
     for (int i = 0; i < MT; ++i) {
       if (m0 + i >= M) continue;
       const size_t idx = size_t(m0 + i) * d.N + n;
+      if constexpr (SCALED) {
+        store_out_scaled(C, idx, acc[i], sc.a_scale[m0 + i], sc.w_scale[n], d.with_bias ? bias : nullptr, n, d.out_dtype);
+        continue;
+      }
       const int b = d.with_bias ? int(bias[n]) : 0;
       switch (d.out_dtype) {
         case BB_I32: reinterpret_cast<int*>(C)[idx] = acc[i] + b; break;
@@ -284,8 +290,9 @@ int launch_generic(const MatmulArgs& a) {
   } else if (d.a_dtype == BB_BF16) {
     run_float(TypeTag<__nv_bfloat16>{});
   } else {
-    generic_int_kernel<<<grid, block, 0, a.stream>>>(d, (const int8_t*)a.A, (const uint8_t*)a.W, (const int8_t*)a.scale,
-                                                      a.zeros, (const int8_t*)a.bias, a.C, a.m);
+    auto kernel = a.is_scaled() ? generic_int_kernel<true> : generic_int_kernel<false>;
+    kernel<<<grid, block, 0, a.stream>>>(d, (const int8_t*)a.A, (const uint8_t*)a.W, (const int8_t*)a.scale, a.zeros,
+                                         (const int8_t*)a.bias, a.C, a.m, a.scaled);
   }
   BB_LAUNCH_CHECK();
   return 0;

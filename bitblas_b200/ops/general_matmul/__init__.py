@@ -387,9 +387,10 @@ class Matmul(Operator):
         return input_tensor  # no ladder propagation on H100
 
     # ---- forward ------------------------------------------------------------------------------------
-    def _check_params(self, W, scale, zeros, bias, device):
+    def _check_params(self, W, scale, zeros, bias, device, scaled=False):
         """full validation of the (static) parameter tensors, all of them on `device` (A's: the kernel gets bare pointers);
-        forward() runs it once per distinct set of tensors."""
+        forward() runs it once per distinct set of tensors.  scaled (forward_scaled): `scale` is the fp32 [N] w_scale and the
+        bias is in the output dtype."""
         c = self.config
         adt = getattr(torch, c.A_dtype)
         wshape = self.retrieve_weight_shape()
@@ -409,8 +410,12 @@ class Matmul(Operator):
         if c.with_bias:
             if bias is None:
                 raise ValueError("with_bias=True but bias is None")
-            _lib.check_tensor(bias, "bias", adt, numel=c.N)
-        for t in (W, scale if c.with_scaling else None, zeros if c.with_zeros else None, bias if c.with_bias else None):
+            _lib.check_tensor(bias, "bias", self.torch_output_dtype if scaled else adt, numel=c.N)
+        if scaled:
+            if scale is None:
+                raise ValueError("forward_scaled needs w_scale (float32 [N])")
+            _lib.check_tensor(scale, "w_scale", torch.float32, numel=c.N)
+        for t in (W, scale if c.with_scaling or scaled else None, zeros if c.with_zeros else None, bias if c.with_bias else None):
             if t is not None and t.device != device:
                 raise ValueError(f"the layer's buffers must be on A's device {device} (a buffer is on {t.device})")
 
@@ -429,9 +434,10 @@ class Matmul(Operator):
         output, ptrs = self._check_forward(A, W, scale, zeros, bias, output)
         return self._launch(A, ptrs, output)
 
-    def _check_forward(self, A, W, scale, zeros, bias, output, swiglu=False):
-        """the checking half of forward() (swiglu: of forward_swiglu, whose output has N / 2 columns): validates every argument
-        and launches nothing.  Returns the output and, for _launch, the data pointers of W, scale, zeros and bias."""
+    def _check_forward(self, A, W, scale, zeros, bias, output, swiglu=False, scaled=False):
+        """the checking half of forward() (swiglu: of forward_swiglu, whose output has N / 2 columns; scaled: of forward_scaled,
+        with `scale` the w_scale): validates every argument and launches nothing.  Returns the output and, for _launch, the data
+        pointers of W, scale, zeros and bias."""
         c = self.config
         if not (A.is_cuda and A.dtype == self._torch_a_dtype and A.is_contiguous()):
             _lib.check_tensor(A, "A", self._torch_a_dtype)
@@ -439,9 +445,9 @@ class Matmul(Operator):
         # pointers and A's device; a new tensor -- or a re-allocated one -- is validated again).  The activations are checked
         # every call.
         key = (W.data_ptr(), scale.data_ptr() if scale is not None else 0, zeros.data_ptr() if zeros is not None else 0,
-               bias.data_ptr() if bias is not None else 0, A.device)
+               bias.data_ptr() if bias is not None else 0, A.device, scaled)
         if key != self._checked_key:
-            self._check_params(W, scale, zeros, bias, A.device)
+            self._check_params(W, scale, zeros, bias, A.device, scaled)
             self._checked_key = key
         K = c.K
         if A.shape[-1] != K:
@@ -461,10 +467,13 @@ class Matmul(Operator):
                         output.data_ptr(), A.numel() // self.config.K, idx, stream, swiglu)
         return output
 
-    def _launch_raw(self, A, W, lut, scale, zeros, bias, C, m, device, stream, swiglu=False):
-        """the package's one bb_matmul (swiglu: bb_matmul_swiglu) call: raw pointers (0 = absent), m rows, on the device of
-        ordinal `device`"""
+    def _launch_raw(self, A, W, lut, scale, zeros, bias, C, m, device, stream, swiglu=False, a_scale=None):
+        """the package's one bb_matmul (swiglu: bb_matmul_swiglu; a_scale, the pointer of the fp32 [m] activation scales:
+        bb_matmul_scaled with `scale` the w_scale) call: raw pointers (0 = absent), m rows, on the device of ordinal `device`"""
         ws_ptr, ws_bytes = self._workspace_for(m, device, stream)
+        if a_scale is not None:
+            _lib.call("bb_matmul_scaled", device, self._desc_ref, A, W, a_scale, scale, bias, C, m, ws_ptr, ws_bytes, stream)
+            return
         _lib.call("bb_matmul_swiglu" if swiglu else "bb_matmul", device, self._desc_ref, A, W, lut, scale, zeros, bias, C, m,
                   ws_ptr, ws_bytes, stream)
 
@@ -487,6 +496,40 @@ class Matmul(Operator):
         self.check_swiglu()
         output, ptrs = self._check_forward(A, W, scale, zeros, bias, output, swiglu=True)
         return self._launch(A, ptrs, output, swiglu=True)
+
+    def check_scaled(self) -> None:
+        """raise unless forward_scaled covers this operator: NotImplementedError for a consistent (A_dtype == W_dtype) operator,
+        ValueError for 16-bit activations, an integer out_dtype, or group scales / zeros (the weight's scale is w_scale)"""
+        if self.consistent:
+            raise NotImplementedError("forward_scaled needs a low-bit weight operator")
+        c = self.config
+        if c.A_dtype != "int8":
+            raise ValueError(f"forward_scaled needs int8 activations (A_dtype={c.A_dtype}; quantize_act_int8 makes them from "
+                             "float16 / bfloat16)")
+        if c.out_dtype not in ("float16", "bfloat16", "float32"):
+            raise ValueError(f"forward_scaled needs out_dtype float16, bfloat16 or float32 (got {c.out_dtype})")
+        if c.with_scaling or c.with_zeros:
+            raise ValueError("forward_scaled takes the weight's scale as w_scale: the operator needs with_scaling=False and "
+                             "with_zeros=False")
+
+    def forward_scaled(self, A, W, a_scale, w_scale, bias=None, output=None):
+        """The int8 matmul with a dequantizing epilogue in one launch (bb_matmul_scaled; two with split-K): A int8 [.., K] (e.g.
+        from quantize_act_int8), a_scale float32 [m] one quantization scale per row of A, w_scale float32 [N] one per output
+        row of W, and output [.., N] = round((float(acc) / a_scale[r]) / w_scale[n]) (+ bias, [N] in the output dtype, added
+        after the rounding), acc the exact int32 sum forward() forms.  The kernel is the one forward() picks for the same m,
+        with the same workspace."""
+        self.check_scaled()
+        output, ptrs = self._check_forward(A, W, w_scale, None, bias, output, scaled=True)
+        m = A.numel() // self.config.K
+        if not (isinstance(a_scale, torch.Tensor) and a_scale.is_cuda and a_scale.dtype == torch.float32
+                and a_scale.is_contiguous() and a_scale.numel() == m):
+            _lib.check_tensor(a_scale, "a_scale", torch.float32, numel=m)
+        if a_scale.device != A.device:
+            raise ValueError(f"a_scale must be on A's device {A.device} (got {a_scale.device})")
+        _, idx, stream = _lib.device_stream(A)
+        self._launch_raw(A.data_ptr(), ptrs[0], 0, ptrs[1], 0, ptrs[3], output.data_ptr(), m, idx, stream,
+                         a_scale=a_scale.data_ptr())
+        return output
 
     def _workspace_for(self, m: int, device: int, stream: int):
         """scratch the kernel picked for `m` needs (bb_workspace_bytes: split-K partials, stream-K exchange slots); one cached,

@@ -146,6 +146,33 @@ int bb_matmul_swiglu(const bb_matmul_desc* desc, const void* A, const void* W, c
                      const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes,
                      void* stream);
 
+/* BitNet b1.58 layers from 16-bit activations: bb_quantize_act_int8 quantizes each row of x to int8 with its own scale, and
+ * bb_matmul_scaled runs the int8 matmul of those rows with an epilogue that undoes both quantization scales.  Every operation is
+ * in fp32 and correctly rounded, so results are reproducible bit for bit.
+ *
+ * bb_quantize_act_int8: x [rows, K] of a_dtype (float16 | bfloat16) -> q int8 [rows, K] and scale fp32 [rows], per row r:
+ *     amax     = max_k |float(x[r, k])|                                   (exact)
+ *     scale[r] = 127.0f * (1.0f / max(amax, 1e-5f))                      (IEEE reciprocal, then IEEE product)
+ *     q[r, k]  = int8(clamp(rint(float(x[r, k]) * scale[r]), -128, 127))  (IEEE product, then round half to even)
+ * (BitNet's activation_quant exactly as torch evaluates it: `127.0 / t` is reciprocal(t) * 127 there; an all-zero row gives scale 1.27e7 and q = 0; a row holding Inf or NaN gives unspecified values.)
+ * K % 8 == 0; x and q 16-byte aligned, scale 4-byte aligned (code 5 otherwise).  ONE launch, no workspace, no host
+ * synchronisation (CUDA-graph capturable); programmatic stream serialization: x is read only after the preceding kernel has
+ * completed, and the next kernel may launch once this one has stored its results.  rows == 0 validates and returns 0 without
+ * touching the device.
+ *
+ * bb_matmul_scaled: the int8 matmul of bb_matmul (A int8 [m, K] x W, exact int32 accumulation acc) with a dequantizing epilogue
+ *     C[r, n] = round_out((float(acc[r, n]) / a_scale[r]) / w_scale[n])   (+ bias[n], added in out_dtype after the rounding)
+ * with float(acc) round-to-nearest and both divisions IEEE; an fp32 output is (...) + bias in fp32.  a_scale is fp32 [m] (the
+ * scale of bb_quantize_act_int8), w_scale fp32 [N] (one quantization scale per output row of W; a per-tensor scale is N copies),
+ * both 4-byte aligned; bias, when desc->with_bias, is [N] in out_dtype.  Covers every desc bb_matmul accepts with a_dtype ==
+ * BB_I8, out_dtype float16 | bfloat16 | float32 and with_scaling == with_zeros == 0; everything else is rejected, each with its own
+ * message, in bb_matmul's order (descriptor, then m, then pointers).  Kernel choice (bb_select_kernel, the kernel override, the
+ * SM-count cap), bb_workspace_bytes, launch count and stream semantics are those of bb_matmul for the same desc; m == 0 returns 0
+ * and launches nothing.  a_scale, like A, is read only after the preceding kernel has completed. */
+int bb_quantize_act_int8(const void* x, int a_dtype, int rows, int K, int8_t* q, float* scale, void* stream);
+int bb_matmul_scaled(const bb_matmul_desc* desc, const void* A, const void* W, const float* a_scale, const float* w_scale,
+                     const void* bias, void* C, int m, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Grouped matmul for mixture-of-experts layers (no reference counterpart; the contract of torch._grouped_mm with offsets).
  * `num_groups` problems share `desc` and run as ONE kernel launch.  A[total_rows, K] holds the rows of every group, sorted so
  * that group e owns rows [offsets[e], offsets[e+1]); `offsets` is a DEVICE int32 array of num_groups + 1 entries, read by the
