@@ -277,6 +277,12 @@ bool generic_supported(const bb_matmul_desc& d) {
 
 int launch_generic(const MatmulArgs& a) {
   const bb_matmul_desc& d = a.d;
+  // load_field reads sub-byte weights as whole 32-bit words (every row starts on one: K * bits % 32 == 0), so only the base
+  // pointer can break their alignment; everything else is read element by element
+  if (d.w_bits < 8 && (reinterpret_cast<uintptr_t>(a.W) & 3)) {
+    set_error("generic_simt: W must be 4-byte aligned for %d-bit weights (they are read as 32-bit words)", d.w_bits);
+    return 5;
+  }
   dim3 grid(((a.swiglu ? d.N / 2 : d.N) + WARPS - 1) / WARPS, (a.m + MT - 1) / MT);
   dim3 block(WARPS * 32);
   auto run_float = [&](auto t) {

@@ -186,7 +186,9 @@ def _decoded(case):
             return u.to(torch.uint8).view(torch.int8).double()
         return (u - 2 ** (bit - 1)).double()
     adt = O.TORCH_DTYPE[case["cfg"]["A_dtype"]]
-    lut = torch.tensor(O.NF4_LUT, dtype=adt) if fmt == "nf" else None
+    lut = None
+    if fmt == "nf":   # the operator's table: the standard NF4 one unless the case carries its own 16 entries
+        lut = case["lut"].to(adt) if case.get("lut") is not None else torch.tensor(O.NF4_LUT, dtype=adt)
     return O.decode_fields(u.to(torch.int32), fmt, bit, adt, lut).double()
 
 
@@ -248,7 +250,9 @@ def _ulp(x, dtype):
     return torch.pow(2.0, torch.clamp(e, min=emin) - mant)
 
 
-def check_float(got, case, rule, what, layout_il=False, rows=None):
+def float_reference(case, rule, layout_il=False, rows=None):
+    """(reference, per-element bound) of the float output by the family's rule: what check_float compares with, computed once
+    where several kernels of one rule run the same case"""
     A = case["A"] if rows is None else case["A"][rows]
     W = dequant(case, rule, layout_il)
     A64 = A.double()
@@ -264,8 +268,14 @@ def check_float(got, case, rule, what, layout_il=False, rows=None):
         mag = torch.maximum(torch.maximum(ref.abs(), ref_nb.abs()), b.abs().expand_as(ref))
         k_out = 2.0
     odt = O.TORCH_DTYPE[out]
-    assert torch.isfinite(ref.to(odt).float()).all(), f"{what}: reference not finite in {out}"
-    bound = k_out * _ulp(mag, out) + C_ACC[rule] * EPS32 * acc
+    assert torch.isfinite(ref.to(odt).float()).all(), f"reference not finite in {out}"
+    return ref, k_out * _ulp(mag, out) + C_ACC[rule] * EPS32 * acc
+
+
+def check_float(got, case, rule, what, layout_il=False, rows=None, reference=None):
+    """got against float_reference(case, rule, layout_il, rows), or the `reference` pair already computed for it"""
+    ref, bound = reference if reference is not None else float_reference(case, rule, layout_il, rows)
+    out = case["cfg"]["out_dtype"]
     g = got.double()
     err = (g - ref).abs()
     bad = ~(err <= bound)
