@@ -283,8 +283,45 @@ static bool scaled_desc_ok(const bb_matmul_desc* desc) {
   return true;
 }
 
-// scaled: bb_matmul_scaled's two scales (null for every other entry point)
-static int matmul_impl(bool swiglu, const ScaledArgs* scaled, const bb_matmul_desc* desc, const void* A, const void* W,
+// the descriptor checks of bb_matmul_w4a8 on top of validate(), in the order of scaled_desc_ok
+static bool w4a8_desc_ok(const bb_matmul_desc* desc) {
+  if (desc->a_dtype != BB_I8) {
+    set_error("bb_matmul_w4a8: needs int8 activations (a_dtype=%d; quantize 16-bit ones with bb_quantize_act_int8)", desc->a_dtype);
+    return false;
+  }
+  if (desc->out_dtype != BB_F16 && desc->out_dtype != BB_BF16 && desc->out_dtype != BB_F32) {
+    set_error("bb_matmul_w4a8: out_dtype must be float16, bfloat16 or float32 (got %d)", desc->out_dtype);
+    return false;
+  }
+  if (!desc->with_scaling) { set_error("bb_matmul_w4a8: needs with_scaling = 1 (fp32 group scales [N, K/g])"); return false; }
+  if (desc->with_zeros && desc->zeros_mode != BB_ZEROS_QUANTIZED) {
+    set_error("bb_matmul_w4a8: zero points must be BB_ZEROS_QUANTIZED (packed [K/g, N/2]; got zeros_mode=%d)", desc->zeros_mode);
+    return false;
+  }
+  if (desc->w_bits != 4 || (desc->w_fmt != BB_W_UINT && desc->w_fmt != BB_W_INT)) {
+    set_error("bb_matmul_w4a8: needs 4-bit uint or int weights (w_bits=%d, w_fmt=%d)", desc->w_bits, desc->w_fmt);
+    return false;
+  }
+  if (desc->with_zeros && desc->w_fmt == BB_W_INT) { set_error("bb_matmul_w4a8: int weights take no zero points"); return false; }
+  return true;
+}
+
+// bb_matmul_w4a8's kernel: the family select() picks for the descriptor without group scales and zeros (so its workspace is
+// bb_workspace_bytes of that descriptor), with gemv_i8 and gemm_ts_i8 replaced by generic_simt when g is not a multiple of 128
+// (their 128-k steps and k-blocks must not straddle a group); under a kernel override forcing one of the two, such a g is not
+// supported (-1)
+static int select_w4a8(const bb_matmul_desc& d, int m) {
+  bb_matmul_desc c = d;
+  c.with_scaling = c.with_zeros = 0;
+  const int k = select(c, m);
+  const int g = d.group_size <= 0 ? d.K : d.group_size;
+  if ((k == BB_KERNEL_GEMV_I8 || k == BB_KERNEL_GEMM_TS_I8) && g % 128)
+    return g_override.load() == BB_KERNEL_AUTO ? BB_KERNEL_GENERIC : -1;
+  return k;
+}
+
+// scaled: bb_matmul_scaled's two scales, or (w4a8) bb_matmul_w4a8's a_scale and group scales (null for every other entry point)
+static int matmul_impl(bool swiglu, const ScaledArgs* scaled, bool w4a8, const bb_matmul_desc* desc, const void* A, const void* W,
                        const void* lut, const void* scale, const void* zeros, const void* bias, void* C, void* const* peer_C,
                        int n_peers, long long ldc, long long col_offset, int m, void* workspace, size_t workspace_bytes,
                        void* stream) {
@@ -293,11 +330,18 @@ static int matmul_impl(bool swiglu, const ScaledArgs* scaled, const bb_matmul_de
     if (desc->a_dtype == BB_I8) { set_error("bb_matmul_swiglu: int8 activations are not supported (float16 | bfloat16)"); return 1; }
     if (!swiglu_shape_ok(desc)) return 1;
   }
-  if (scaled && !scaled_desc_ok(desc)) return 1;
+  if (scaled && !(w4a8 ? w4a8_desc_ok(desc) : scaled_desc_ok(desc))) return 1;
   if (m == 0) return 0;  // wrapper/tl.py:156-157
   if (m < 0) { set_error("m must be >= 0 (got %d)", m); return 1; }
   if (!A || !W || (!C && n_peers == 0)) { set_error("A, W and C must be non-null"); return 1; }
-  if (scaled) {
+  if (w4a8) {
+    if (!scaled->a_scale) { set_error("bb_matmul_w4a8: a_scale must be non-null (fp32 [m], one scale per row of A)"); return 1; }
+    if (!scaled->w_scale) { set_error("bb_matmul_w4a8: scale must be non-null (fp32 [N, K/g] group scales)"); return 1; }
+    if ((reinterpret_cast<uintptr_t>(scaled->a_scale) & 3) || (reinterpret_cast<uintptr_t>(scaled->w_scale) & 3)) {
+      set_error("bb_matmul_w4a8: a_scale and scale must be 4-byte aligned");
+      return 5;
+    }
+  } else if (scaled) {
     if (!scaled->a_scale) { set_error("bb_matmul_scaled: a_scale must be non-null (fp32 [m], one scale per row of A)"); return 1; }
     if (!scaled->w_scale) { set_error("bb_matmul_scaled: w_scale must be non-null (fp32 [N], one scale per output column)"); return 1; }
     if ((reinterpret_cast<uintptr_t>(scaled->a_scale) & 3) || (reinterpret_cast<uintptr_t>(scaled->w_scale) & 3)) {
@@ -322,7 +366,8 @@ static int matmul_impl(bool swiglu, const ScaledArgs* scaled, const bb_matmul_de
   a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.stream = (cudaStream_t)stream;
   a.swiglu = swiglu;
   if (scaled) a.scaled = *scaled;
-  const int k = select(a.d, m);
+  a.w4a8 = w4a8;
+  const int k = w4a8 ? select_w4a8(a.d, m) : select(a.d, m);
   if (n_peers > 0 && k == BB_KERNEL_GENERIC) {
     set_error("the column-parallel scatter epilogue needs a fast kernel (gemv_mma / gemv_i8 / gemm_ts); this configuration dispatches to generic_simt");
     return 1;
@@ -342,14 +387,14 @@ static int matmul_impl(bool swiglu, const ScaledArgs* scaled, const bb_matmul_de
 int bb_matmul(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
               const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes,
               void* stream) {
-  return matmul_impl(false, nullptr, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
+  return matmul_impl(false, nullptr, false, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
                      stream);
 }
 
 int bb_matmul_swiglu(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
                      const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes,
                      void* stream) {
-  return matmul_impl(true, nullptr, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
+  return matmul_impl(true, nullptr, false, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
                      stream);
 }
 
@@ -357,15 +402,28 @@ int bb_matmul_scaled(const bb_matmul_desc* desc, const void* A, const void* W, c
                      const void* bias, void* C, int m, void* workspace, size_t workspace_bytes, void* stream) {
   ScaledArgs sc;
   sc.a_scale = a_scale; sc.w_scale = w_scale;
-  return matmul_impl(false, &sc, desc, A, W, nullptr, nullptr, nullptr, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
+  return matmul_impl(false, &sc, false, desc, A, W, nullptr, nullptr, nullptr, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
                      stream);
+}
+
+int bb_matmul_w4a8(const bb_matmul_desc* desc, const void* A, const void* W, const float* a_scale, const float* scale,
+                   const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes, void* stream) {
+  ScaledArgs sc;
+  sc.a_scale = a_scale; sc.w_scale = scale;
+  return matmul_impl(false, &sc, true, desc, A, W, nullptr, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
+                     stream);
+}
+
+int bb_select_kernel_w4a8(const bb_matmul_desc* desc, int m) {
+  if (validate(desc) || !w4a8_desc_ok(desc)) return -1;
+  return select_w4a8(*desc, m);
 }
 
 int bb_matmul_scatter(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
                       const void* zeros, const void* bias, void* const* peer_C, int n_peers, int64_t ldc,
                       int64_t col_offset, int m, void* workspace, size_t workspace_bytes, void* stream) {
   if (n_peers < 1) { set_error("bb_matmul_scatter needs n_peers >= 1"); return 1; }
-  return matmul_impl(false, nullptr, desc, A, W, lut, scale, zeros, bias, nullptr, peer_C, n_peers, ldc, col_offset, m, workspace,
+  return matmul_impl(false, nullptr, false, desc, A, W, lut, scale, zeros, bias, nullptr, peer_C, n_peers, ldc, col_offset, m, workspace,
                      workspace_bytes, stream);
 }
 

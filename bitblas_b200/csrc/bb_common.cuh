@@ -66,6 +66,8 @@ struct MatmulArgs {
   cudaStream_t stream;
   bool swiglu;           // bb_matmul_swiglu: W holds gate/up interleaved (d.N = 2I rows), C is [m, d.N / 2] = silu(gate) * up
   ScaledArgs scaled;     // bb_matmul_scaled (int8 activations): the dequantizing epilogue store_out_scaled
+  // bb_matmul_w4a8: per-group fp32 weight scales; `scaled` then holds a_scale [m] and, as w_scale, the group scales [N, K/g]
+  bool w4a8 = false;
   bool is_scaled() const { return scaled.a_scale != nullptr; }
   int groups() const { return d.K / (d.group_size <= 0 ? d.K : d.group_size); }
   int gsize() const { return d.group_size <= 0 ? d.K : d.group_size; }
@@ -615,6 +617,27 @@ __device__ __forceinline__ void store_out_scaled(void* C, size_t o, int acc, flo
   } else {
     reinterpret_cast<float*>(C)[o] = round_out<float>(y, hb, hb ? reinterpret_cast<const float*>(bias)[n] : 0.f);
   }
+}
+
+// The epilogue of bb_matmul_w4a8: C[o] = round_out(y) with y = S / a_scale[r] already divided (__fdiv_rn), the bias element n
+// (out_dtype, null: none) added in out_dtype after the rounding; an fp32 output is one sum
+__device__ __forceinline__ void store_out_dequant(void* C, size_t o, float y, const void* bias, int n, int out_dtype) {
+  const bool hb = bias != nullptr;
+  if (out_dtype == BB_F16) {
+    reinterpret_cast<__half*>(C)[o] = round_out<__half>(y, hb, hb ? __half2float(reinterpret_cast<const __half*>(bias)[n]) : 0.f);
+  } else if (out_dtype == BB_BF16) {
+    reinterpret_cast<__nv_bfloat16*>(C)[o] =
+        round_out<__nv_bfloat16>(y, hb, hb ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(bias)[n]) : 0.f);
+  } else {
+    reinterpret_cast<float*>(C)[o] = round_out<float>(y, hb, hb ? reinterpret_cast<const float*>(bias)[n] : 0.f);
+  }
+}
+// one group's promotion in bb_matmul_w4a8: S + float(acc) * s, each step rounded to nearest (never contracted into an fma)
+__device__ __forceinline__ float w4a8_promote(float S, int acc, float s) { return __fadd_rn(S, __fmul_rn(__int2float_rn(acc), s)); }
+// the zero point of 4-bit weight row n in group gi: its nibble of the packed quantized zeros [G, N / 2], or z_const (8 for int
+// weights, 0 for uint weights without zeros) when qz is null
+__device__ __forceinline__ int w4a8_zero(const uint8_t* qz, int N, int gi, int n, int z_const) {
+  return qz ? int((__ldg(qz + size_t(gi) * (size_t(N) / 2) + n / 2) >> (4 * (n & 1))) & 15u) : z_const;
 }
 
 // ---- SwiGLU epilogue of bb_matmul_swiglu and the grouped SwiGLU calls (gate/up interleave: weight row 16b + i is gate row 8b + i for

@@ -32,7 +32,10 @@ namespace {
 //      silu(gate) * up.  SCALED (int8 activations only): bb_matmul_scaled -- without split-K the tile is stored through
 //      store_out_scaled; with it the raw int32 partials are written as in the plain instance and splitk_reduce_kernel scales them.
 //      The scales are a parameter of their own (null in every other instance): TsParams is also the grouped GEMM's.
-template <typename T, int BITS, int BM, bool IL, int FMT = 0, bool SWIGLU = false, bool SCALED = false>
+//      W4A8 (int8 activations, 4-bit weights): bb_matmul_w4a8 -- per-group fp32 scales (sc.w_scale [N, G]) and zero points,
+//      promoted from exact int32 group sums into fp32 (main loop below); the tile, or the split's fp32 partial, ends in
+//      store_out_dequant / splitk_reduce_w4a8.
+template <typename T, int BITS, int BM, bool IL, int FMT = 0, bool SWIGLU = false, bool SCALED = false, bool W4A8 = false>
 __global__ void __launch_bounds__(TS_THREADS, 1)
 gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const TsParams p,
                const ScaledArgs sc) {
@@ -105,6 +108,100 @@ gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const bool e5m2 = p.w_fmt == BB_W_FP8_E5M2;
   const uint32_t zp4 = uint32_t(p.zp_const) * 0x01010101u;
   const uint32_t srcA = smem_u32(sW) + uint32_t(rA * PRB), srcB = srcA + 8u * PRB;
+
+  if constexpr (W4A8) {
+    // Each group's k-blocks accumulate, exactly, into acc; the first wgmma of a group overwrites it (scale-d = 0).  Every k-block
+    // decodes its fragments while the previous k-block's MMAs run, then wait<0> retires those MMAs; at a group's first k-block
+    // the finished group is promoted into facc with its scale, and the new MMAs are issued.  So one k-block's MMAs are in flight
+    // during each decode, and the tensor pipe drains once per k-block (at g = 128 every k-block closes a group anyway).  The
+    // loop body is the same for every k-block: whether it opens a group only selects values (the promotion, scale-d).  A branch
+    // on it, or on the group size, around the wait or the wgmmas makes ptxas serialize every wgmma (C7515 / C7520).  A split
+    // starts on a group boundary (launch_ts_inst).
+    float facc[BM / 2];
+#pragma unroll
+    for (int i = 0; i < BM / 2; ++i) facc[i] = 0.f;
+    const float* scA = sc.w_scale + size_t(nA) * p.G;
+    const float* scB = sc.w_scale + size_t(nB) * p.G;
+    const uint8_t* qz = reinterpret_cast<const uint8_t*>(p.zeros);
+    const int kpg = p.g / KB;                      // k-blocks per group
+    // zero bytes and scales of the next k-block's group (fetched one k-block ahead), of this k-block's, and the previous
+    // k-block's scale (0 before the first: promoting the zeroed acc then adds 0)
+    uint32_t nzA, nzB;
+    float nscA, nscB, pscA = 0.f, pscB = 0.f;
+    auto fetch = [&](int kb) {
+      const int g = min((kb0 + kb) / kpg, p.G - 1);
+      nzA = uint32_t(w4a8_zero(qz, p.N, g, nA, p.zp_const)) * 0x01010101u;
+      nzB = uint32_t(w4a8_zero(qz, p.N, g, nB, p.zp_const)) * 0x01010101u;
+      nscA = __ldg(scA + g);
+      nscB = __ldg(scB + g);
+    };
+    fetch(0);
+    int st = 0;
+    uint32_t full_par = 0;
+    int prev_st = -1;
+    auto step = [&](int kb, uint32_t (&fa)[8], uint32_t (&fb)[8]) {
+      const uint32_t zA = nzA, zB = nzB;
+      const float scaleA = nscA, scaleB = nscB;
+      const bool start = kb % kpg == 0;
+      fetch(kb + 1);
+      mbar_wait(&full[st], full_par);
+      const uint32_t wofs = uint32_t(st * SM::kWBytes);
+      dequant_row_i8<BITS, IL>(srcA + wofs, t, fa, zA);   // bytes u - z, signed
+      dequant_row_i8<BITS, IL>(srcB + wofs, t, fb, zB);
+      wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < BM / 2; ++i) {
+        const float f = w4a8_promote(facc[i], int(acc[i]), ((i >> 1) & 1) ? pscB : pscA);
+        facc[i] = start ? f : facc[i];
+      }
+      const uint64_t bdesc = make_sw128_desc(smem_u32(sA + st * SM::kActBytes));
+      wgmma_fence();
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        const uint32_t a[4] = {fa[2 * s], fb[2 * s], fa[2 * s + 1], fb[2 * s + 1]};
+        Wgmma<BM>::template i8<true>(acc, a, bdesc + uint64_t(2 * s), (s == 0 && start) ? 0u : 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();   // the MMAs of the previous k-block are done: its fragments and smem stage are free
+      if (prev_st >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev_st]);
+      }
+      prev_st = st;
+      if (++st == S) { st = 0; full_par ^= 1; }
+      pscA = scaleA; pscB = scaleB;
+    };
+    uint32_t fa0[8], fb0[8], fa1[8], fb1[8];
+    int kb = 0;
+    for (; kb + 1 < num_kb; kb += 2) {
+      step(kb, fa0, fb0);
+      step(kb + 1, fa1, fb1);
+    }
+    if (kb < num_kb) step(kb, fa0, fb0);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < BM / 2; ++i) facc[i] = w4a8_promote(facc[i], int(acc[i]), ((i >> 1) & 1) ? pscB : pscA);
+
+    // ----- epilogue: facc[4i + 2h + j] = S^T[row rA + 8h][column 8i + 2t + j] -----
+#pragma unroll
+    for (int i = 0; i < BM / 8; ++i) {
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int m = m0 + 8 * i + 2 * t + j;
+        if (m >= p.M) continue;
+        if (p.splits > 1) {   // the split's fp32 partial; splitk_reduce_w4a8 sums the splits in order
+          float* ws = reinterpret_cast<float*>(p.ws) + (size_t(split) * p.M + m) * p.N;
+          ws[nA] = facc[4 * i + j];
+          ws[nB] = facc[4 * i + 2 + j];
+          continue;
+        }
+        const float sa = sc.a_scale[m];
+        store_out_dequant(p.out.ptr[0], size_t(m) * p.N + nA, __fdiv_rn(facc[4 * i + j], sa), p.bias, nA, p.out_dtype);
+        store_out_dequant(p.out.ptr[0], size_t(m) * p.N + nB, __fdiv_rn(facc[4 * i + 2 + j], sa), p.bias, nB, p.out_dtype);
+      }
+    }
+    return;
+  }
 
   auto main_loop = [&](auto mode_tag) {
     constexpr int MODE = decltype(mode_tag)::value;
@@ -332,11 +429,34 @@ __device__ __forceinline__ void splitk_reduce_scaled(const TsParams& p, const Sc
   }
 }
 
+// splitk_reduce_kernel of the W4A8 instances: S = the fp32 partials summed in split order (from 0), then round_out(S / a_scale[m])
+// with the bias in out_dtype
+__device__ __forceinline__ void splitk_reduce_w4a8(const TsParams& p, const ScaledArgs& sc) {
+  const unsigned n4 = unsigned(p.N) >> 2;
+  const unsigned total4 = unsigned(p.M) * n4;
+  const size_t split_stride4 = size_t(p.M) * n4;
+  for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < total4; i += gridDim.x * blockDim.x) {
+    const unsigned m = i / n4, n = (i - m * n4) * 4u;
+    float S[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int sp = 0; sp < p.splits; ++sp) {
+      const float4 v = __ldcs(reinterpret_cast<const float4*>(p.ws) + size_t(sp) * split_stride4 + i);
+      S[0] = __fadd_rn(S[0], v.x); S[1] = __fadd_rn(S[1], v.y); S[2] = __fadd_rn(S[2], v.z); S[3] = __fadd_rn(S[3], v.w);
+    }
+    const float sa = sc.a_scale[m];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) store_out_dequant(p.out.ptr[0], size_t(m) * p.N + n + j, __fdiv_rn(S[j], sa), p.bias, n + j, p.out_dtype);
+  }
+}
+
 // out[m, n] = cast(sum_s ws[s][m][n]) (+ bias), stored to every destination of the OutSpec.  One thread = 4 consecutive n
 // (N is a multiple of 128 here): 128-bit loads of the partials, 32-bit index arithmetic, one vector store per destination.
-// SWIGLU: splitk_reduce_swiglu; SCALED: splitk_reduce_scaled.
-template <bool INT8, bool SWIGLU = false, bool SCALED = false>
+// SWIGLU: splitk_reduce_swiglu; SCALED: splitk_reduce_scaled; W4A8: splitk_reduce_w4a8.
+template <bool INT8, bool SWIGLU = false, bool SCALED = false, bool W4A8 = false>
 __global__ void splitk_reduce_kernel(const TsParams p, const ScaledArgs sc) {
+  if constexpr (W4A8) {
+    splitk_reduce_w4a8(p, sc);
+    return;
+  }
   if constexpr (SWIGLU) {
     splitk_reduce_swiglu(p);
     return;
@@ -456,11 +576,19 @@ int make_map_w_tiled(CUtensorMap* map, const void* base, uint64_t row_bytes, uin
   return 0;
 }
 
-template <typename T, int BITS, int BM, bool IL, int FMT, bool SWIGLU, bool SCALED>
+// W4A8: the largest split factor up to the plain instance's that divides the group count, so every split starts on a group
+// boundary (and needs no more workspace than the plain instance)
+int choose_splits_w4a8(int tiles, int num_kb, int groups, int sms) {
+  int sp = choose_splits(tiles, num_kb, sms);
+  while (groups % sp) --sp;
+  return sp;
+}
+
+template <typename T, int BITS, int BM, bool IL, int FMT, bool SWIGLU, bool SCALED, bool W4A8 = false>
 int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
   using SM = TsSmem<T, BITS, BM>;
   using EI = ElemInfo<T>;
-  auto kernel = gemm_ts_kernel<T, BITS, BM, IL, FMT, SWIGLU, SCALED>;
+  auto kernel = gemm_ts_kernel<T, BITS, BM, IL, FMT, SWIGLU, SCALED, W4A8>;
   static KernelCache<> cache;
   if (!kernel_setup(cache, kernel, SM::kTotal)) {
     set_error("gemm_ts: cannot raise the kernel's dynamic shared memory to %d bytes on this device", SM::kTotal);
@@ -470,7 +598,8 @@ int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
   p.m_tiles = (a.m + BM - 1) / BM;
   const int num_kb_total = a.d.K / EI::kKB;
   const int tiles = p.m_tiles * (a.d.N / TS_ROWS);
-  p.splits = a.m <= 128 ? choose_splits(tiles, num_kb_total, device_sm_count()) : 1;
+  if constexpr (W4A8) p.splits = a.m <= 128 ? choose_splits_w4a8(tiles, num_kb_total, p.G, device_sm_count()) : 1;
+  else p.splits = a.m <= 128 ? choose_splits(tiles, num_kb_total, device_sm_count()) : 1;
   const size_t ws_off = splitk_partials_offset();
   if (p.splits > 1 && a.workspace_bytes < ws_off + size_t(p.splits) * a.m * a.d.N * 4) p.splits = 1;  // no scratch given
   p.kb_per_split = num_kb_total / p.splits;
@@ -496,7 +625,8 @@ int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
     const size_t total = size_t(a.m) * a.d.N / (SWIGLU ? 8 : 4);   // one thread per 4 consecutive output columns
     const int rthreads = 256;
     const int rblocks = int(std::min<size_t>((total + rthreads - 1) / rthreads, size_t(device_sm_count()) * 8));
-    if constexpr (SCALED) splitk_reduce_kernel<true, false, true><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
+    if constexpr (W4A8) splitk_reduce_kernel<true, false, false, true><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
+    else if constexpr (SCALED) splitk_reduce_kernel<true, false, true><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
     else if (EI::kInt8) splitk_reduce_kernel<true><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
     else if (SWIGLU) splitk_reduce_kernel<false, true><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
     else splitk_reduce_kernel<false><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
@@ -526,6 +656,13 @@ int launch_ts_bm(const MatmulArgs& a, const TsParams& p) {
 template <typename T, int BITS>
 int launch_ts_layout(const MatmulArgs& a, const TsParams& p) {
   return a.d.w_layout == BB_LAYOUT_COMPRESSED ? launch_ts_bm<T, BITS, false, 0>(a, p) : launch_ts_bm<T, BITS, true, 0>(a, p);
+}
+// bb_matmul_w4a8 (int8 activations, 4-bit weights): 32 activation rows per CTA up to m = 32, else 64 (at 128 the fp32 group sums
+// do not fit beside the int32 accumulators: ptxas spills)
+template <bool IL>
+int launch_ts_w4a8(const MatmulArgs& a, const TsParams& p) {
+  if (a.m <= 32) return launch_ts_inst<int8_t, 4, 32, IL, 0, false, false, true>(a, p);
+  return launch_ts_inst<int8_t, 4, 64, IL, 0, false, false, true>(a, p);
 }
 
 }  // namespace
@@ -579,6 +716,7 @@ int launch_gemm_ts(const MatmulArgs& a) {
     return d.a_dtype == BB_F16 ? launch_ts_bm<__half, 4, false, 1>(a, p) : launch_ts_bm<__nv_bfloat16, 4, false, 1>(a, p);
   if (d.w_fmt == BB_W_FP8_E4M3 || d.w_fmt == BB_W_FP8_E5M2)
     return d.a_dtype == BB_F16 ? launch_ts_bm<__half, 8, false, 2>(a, p) : launch_ts_bm<__nv_bfloat16, 8, false, 2>(a, p);
+  if (a.w4a8) return d.w_layout == BB_LAYOUT_COMPRESSED ? launch_ts_w4a8<false>(a, p) : launch_ts_w4a8<true>(a, p);
   if (d.a_dtype == BB_I8) return d.w_bits == 4 ? launch_ts_layout<int8_t, 4>(a, p) : launch_ts_layout<int8_t, 2>(a, p);
   if (d.a_dtype == BB_F16) return d.w_bits == 4 ? launch_ts_layout<__half, 4>(a, p) : launch_ts_layout<__half, 2>(a, p);
   return d.w_bits == 4 ? launch_ts_layout<__nv_bfloat16, 4>(a, p) : launch_ts_layout<__nv_bfloat16, 2>(a, p);

@@ -40,6 +40,151 @@ gemv_mma_kernel(const GemvParams p) {
   gemv_mma_tile<T, BITS, IL, NT, ZK, SC, true, SWIGLU>(p, blockIdx.x, red);
 }
 
+__device__ __forceinline__ void mma_16832_s8s8(int (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+// register budget of one gemv_i8 instance (W4A8 also carries the fp32 group sums and the group parameters)
+constexpr int gemv_i8_maxnreg(int nt, bool w4a8) {
+  return w4a8 ? (nt == 1 ? 128 : (nt == 2 ? 168 : 232)) : (nt == 1 ? 96 : (nt == 2 ? 128 : 208));
+}
+
+// bb_matmul_w4a8 on the streaming GEMV: 4-bit weights (interleaved-8), per-group fp32 scales sc.w_scale [N, G] and zero points.
+// Warp w of the CTA owns whole groups (split_range over the G groups); each 128-k step decodes u - z into signed bytes for an
+// s8.s8 MMA, and at a group's last step the exact int32 sums are promoted into fp32 with the group's scale (fetched one group
+// ahead).  The CTA then sums the warps' fp32 partials in warp order and stores round_out(S / a_scale[m]) (+ bias).
+template <int NT>
+__device__ __forceinline__ void gemv_i8_w4a8(const GemvParams& p, const ScaledArgs& sc, int (&red)[MAX_KS][16][8 * NT]) {
+  constexpr int BITS = 4, WPS = BITS, STEP_BYTES = 16 * BITS;
+  const int lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
+  const int r = lane >> 2, q = lane & 3;
+  const int rb = blockIdx.x;
+  const int n_a = rb * 16 + r, n_b = n_a + 8;
+  const int spg = p.g / 128;   // steps per group
+  int g_begin, g_end;
+  split_range(p.G, p.ks, warp, g_begin, g_end);
+  const int step_begin = g_begin * spg;
+  const int ns = (g_end - g_begin) * spg;
+  const size_t row_bytes = size_t(p.K) * BITS / 8;
+  const uint8_t* wpa = p.W + size_t(n_a) * row_bytes + q * (4 * WPS) + size_t(step_begin) * STEP_BYTES;
+  const uint8_t* wpb = wpa + 8 * row_bytes;
+  const uint4* ap[NT];
+#pragma unroll
+  for (int t = 0; t < NT; ++t) {
+    const int m = min(8 * t + r, p.M - 1);
+    ap[t] = reinterpret_cast<const uint4*>(reinterpret_cast<const int8_t*>(p.A) + size_t(m) * p.K) + step_begin * 8 + q * 2;
+  }
+  const uint8_t* qz = reinterpret_cast<const uint8_t*>(p.zeros);
+  const float* scA = sc.w_scale + size_t(n_a) * p.G;
+  const float* scB = sc.w_scale + size_t(n_b) * p.G;
+  int acc[NT][4];
+  float facc[NT][4];
+#pragma unroll
+  for (int t = 0; t < NT; ++t)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { acc[t][j] = 0; facc[t][j] = 0.f; }
+  // group gi's zero bytes / scales (z, s) and group gi + 1's (nz, ns_)
+  int gi = g_begin, left = spg;
+  uint32_t zA = 0, zB = 0, nzA = 0, nzB = 0;
+  float sA = 0.f, sB = 0.f, nsA = 0.f, nsB = 0.f;
+  auto fetch = [&](int g) {
+    nzA = uint32_t(w4a8_zero(qz, p.N, g, n_a, p.zp_const)) * 0x01010101u;
+    nzB = uint32_t(w4a8_zero(qz, p.N, g, n_b, p.zp_const)) * 0x01010101u;
+    nsA = __ldg(scA + g);
+    nsB = __ldg(scB + g);
+  };
+  auto enter = [&]() {   // group gi begins: its fetched parameters become current; fetch the next group's
+    zA = nzA; zB = nzB; sA = nsA; sB = nsB;
+    if (gi + 1 < g_end) fetch(gi + 1);
+  };
+
+  auto process = [&](const uint32_t (&wa)[WPS], const uint32_t (&wb)[WPS]) {
+    uint32_t da[8], db[8];  // 8 byte-quads = 32 k per row, natural k order: u - z as signed bytes
+#pragma unroll
+    for (int wi = 0; wi < WPS; ++wi) {
+      uint32_t ta[2], tb[2];
+      decode_u4x8_to_u8(wa[wi], 0x80808080u, ta);
+      decode_u4x8_to_u8(wb[wi], 0x80808080u, tb);
+#pragma unroll
+      for (int x = 0; x < 2; ++x) { da[2 * wi + x] = bytes_sub_zp(ta[x], zA); db[2 * wi + x] = bytes_sub_zp(tb[x], zB); }
+    }
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+      const uint4 v0 = __ldg(ap[t]), v1 = __ldg(ap[t] + 1);
+      const uint32_t R[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+      ap[t] += 8;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint32_t af[4] = {da[2 * j], db[2 * j], da[2 * j + 1], db[2 * j + 1]};
+        mma_16832_s8s8(acc[t], af, R[2 * j], R[2 * j + 1]);
+      }
+    }
+    if (--left == 0) {   // the group's last step: promote (acc[t][0..1] are row n_a, acc[t][2..3] row n_b) and restart
+#pragma unroll
+      for (int t = 0; t < NT; ++t)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          facc[t][j] = w4a8_promote(facc[t][j], acc[t][j], j < 2 ? sA : sB);
+          acc[t][j] = 0;
+        }
+      left = spg;
+      ++gi;
+      if (gi < g_end) enter();
+    }
+  };
+
+  if (ns > 0) {
+    fetch(gi);
+    enter();
+    uint32_t wq[PF][2][WPS];
+    const uint8_t* wnext_a = wpa;
+    const uint8_t* wnext_b = wpb;
+#pragma unroll
+    for (int u = 0; u < PF; ++u) {
+      if (u < ns) { load_w<BITS>(wnext_a, wq[u][0]); load_w<BITS>(wnext_b, wq[u][1]); }
+      wnext_a += STEP_BYTES; wnext_b += STEP_BYTES;
+    }
+    pdl_wait();
+    auto chunk = [&](auto guard_tag, int s) {
+      constexpr bool GUARD = decltype(guard_tag)::value;
+#pragma unroll
+      for (int u = 0; u < PF; ++u) {
+        if (!GUARD || s + u < ns) {
+          process(wq[u][0], wq[u][1]);
+          if (!GUARD || s + u + PF < ns) { load_w<BITS>(wnext_a, wq[u][0]); load_w<BITS>(wnext_b, wq[u][1]); }
+          wnext_a += STEP_BYTES; wnext_b += STEP_BYTES;
+        }
+      }
+    };
+    int s = 0;
+#pragma unroll 1
+    for (; s + 2 * PF <= ns; s += PF) chunk(std::false_type{}, s);
+#pragma unroll 1
+    for (; s < ns; s += PF) chunk(std::true_type{}, s);
+  }
+  if (ns <= 0) pdl_wait();
+  pdl_launch_dependents();
+#pragma unroll
+  for (int t = 0; t < NT; ++t) {
+    red[warp][r][8 * t + 2 * q] = __float_as_int(facc[t][0]);
+    red[warp][r][8 * t + 2 * q + 1] = __float_as_int(facc[t][1]);
+    red[warp][r + 8][8 * t + 2 * q] = __float_as_int(facc[t][2]);
+    red[warp][r + 8][8 * t + 2 * q + 1] = __float_as_int(facc[t][3]);
+  }
+  __syncthreads();
+  for (int idx = threadIdx.x; idx < 16 * 8 * NT; idx += blockDim.x) {
+    const int row = idx & 15, m = idx >> 4;
+    if (m >= p.M) continue;
+    float S = 0.f;
+    for (int w = 0; w < p.ks; ++w) S = __fadd_rn(S, __int_as_float(red[w][row][m]));
+    const int n = rb * 16 + row;
+    store_out_dequant(p.out.ptr[0], size_t(m) * size_t(p.out.ld) + n, __fdiv_rn(S, sc.a_scale[m]), p.bias, n, p.out_dtype);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // int8 activations (W2A8 / W4A8), exact int32 accumulation.  Weights are used as raw unsigned fields
 // (mma .u8.s8); the constant zero point of the signed formats is removed with zp * sum_k(a), the sum
@@ -47,12 +192,17 @@ gemv_mma_kernel(const GemvParams p) {
 // SCALED: bb_matmul_scaled -- the epilogue divides by sc.a_scale[m] (read after the PDL wait) and sc.w_scale[n] (store_out_scaled;
 // bias in out_dtype).  The scales are a parameter of their own: GemvParams is also the grouped GEMV's, whose layout stays put.
 // ---------------------------------------------------------------------------------------------
-template <int BITS, int NT, bool SCALED = false>
-__global__ void __launch_bounds__(gemv_max_ks(NT) * 32) __maxnreg__(NT == 1 ? 96 : (NT == 2 ? 128 : 208))
+// W4A8 (BITS = 4): bb_matmul_w4a8, gemv_i8_w4a8 (red then holds fp32 bits).
+template <int BITS, int NT, bool SCALED = false, bool W4A8 = false>
+__global__ void __launch_bounds__(gemv_max_ks(NT) * 32) __maxnreg__(gemv_i8_maxnreg(NT, W4A8))
 gemv_i8_kernel(const GemvParams p, const ScaledArgs sc) {
   constexpr int WPS = BITS;            // words per thread per row per step (32 k)
   constexpr int STEP_BYTES = 16 * BITS;
   __shared__ int red[MAX_KS][16][8 * NT];
+  if constexpr (W4A8) {
+    gemv_i8_w4a8<NT>(p, sc, red);
+    return;
+  }
   const int lane = threadIdx.x & 31;
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const int r = lane >> 2, q = lane & 3;
@@ -238,7 +388,13 @@ int launch_gemv_i8(const MatmulArgs& a) {
   const GemvParams p = make_params(a);
   return gemv_nt(p.M, [&](auto nt) {
     constexpr int NT = decltype(nt)::value;
-    static KernelCache<MAX_KS + 1> cache2, cache4, cache2s, cache4s;
+    static KernelCache<MAX_KS + 1> cache2, cache4, cache2s, cache4s, cache_w4a8;
+    if (a.w4a8) {   // the warps split the groups, not the steps: ks <= G
+      auto kernel = gemv_i8_kernel<4, NT, false, true>;
+      GemvParams pw = p;
+      pw.ks = pick_ks(cache_w4a8, kernel, gemv_max_ks(NT), pw.N / 16, pw.G);
+      return launch_pdl(kernel, pw.N / 16, pw.ks * 32, 0, a.stream, pdl_enabled(), pw, a.scaled);
+    }
     if (a.is_scaled())
       return a.d.w_bits == 2 ? launch_gemv_kernel<NT>(gemv_i8_kernel<2, NT, true>, cache2s, p, a.stream, a.scaled)
                              : launch_gemv_kernel<NT>(gemv_i8_kernel<4, NT, true>, cache4s, p, a.stream, a.scaled);

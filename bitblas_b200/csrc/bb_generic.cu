@@ -196,8 +196,8 @@ generic_float_kernel(const bb_matmul_desc d, const T* __restrict__ A, const uint
 }
 
 // int8 activations, exact int32 accumulate.  SCALED: bb_matmul_scaled -- store_out_scaled with a_scale [M], w_scale [N] and a bias
-// in out_dtype
-template <bool SCALED = false>
+// in out_dtype.  W4A8: bb_matmul_w4a8 -- 4-bit weights, fp32 group scales sc.w_scale [N, G], zero points, store_out_dequant
+template <bool SCALED = false, bool W4A8 = false>
 __global__ void __launch_bounds__(WARPS * 32)
 generic_int_kernel(const bb_matmul_desc d, const int8_t* __restrict__ A, const uint8_t* __restrict__ W,
                    const int8_t* __restrict__ scale, const void* __restrict__ zeros,
@@ -206,6 +206,44 @@ generic_int_kernel(const bb_matmul_desc d, const int8_t* __restrict__ A, const u
   const int n = blockIdx.x * WARPS + warp;
   const int m0 = blockIdx.y * MT;
   if (n >= d.N) return;
+  if constexpr (W4A8) {
+    // group by group: the exact int32 sum of the group (lanes stride k, then a butterfly sum), promoted into fp32 with the
+    // group's scale in group order -- the order of gemm_ts_kernel without split-K
+    const int K = d.K, g = d.group_size <= 0 ? K : d.group_size, G = K / g;
+    const int tiled = d.w_tile == BB_TILE_SLAB;
+    const uint8_t* Wrow = W + (tiled ? tiled_byte_offset(n, 0, (long long)K / 2) : size_t(n) * (size_t(K) / 2));
+    const uint8_t* qz = d.with_zeros ? reinterpret_cast<const uint8_t*>(zeros) : nullptr;
+    float S[MT];
+#pragma unroll
+    for (int i = 0; i < MT; ++i) S[i] = 0.f;
+    for (int gi = 0; gi < G; ++gi) {
+      const int z = w4a8_zero(qz, d.N, gi, n, d.w_fmt == BB_W_INT ? 8 : 0);
+      int acc[MT];
+#pragma unroll
+      for (int i = 0; i < MT; ++i) acc[i] = 0;
+      for (int k = gi * g + lane; k < (gi + 1) * g; k += 32) {
+        const int w = int(load_field(Wrow, k, 4, d.w_layout, tiled)) - z;
+#pragma unroll
+        for (int i = 0; i < MT; ++i)
+          if (m0 + i < M) acc[i] += int(A[size_t(m0 + i) * K + k]) * w;
+      }
+      const float s = sc.w_scale[size_t(n) * G + gi];
+#pragma unroll
+      for (int i = 0; i < MT; ++i) {
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) acc[i] += __shfl_xor_sync(0xffffffffu, acc[i], off);
+        S[i] = w4a8_promote(S[i], acc[i], s);
+      }
+    }
+    if (lane == 0) {
+#pragma unroll
+      for (int i = 0; i < MT; ++i)
+        if (m0 + i < M)
+          store_out_dequant(C, size_t(m0 + i) * d.N + n, __fdiv_rn(S[i], sc.a_scale[m0 + i]), d.with_bias ? bias : nullptr, n,
+                            d.out_dtype);
+    }
+    return;
+  }
   const int K = d.K, bits = d.w_bits;
   const int g = d.group_size <= 0 ? K : d.group_size;
   const int G = K / g;
@@ -296,7 +334,7 @@ int launch_generic(const MatmulArgs& a) {
   } else if (d.a_dtype == BB_BF16) {
     run_float(TypeTag<__nv_bfloat16>{});
   } else {
-    auto kernel = a.is_scaled() ? generic_int_kernel<true> : generic_int_kernel<false>;
+    auto kernel = a.w4a8 ? generic_int_kernel<false, true> : (a.is_scaled() ? generic_int_kernel<true> : generic_int_kernel<false>);
     kernel<<<grid, block, 0, a.stream>>>(d, (const int8_t*)a.A, (const uint8_t*)a.W, (const int8_t*)a.scale, a.zeros,
                                          (const int8_t*)a.bias, a.C, a.m, a.scaled);
   }

@@ -387,16 +387,21 @@ class Matmul(Operator):
         return input_tensor  # no ladder propagation on H100
 
     # ---- forward ------------------------------------------------------------------------------------
-    def _check_params(self, W, scale, zeros, bias, device, scaled=False):
+    def _check_params(self, W, scale, zeros, bias, device, scaled=False, w4a8=False):
         """full validation of the (static) parameter tensors, all of them on `device` (A's: the kernel gets bare pointers);
         forward() runs it once per distinct set of tensors.  scaled (forward_scaled): `scale` is the fp32 [N] w_scale and the
-        bias is in the output dtype."""
+        bias is in the output dtype; w4a8 (forward_w4a8): `scale` is fp32 [N, K/g] and the bias is in the output dtype."""
         c = self.config
         adt = getattr(torch, c.A_dtype)
         wshape = self.retrieve_weight_shape()
         _lib.check_tensor(W, "W", torch.int8 if W.dtype != torch.uint8 else torch.uint8, numel=wshape[0] * wshape[1])
         G = c.K // (c.group_size if c.group_size and c.group_size > 0 else c.K)
-        if c.with_scaling:
+        if w4a8:
+            if scale is None:
+                raise ValueError("forward_w4a8 needs scale (float32 [N, K/g])")
+            _lib.check_tensor(scale, "scale", torch.float32, numel=c.N * G)
+            scaled, adt = True, None   # the bias check below is forward_scaled's
+        elif c.with_scaling:
             if scale is None:
                 raise ValueError("with_scaling=True but scale is None")
             _lib.check_tensor(scale, "scale", adt, numel=c.N * G)
@@ -411,7 +416,7 @@ class Matmul(Operator):
             if bias is None:
                 raise ValueError("with_bias=True but bias is None")
             _lib.check_tensor(bias, "bias", self.torch_output_dtype if scaled else adt, numel=c.N)
-        if scaled:
+        if scaled and not w4a8:
             if scale is None:
                 raise ValueError("forward_scaled needs w_scale (float32 [N])")
             _lib.check_tensor(scale, "w_scale", torch.float32, numel=c.N)
@@ -434,7 +439,7 @@ class Matmul(Operator):
         output, ptrs = self._check_forward(A, W, scale, zeros, bias, output)
         return self._launch(A, ptrs, output)
 
-    def _check_forward(self, A, W, scale, zeros, bias, output, swiglu=False, scaled=False):
+    def _check_forward(self, A, W, scale, zeros, bias, output, swiglu=False, scaled=False, w4a8=False):
         """the checking half of forward() (swiglu: of forward_swiglu, whose output has N / 2 columns; scaled: of forward_scaled,
         with `scale` the w_scale): validates every argument and launches nothing.  Returns the output and, for _launch, the data
         pointers of W, scale, zeros and bias."""
@@ -445,9 +450,9 @@ class Matmul(Operator):
         # pointers and A's device; a new tensor -- or a re-allocated one -- is validated again).  The activations are checked
         # every call.
         key = (W.data_ptr(), scale.data_ptr() if scale is not None else 0, zeros.data_ptr() if zeros is not None else 0,
-               bias.data_ptr() if bias is not None else 0, A.device, scaled)
+               bias.data_ptr() if bias is not None else 0, A.device, scaled, w4a8)
         if key != self._checked_key:
-            self._check_params(W, scale, zeros, bias, A.device, scaled)
+            self._check_params(W, scale, zeros, bias, A.device, scaled, w4a8)
             self._checked_key = key
         K = c.K
         if A.shape[-1] != K:
@@ -467,10 +472,14 @@ class Matmul(Operator):
                         output.data_ptr(), A.numel() // self.config.K, idx, stream, swiglu)
         return output
 
-    def _launch_raw(self, A, W, lut, scale, zeros, bias, C, m, device, stream, swiglu=False, a_scale=None):
+    def _launch_raw(self, A, W, lut, scale, zeros, bias, C, m, device, stream, swiglu=False, a_scale=None, w4a8=False):
         """the package's one bb_matmul (swiglu: bb_matmul_swiglu; a_scale, the pointer of the fp32 [m] activation scales:
-        bb_matmul_scaled with `scale` the w_scale) call: raw pointers (0 = absent), m rows, on the device of ordinal `device`"""
-        ws_ptr, ws_bytes = self._workspace_for(m, device, stream)
+        bb_matmul_scaled with `scale` the w_scale, or with w4a8 bb_matmul_w4a8 with `scale` the fp32 group scales) call: raw
+        pointers (0 = absent), m rows, on the device of ordinal `device`"""
+        ws_ptr, ws_bytes = self._workspace_for(m, device, stream, w4a8)
+        if w4a8:
+            _lib.call("bb_matmul_w4a8", device, self._desc_ref, A, W, a_scale, scale, zeros, bias, C, m, ws_ptr, ws_bytes, stream)
+            return
         if a_scale is not None:
             _lib.call("bb_matmul_scaled", device, self._desc_ref, A, W, a_scale, scale, bias, C, m, ws_ptr, ws_bytes, stream)
             return
@@ -531,14 +540,16 @@ class Matmul(Operator):
                          a_scale=a_scale.data_ptr())
         return output
 
-    def _workspace_for(self, m: int, device: int, stream: int):
-        """scratch the kernel picked for `m` needs (bb_workspace_bytes: split-K partials, stream-K exchange slots); one cached,
-        ZERO-INITIALISED buffer per operator, device (ordinal) and stream, grown on demand.  The m = 1 slab kernel leaves its slots
-        zero-tagged, so the buffer is reused by later calls on the same stream without clearing (include/bitblas_b200.h)."""
-        key = (int(m), _lib.OVERRIDE_GEN)
+    def _workspace_for(self, m: int, device: int, stream: int, w4a8: bool = False):
+        """scratch the kernel picked for `m` needs (bb_workspace_bytes: split-K partials, stream-K exchange slots; w4a8: of the
+        descriptor without group scales and zeros, which bb_matmul_w4a8's kernels need at most); one cached, ZERO-INITIALISED
+        buffer per operator, device (ordinal) and stream, grown on demand.  The m = 1 slab kernel leaves its slots zero-tagged,
+        so the buffer is reused by later calls on the same stream without clearing (include/bitblas_b200.h)."""
+        key = (int(m), _lib.OVERRIDE_GEN, w4a8)
         need = self._ws_need.get(key)
         if need is None:
-            need = self._ws_need[key] = int(self.lib._c.bb_workspace_bytes(ctypes.byref(self._desc), int(m)))
+            need = self._ws_need[key] = int(self.lib._c.bb_workspace_bytes(ctypes.byref(self._w4a8_cleared_desc() if w4a8 else
+                                                                                        self._desc), int(m)))
         if need == 0:
             return 0, 0
         wkey = (device, stream)
@@ -547,6 +558,59 @@ class Matmul(Operator):
             ws = torch.zeros(need, dtype=torch.uint8, device=torch.device("cuda", device))
             self._ws[wkey] = ws
         return ws.data_ptr(), ws.numel()
+
+    def check_w4a8(self) -> None:
+        """raise unless forward_w4a8 covers this operator: NotImplementedError for a consistent (A_dtype == W_dtype) operator,
+        ValueError for 16-bit activations, an integer out_dtype, no group scales, zeros other than "quantized", weights other than
+        4-bit uint / int, or int weights with zeros"""
+        if self.consistent:
+            raise NotImplementedError("forward_w4a8 needs a low-bit weight operator")
+        c = self.config
+        if c.A_dtype != "int8":
+            raise ValueError(f"forward_w4a8 needs int8 activations (A_dtype={c.A_dtype}; quantize_act_int8 makes them from "
+                             "float16 / bfloat16)")
+        if c.out_dtype not in ("float16", "bfloat16", "float32"):
+            raise ValueError(f"forward_w4a8 needs out_dtype float16, bfloat16 or float32 (got {c.out_dtype})")
+        if not c.with_scaling:
+            raise ValueError("forward_w4a8 needs with_scaling=True (float32 group scales)")
+        if c.with_zeros and c.zeros_mode != "quantized":
+            raise ValueError(f"forward_w4a8 needs zeros_mode='quantized' (got {c.zeros_mode})")
+        if c.W_dtype not in ("uint4", "int4"):
+            raise ValueError(f"forward_w4a8 needs uint4 or int4 weights (got {c.W_dtype})")
+        if c.with_zeros and c.W_dtype == "int4":
+            raise ValueError("forward_w4a8: int4 weights take no zero points")
+
+    def _w4a8_cleared_desc(self) -> _lib.MatmulDesc:
+        """this operator's descriptor without group scales and zeros: its bb_workspace_bytes sizes bb_matmul_w4a8's workspace"""
+        d = getattr(self, "_w4a8_desc", None)
+        if d is None:
+            d = self._w4a8_desc = _lib.MatmulDesc.from_buffer_copy(self._desc)
+            d.with_scaling = d.with_zeros = 0
+        return d
+
+    def kernel_for_w4a8(self, m: int) -> str:
+        """the kernel family forward_w4a8 runs for m rows (bb_select_kernel_w4a8)"""
+        return _lib.kernel_name(self.lib._c.bb_select_kernel_w4a8(ctypes.byref(self._desc), int(m)))
+
+    def forward_w4a8(self, A_q, W, a_scale, scale, zeros=None, bias=None, output=None):
+        """GPTQ-style 4-bit weights against int8 activations in one launch (bb_matmul_w4a8; two with split-K): A_q int8 [.., K]
+        (e.g. from quantize_act_int8), a_scale float32 [m] one quantization scale per row of A_q, scale float32 [N, K/g] the group
+        scales, zeros the packed quantized zero points [K/g, N/2] (with_zeros), and output [.., N] = round(S / a_scale[r])
+        (+ bias, [N] in the output dtype, added after the rounding) with S = sum_g float(acc_g) * scale[n, g] in fp32 and acc_g
+        the exact int32 dot product of group g.  The kernel is kernel_for_w4a8(m)."""
+        self.check_w4a8()
+        c = self.config
+        output, ptrs = self._check_forward(A_q, W, scale, zeros, bias, output, scaled=True, w4a8=True)
+        m = A_q.numel() // c.K
+        if not (isinstance(a_scale, torch.Tensor) and a_scale.is_cuda and a_scale.dtype == torch.float32
+                and a_scale.is_contiguous() and a_scale.numel() == m):
+            _lib.check_tensor(a_scale, "a_scale", torch.float32, numel=m)
+        if a_scale.device != A_q.device:
+            raise ValueError(f"a_scale must be on A's device {A_q.device} (got {a_scale.device})")
+        _, idx, stream = _lib.device_stream(A_q)
+        self._launch_raw(A_q.data_ptr(), ptrs[0], 0, ptrs[1], ptrs[2], ptrs[3], output.data_ptr(), m, idx, stream,
+                         a_scale=a_scale.data_ptr(), w4a8=True)
+        return output
 
     def forward_scatter(self, A, W, scale=None, zeros=None, bias=None, *, peer_ptrs, ldc: int, col_offset: int):
         """Column-parallel forward (bb_matmul_scatter): this operator's N is the local shard; the kernel epilogue stores the

@@ -173,6 +173,35 @@ int bb_quantize_act_int8(const void* x, int a_dtype, int rows, int K, int8_t* q,
 int bb_matmul_scaled(const bb_matmul_desc* desc, const void* A, const void* W, const float* a_scale, const float* w_scale,
                      const void* bias, void* C, int m, void* workspace, size_t workspace_bytes, void* stream);
 
+/* GPTQ-style 4-bit weights with int8 activations (W4A8): A int8 [m, K] (from bb_quantize_act_int8) against 4-bit weights with one
+ * fp32 scale per (row, group) and optional quantized zero points.  desc: a_dtype = BB_I8, accum_dtype = BB_I32, w_bits = 4, w_fmt
+ * uint or int, with_scaling = 1, with_zeros only for uint weights and only in mode BB_ZEROS_QUANTIZED (zeros [K/g, N/2] packed as
+ * bb_repack_gptq_qzeros_device writes them), out_dtype float16 | bfloat16 | float32, g = -1 or a divisor of K.  With w[n, k] the
+ * integer bb_matmul decodes (u for uint, u - 8 for int, u - z[n, g] with zeros; always in [-15, 15]):
+ *     acc[r, n, g] = sum_{k in group g} A[r, k] * w[n, k]                        exact int32
+ *     S[r, n]      = sum_g float(acc[r, n, g]) * scale[n, g]                      fp32, each conversion, product and sum rounded
+ *     C[r, n]      = round_out(S[r, n] / a_scale[r])   (+ bias[n], [N] in out_dtype, added after the rounding; IEEE division)
+ * scale is fp32 [N, K/g] and a_scale fp32 [m], both 4-byte aligned.  The order of the fp32 sum over groups is fixed per kernel,
+ * split factor and SM count, so a call is deterministic:
+ *   - generic_simt and gemm_ts_wgmma_i8 without split-K: S = (((0 + p_0) + p_1) + ...) + p_{G-1}, p_g = float(acc) * scale, in
+ *     group order;
+ *   - gemm_ts_wgmma_i8 split s ways (s divides G; split j owns groups [jG/s, (j+1)G/s)): each split sums its groups as above, and
+ *     S = ((0 + S_0) + S_1) + ... + S_{s-1};
+ *   - gemv_i8: the CTA's warps own contiguous ranges of whole groups (as many warps as the launch picks, at most G); each sums
+ *     its groups as above, and S = ((0 + S_warp0) + S_warp1) + ... in warp order.  So with few groups the K split is small: at
+ *     g = -1 (G = 1) every 16-row block of W is streamed by one warp, which makes such a decode much slower than with g = 128.
+ * Kernel choice: the family bb_select_kernel picks for the same desc with with_scaling = with_zeros = 0 (gemv_i8, gemm_ts_wgmma_i8
+ * or generic_simt), except that g % 128 != 0 runs generic_simt instead of gemv_i8 / gemm_ts_wgmma_i8 (under a kernel override
+ * forcing one of those two it is not supported).  The override and the SM-count cap apply; bb_select_kernel_w4a8 reports the
+ * choice (-1 on an invalid desc).  The workspace is bb_workspace_bytes of that cleared desc, which always suffices (a split factor
+ * is never above the plain call's); a smaller or null workspace runs without split-K.  Rejections come in bb_matmul_scaled's order,
+ * each with its own message: 16-bit activations, an int out_dtype, with_scaling = 0, original / rescale zeros, other bit widths and
+ * formats, int weights with zeros, then m, then null a_scale / scale (code 1) and misaligned ones (code 5).  m == 0 returns 0 and
+ * launches nothing.  Launch count, stream semantics, PDL behaviour and graph capture are those of bb_matmul_scaled. */
+int bb_matmul_w4a8(const bb_matmul_desc* desc, const void* A, const void* W, const float* a_scale, const float* scale,
+                   const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes, void* stream);
+int bb_select_kernel_w4a8(const bb_matmul_desc* desc, int m);
+
 /* Grouped matmul for mixture-of-experts layers (no reference counterpart; the contract of torch._grouped_mm with offsets).
  * `num_groups` problems share `desc` and run as ONE kernel launch.  A[total_rows, K] holds the rows of every group, sorted so
  * that group e owns rows [offsets[e], offsets[e+1]); `offsets` is a DEVICE int32 array of num_groups + 1 entries, read by the
