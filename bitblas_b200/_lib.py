@@ -15,7 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libbitblas_b200.so")
 
 # enums (include/bitblas_b200.h)
-BB_F16, BB_BF16, BB_F32, BB_I8, BB_I32 = 0, 1, 2, 3, 4
+BB_F16, BB_BF16, BB_F32, BB_I8, BB_I32, BB_E4M3 = 0, 1, 2, 3, 4, 5
 BB_W_UINT, BB_W_INT, BB_W_NF, BB_W_FP4, BB_W_FP8_E4M3, BB_W_FP8_E5M2 = 0, 1, 2, 3, 4, 5
 BB_ZEROS_ORIGINAL, BB_ZEROS_RESCALE, BB_ZEROS_QUANTIZED = 0, 1, 2
 BB_LAYOUT_COMPRESSED, BB_LAYOUT_INTERLEAVED_16, BB_LAYOUT_INTERLEAVED_8 = 0, 1, 2
@@ -25,6 +25,7 @@ BB_PEER_FLAG_BYTES = 128
 BB_GROUPED_MAX_GROUPS = 256
 (BB_KERNEL_AUTO, BB_KERNEL_GENERIC, BB_KERNEL_GEMV_MMA, BB_KERNEL_GEMV_I8, BB_KERNEL_GEMM_TS,
  BB_KERNEL_GEMM_TS_I8, BB_KERNEL_GEMV_SLAB) = 0, 1, 2, 3, 4, 5, 7
+BB_KERNEL_GEMM_FP8 = 8   # bb_matmul_fp8 only
 
 DTYPE_IDS = {"float16": BB_F16, "bfloat16": BB_BF16, "float32": BB_F32, "int8": BB_I8, "int32": BB_I32}
 WFMT_IDS = {"uint": BB_W_UINT, "int": BB_W_INT, "nf": BB_W_NF, "fp": BB_W_FP4, "fp_e4m3": BB_W_FP8_E4M3,
@@ -32,7 +33,8 @@ WFMT_IDS = {"uint": BB_W_UINT, "int": BB_W_INT, "nf": BB_W_NF, "fp": BB_W_FP4, "
 ZEROS_IDS = {"original": BB_ZEROS_ORIGINAL, "rescale": BB_ZEROS_RESCALE, "quantized": BB_ZEROS_QUANTIZED}
 
 EXPORTS = [
-    "bb_init", "bb_matmul", "bb_matmul_swiglu", "bb_matmul_scaled", "bb_matmul_w4a8", "bb_select_kernel_w4a8", "bb_quantize_act_int8", "bb_matmul_scatter", "bb_matmul_grouped", "bb_matmul_grouped_gemm", "bb_matmul_grouped_swiglu",
+    "bb_init", "bb_matmul", "bb_matmul_swiglu", "bb_matmul_scaled", "bb_matmul_w4a8", "bb_select_kernel_w4a8", "bb_quantize_act_int8",
+    "bb_quantize_act_fp8", "bb_matmul_fp8", "bb_select_kernel_fp8", "bb_workspace_bytes_fp8", "bb_matmul_scatter", "bb_matmul_grouped", "bb_matmul_grouped_gemm", "bb_matmul_grouped_swiglu",
     "bb_matmul_grouped_gemm_swiglu", "bb_matmul_grouped_gemm_swiglu_gather", "bb_moe_route", "bb_moe_route_index",
     "bb_moe_combine", "bb_moe_topk", "bb_permute_cols", "bb_peer_barrier", "bb_workspace_bytes", "bb_select_kernel", "bb_kernel_name", "bb_set_kernel_override",
     "bb_set_sm_count_cap", "bb_launch_count", "bb_last_error", "bb_version", "bb_compress_host", "bb_interleave_host",
@@ -73,6 +75,10 @@ def load() -> ctypes.CDLL:
     lib.bb_matmul_w4a8.argtypes = [dp, vp, vp, vp, vp, vp, vp, vp, i32, vp, sz, vp]; lib.bb_matmul_w4a8.restype = i32
     lib.bb_select_kernel_w4a8.argtypes = [dp, i32]; lib.bb_select_kernel_w4a8.restype = i32
     lib.bb_quantize_act_int8.argtypes = [vp, i32, i32, i32, vp, vp, vp]; lib.bb_quantize_act_int8.restype = i32
+    lib.bb_quantize_act_fp8.argtypes = [vp, i32, i32, i32, vp, vp, i32, vp]; lib.bb_quantize_act_fp8.restype = i32
+    lib.bb_matmul_fp8.argtypes = [dp, vp, vp, i32, vp, vp, vp, vp, i32, vp, sz, vp]; lib.bb_matmul_fp8.restype = i32
+    lib.bb_select_kernel_fp8.argtypes = [dp, i32]; lib.bb_select_kernel_fp8.restype = i32
+    lib.bb_workspace_bytes_fp8.argtypes = [dp, i32]; lib.bb_workspace_bytes_fp8.restype = sz
     lib.bb_matmul_scatter.argtypes = [dp, vp, vp, vp, vp, vp, vp, ctypes.POINTER(vp), i32, i64, i64, i32, vp, sz, vp]
     lib.bb_matmul_scatter.restype = i32
     lib.bb_matmul_grouped.argtypes = [dp, i32, vp, vp, vp, vp, vp, vp, vp, i32, vp]; lib.bb_matmul_grouped.restype = i32

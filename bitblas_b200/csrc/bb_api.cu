@@ -233,6 +233,7 @@ const char* bb_kernel_name(int id) {
     case BB_KERNEL_GEMM_TS: return "gemm_ts_wgmma";
     case BB_KERNEL_GEMM_TS_I8: return "gemm_ts_wgmma_i8";
     case BB_KERNEL_GEMV_SLAB: return "gemv_slab";
+    case BB_KERNEL_GEMM_FP8: return "gemm_fp8_wgmma";
   }
   return "unknown";
 }
@@ -417,6 +418,80 @@ int bb_matmul_w4a8(const bb_matmul_desc* desc, const void* A, const void* W, con
 int bb_select_kernel_w4a8(const bb_matmul_desc* desc, int m) {
   if (validate(desc) || !w4a8_desc_ok(desc)) return -1;
   return select_w4a8(*desc, m);
+}
+
+// the descriptor of bb_matmul_fp8 (validate() is not run: it refuses a_dtype = BB_E4M3, as every other entry point does)
+static bool fp8_desc_ok(const bb_matmul_desc* d) {
+  if (!d) { set_error("null descriptor"); return false; }
+  if (d->a_dtype != BB_E4M3) {
+    set_error("bb_matmul_fp8: needs e4m3 activations (a_dtype=%d; quantize 16-bit ones with bb_quantize_act_fp8)", d->a_dtype);
+    return false;
+  }
+  if (d->w_fmt != BB_W_FP8_E4M3 || d->w_bits != 8) {
+    set_error("bb_matmul_fp8: needs e4m3 weights (w_fmt=%d, w_bits=%d; want BB_W_FP8_E4M3, 8)", d->w_fmt, d->w_bits);
+    return false;
+  }
+  if (d->accum_dtype != BB_F32) { set_error("bb_matmul_fp8: accum_dtype must be float32 (got %d)", d->accum_dtype); return false; }
+  if (d->out_dtype != BB_F16 && d->out_dtype != BB_BF16 && d->out_dtype != BB_F32) {
+    set_error("bb_matmul_fp8: out_dtype must be float16, bfloat16 or float32 (got %d)", d->out_dtype);
+    return false;
+  }
+  if (d->group_size != 128) { set_error("bb_matmul_fp8: group_size must be 128 (128 x 128 scale blocks; got %d)", d->group_size); return false; }
+  if (d->with_scaling != 1) { set_error("bb_matmul_fp8: needs with_scaling = 1 (fp32 block scales)"); return false; }
+  if (d->with_zeros) { set_error("bb_matmul_fp8: zero points are not supported (with_zeros must be 0)"); return false; }
+  if (d->w_layout != BB_LAYOUT_COMPRESSED || d->w_tile != BB_TILE_ROW_MAJOR) {
+    set_error("bb_matmul_fp8: W must be row-major compressed storage (w_layout=%d, w_tile=%d)", d->w_layout, d->w_tile);
+    return false;
+  }
+  if (d->reserved[0] || d->reserved[1]) { set_error("reserved fields must be zero"); return false; }
+  if (d->N <= 0 || d->N % 16) { set_error("bb_matmul_fp8: needs N > 0 and N %% 16 == 0 (N=%d)", d->N); return false; }
+  if (d->K <= 0 || d->K % 128) { set_error("bb_matmul_fp8: needs K > 0 and K %% 128 == 0 (K=%d)", d->K); return false; }
+  return true;
+}
+
+static int select_fp8(int m) {
+  const int ov = g_override.load();
+  return m >= 1 && (ov == BB_KERNEL_AUTO || ov == BB_KERNEL_GEMM_FP8) ? BB_KERNEL_GEMM_FP8 : -1;
+}
+
+int bb_matmul_fp8(const bb_matmul_desc* desc, const void* A, const float* a_scale, int a_scale_ld, const void* W,
+                  const float* w_scale, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!fp8_desc_ok(desc)) return 1;
+  if (m == 0) return 0;
+  if (m < 0) { set_error("m must be >= 0 (got %d)", m); return 1; }
+  if (a_scale_ld < m || a_scale_ld % 4) {
+    set_error("bb_matmul_fp8: a_scale_ld must be >= m and a multiple of 4 (a_scale_ld=%d, m=%d)", a_scale_ld, m);
+    return 1;
+  }
+  if (!A || !W || !C) { set_error("A, W and C must be non-null"); return 1; }
+  if (!a_scale) { set_error("bb_matmul_fp8: a_scale must be non-null (fp32 [K/128][a_scale_ld], k-block-major)"); return 1; }
+  if (!w_scale) { set_error("bb_matmul_fp8: w_scale must be non-null (fp32 [ceil(N/128), K/128])"); return 1; }
+  if (desc->with_bias && !bias) { set_error("with_bias is set but bias is null"); return 1; }
+  if ((reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(W) & 15)) {
+    set_error("bb_matmul_fp8: A and W must be 16-byte aligned");
+    return 5;
+  }
+  if (reinterpret_cast<uintptr_t>(a_scale) & 15) { set_error("bb_matmul_fp8: a_scale must be 16-byte aligned"); return 5; }
+  if (reinterpret_cast<uintptr_t>(w_scale) & 3) { set_error("bb_matmul_fp8: w_scale must be 4-byte aligned"); return 5; }
+  if (select_fp8(m) < 0) {
+    set_error("bb_matmul_fp8: kernel override %d does not support this entry (AUTO or BB_KERNEL_GEMM_FP8)", g_override.load());
+    return 1;
+  }
+  Fp8Args a;
+  a.d = *desc; a.A = A; a.a_scale = a_scale; a.a_scale_ld = a_scale_ld; a.W = W; a.w_scale = w_scale;
+  a.bias = desc->with_bias ? bias : nullptr; a.C = C; a.m = m;
+  a.workspace = workspace; a.workspace_bytes = workspace ? workspace_bytes : 0; a.stream = (cudaStream_t)stream;
+  return launch_gemm_fp8(a);
+}
+
+int bb_select_kernel_fp8(const bb_matmul_desc* desc, int m) {
+  if (!fp8_desc_ok(desc)) return -1;
+  return select_fp8(m);
+}
+
+size_t bb_workspace_bytes_fp8(const bb_matmul_desc* desc, int m) {
+  if (!fp8_desc_ok(desc) || select_fp8(m) < 0) return 0;
+  return gemm_fp8_workspace_bytes(*desc, m);
 }
 
 int bb_matmul_scatter(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
@@ -670,6 +745,24 @@ int bb_quantize_act_int8(const void* x, int a_dtype, int rows, int K, int8_t* q,
   if (reinterpret_cast<uintptr_t>(q) & 15) { set_error("quantize act int8: q must be 16-byte aligned"); return 5; }
   if (reinterpret_cast<uintptr_t>(scale) & 3) { set_error("quantize act int8: scale must be 4-byte aligned"); return 5; }
   return launch_quantize_act_int8(x, a_dtype, rows, K, q, scale, (cudaStream_t)stream);
+}
+
+int bb_quantize_act_fp8(const void* x, int a_dtype, int rows, int K, void* q, float* scale, int scale_ld, void* stream) {
+  if (a_dtype != BB_F16 && a_dtype != BB_BF16) { set_error("quantize act fp8: x must be float16 or bfloat16 (a_dtype=%d)", a_dtype); return 1; }
+  if (K <= 0 || K % 128) { set_error("quantize act fp8: needs K > 0 and K %% 128 == 0 (K=%d)", K); return 1; }
+  if (rows < 0) { set_error("quantize act fp8: rows must be >= 0 (got %d)", rows); return 1; }
+  if (scale_ld < rows || scale_ld % 4) {
+    set_error("quantize act fp8: scale_ld must be >= rows and a multiple of 4 (scale_ld=%d, rows=%d)", scale_ld, rows);
+    return 1;
+  }
+  if (rows == 0) return 0;
+  if (!x) { set_error("quantize act fp8: x must be non-null"); return 1; }
+  if (!q) { set_error("quantize act fp8: q must be non-null"); return 1; }
+  if (!scale) { set_error("quantize act fp8: scale must be non-null"); return 1; }
+  if (reinterpret_cast<uintptr_t>(x) & 15) { set_error("quantize act fp8: x must be 16-byte aligned"); return 5; }
+  if (reinterpret_cast<uintptr_t>(q) & 15) { set_error("quantize act fp8: q must be 16-byte aligned"); return 5; }
+  if (reinterpret_cast<uintptr_t>(scale) & 15) { set_error("quantize act fp8: scale must be 16-byte aligned"); return 5; }
+  return launch_quantize_act_fp8(x, a_dtype, rows, K, static_cast<uint8_t*>(q), scale, scale_ld, (cudaStream_t)stream);
 }
 
 int bb_peer_barrier(void* const* peer_flags, int n_peers, int rank, void* stream) {

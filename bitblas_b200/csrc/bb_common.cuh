@@ -172,6 +172,24 @@ int launch_gemv_i8(const MatmulArgs& a);
 bool gemm_ts_supported(const bb_matmul_desc& d, int m);
 int launch_gemm_ts(const MatmulArgs& a);
 size_t gemm_ts_workspace_bytes(const bb_matmul_desc& d, int m);
+int gemm_ts_splits(int tiles, int num_kb, int sms);   // the wgmma GEMM's split-K factor for a tile grid and k-block count
+// one bb_matmul_fp8 call, validated by bb_api.cu (bb_gemm_fp8.cu)
+struct Fp8Args {
+  bb_matmul_desc d;
+  const void* A;          // e4m3 [m, K]
+  const float* a_scale;   // fp32, element (r, b) at a_scale[b * a_scale_ld + r]
+  int a_scale_ld;
+  const void* W;          // e4m3 [N, K]
+  const float* w_scale;   // fp32 [ceil(N / 128), K / 128]
+  const void* bias;       // [N] out_dtype, or null
+  void* C;
+  int m;
+  void* workspace;
+  size_t workspace_bytes;
+  cudaStream_t stream;
+};
+int launch_gemm_fp8(const Fp8Args& a);
+size_t gemm_fp8_workspace_bytes(const bb_matmul_desc& d, int m);
 // one grouped (mixture-of-experts) call, validated by bb_api.cu: num_groups problems of descriptor d, group e on rows
 // [offsets[e], offsets[e + 1]) of A and C; W, scale, zeros and bias are stacked over the groups
 struct GroupedArgs {
@@ -214,6 +232,8 @@ int launch_permute_cols(const void* A, void* out, const int32_t* perm, int rows,
                         cudaStream_t stream);
 // per-token int8 quantization of the activations, bb_quant.cu (validated by bb_quantize_act_int8 in bb_api.cu)
 int launch_quantize_act_int8(const void* x, int a_dtype, int rows, int K, int8_t* q, float* scale, cudaStream_t stream);
+// per-(token, 128-column block) e4m3 quantization, bb_quant.cu (validated by bb_quantize_act_fp8)
+int launch_quantize_act_fp8(const void* x, int a_dtype, int rows, int K, uint8_t* q, float* scale, int scale_ld, cudaStream_t stream);
 
 // bit position of logical element `o` (0 .. 32/bits-1) inside its 32-bit storage word, for each weight
 // layout (restates bitblas/quantization/utils.py:73-110 + testing/cpp/lop3_type_conversion/fast_decoding.hpp:30-95,607-668)

@@ -696,6 +696,8 @@ bool gemm_ts_supported(const bb_matmul_desc& d, int m) {
   return true;
 }
 
+int gemm_ts_splits(int tiles, int num_kb, int sms) { return choose_splits(tiles, num_kb, sms); }
+
 size_t gemm_ts_workspace_bytes(const bb_matmul_desc& d, int m) {
   if (m > 128) return 0;
   const int kb = d.a_dtype == BB_I8 ? 128 : 64;

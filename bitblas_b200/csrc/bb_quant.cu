@@ -1,4 +1,5 @@
-// bb_quant.cu -- per-token int8 quantization of 16-bit activations (bb_quantize_act_int8), BitNet b1.58's activation_quant:
+// bb_quant.cu -- quantization of 16-bit activations on the device.  bb_quantize_act_fp8 (below): e4m3 per (token, 128-column
+// block).  bb_quantize_act_int8: per-token int8, BitNet b1.58's activation_quant:
 //     amax = max_k |x[r, k]|,   s[r] = 127 * (1 / max(amax, 1e-5)),   q[r, k] = clamp(rint(x[r, k] * s[r]), -128, 127)
 // in fp32, each operation correctly rounded (the int8 matmuls' bb_matmul_scaled then divides by s[r]).  The scale is a reciprocal
 // and a product, not one division: that is what torch evaluates for BitNet's `127.0 / t` (Tensor.__rtruediv__ is
@@ -72,7 +73,64 @@ quantize_act_int8_kernel(const uint16_t* __restrict__ x, int K, int8_t* __restri
   pdl_launch_dependents();
 }
 
+// ---- bb_quantize_act_fp8: per (row, 128-column block) e4m3 quantization, vLLM's per_token_group_quant_fp8 with IEEE division:
+//     amax = max(max_{k in block} |x[r, k]|, 1e-10),   s[r, b] = amax / 448,   q[r, k] = e4m3_rn(clamp(x[r, k] / s[r, b], +-448))
+// Schedule: one half-warp per block, 16 lanes x one 16-byte vector of 8 values; the amax is four shuffles inside the half-warp,
+// and each lane stores its 8 e4m3 bytes as one 8-byte vector.  Consecutive half-warps take consecutive blocks of a row, so a
+// warp reads 512 contiguous bytes.  The scale goes to scale[b * scale_ld + r] (k-block-major, the GEMM's layout).
+constexpr int QUANT_FP8_THREADS = 256;
+constexpr float E4M3_MAX = 448.f;
+
+// two floats -> two e4m3 bytes (lo first), round to nearest even, saturating
+__device__ __forceinline__ uint32_t e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(QUANT_FP8_THREADS)
+quantize_act_fp8_kernel(const uint16_t* __restrict__ x, int rows, int K, uint8_t* __restrict__ q, float* __restrict__ scale,
+                        int scale_ld) {
+  const int nkb = K / 128;
+  const long long blk = (long long)blockIdx.x * (QUANT_FP8_THREADS / 16) + (threadIdx.x >> 4);
+  const int l = threadIdx.x & 15;
+  pdl_wait();
+  if (blk < (long long)rows * nkb) {   // (whole half-warps leave together: the shuffles below stay inside live ones)
+    const int r = int(blk / nkb), b = int(blk - (long long)r * nkb);
+    const size_t e0 = size_t(r) * K + size_t(b) * 128 + size_t(l) * 8;
+    float f[8];
+    unpack8<T>(*reinterpret_cast<const uint4*>(x + e0), f);
+    float amax = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) amax = fmaxf(amax, fabsf(f[i]));
+    const unsigned hmask = 0xffffu << (threadIdx.x & 16);
+#pragma unroll
+    for (int off = 8; off > 0; off >>= 1) amax = fmaxf(amax, __shfl_xor_sync(hmask, amax, off));
+    const float s = __fdiv_rn(fmaxf(amax, 1e-10f), E4M3_MAX);
+    uint32_t w[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float v[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) v[i] = fminf(fmaxf(__fdiv_rn(f[4 * h + i], s), -E4M3_MAX), E4M3_MAX);
+      w[h] = e4m3x2(v[0], v[1]) | (e4m3x2(v[2], v[3]) << 16);
+    }
+    *reinterpret_cast<uint2*>(q + e0) = make_uint2(w[0], w[1]);
+    if (l == 0) scale[size_t(b) * scale_ld + r] = s;
+  }
+  pdl_launch_dependents();
+}
+
 }  // namespace
+
+int launch_quantize_act_fp8(const void* x, int a_dtype, int rows, int K, uint8_t* q, float* scale, int scale_ld, cudaStream_t stream) {
+  const long long blocks = (long long)rows * (K / 128);
+  const unsigned grid = unsigned((blocks + QUANT_FP8_THREADS / 16 - 1) / (QUANT_FP8_THREADS / 16));
+  auto kernel = a_dtype == BB_F16 ? quantize_act_fp8_kernel<__half> : quantize_act_fp8_kernel<__nv_bfloat16>;
+  return launch_pdl(kernel, grid, QUANT_FP8_THREADS, 0, stream, pdl_enabled(), reinterpret_cast<const uint16_t*>(x), rows, K, q,
+                    scale, scale_ld);
+}
 
 int launch_quantize_act_int8(const void* x, int a_dtype, int rows, int K, int8_t* q, float* scale, cudaStream_t stream) {
   // one thread per 16-byte vector up to the block size, in whole warps

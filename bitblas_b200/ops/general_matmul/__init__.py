@@ -540,16 +540,20 @@ class Matmul(Operator):
                          a_scale=a_scale.data_ptr())
         return output
 
-    def _workspace_for(self, m: int, device: int, stream: int, w4a8: bool = False):
+    def _workspace_for(self, m: int, device: int, stream: int, w4a8: bool = False, fp8: bool = False):
         """scratch the kernel picked for `m` needs (bb_workspace_bytes: split-K partials, stream-K exchange slots; w4a8: of the
-        descriptor without group scales and zeros, which bb_matmul_w4a8's kernels need at most); one cached, ZERO-INITIALISED
-        buffer per operator, device (ordinal) and stream, grown on demand.  The m = 1 slab kernel leaves its slots zero-tagged,
-        so the buffer is reused by later calls on the same stream without clearing (include/bitblas_b200.h)."""
-        key = (int(m), _lib.OVERRIDE_GEN, w4a8)
+        descriptor without group scales and zeros, which bb_matmul_w4a8's kernels need at most; fp8: bb_workspace_bytes_fp8);
+        one cached, ZERO-INITIALISED buffer per operator, device (ordinal) and stream, grown on demand.  The m = 1 slab kernel
+        leaves its slots zero-tagged, so the buffer is reused by later calls on the same stream without clearing
+        (include/bitblas_b200.h)."""
+        key = (int(m), _lib.OVERRIDE_GEN, w4a8, fp8)
         need = self._ws_need.get(key)
         if need is None:
-            need = self._ws_need[key] = int(self.lib._c.bb_workspace_bytes(ctypes.byref(self._w4a8_cleared_desc() if w4a8 else
-                                                                                        self._desc), int(m)))
+            if fp8:
+                need = int(_lib.load().bb_workspace_bytes_fp8(ctypes.byref(self._fp8_desc()), int(m)))
+            else:
+                need = int(self.lib._c.bb_workspace_bytes(ctypes.byref(self._w4a8_cleared_desc() if w4a8 else self._desc), int(m)))
+            self._ws_need[key] = need
         if need == 0:
             return 0, 0
         wkey = (device, stream)
@@ -610,6 +614,77 @@ class Matmul(Operator):
         _, idx, stream = _lib.device_stream(A_q)
         self._launch_raw(A_q.data_ptr(), ptrs[0], 0, ptrs[1], ptrs[2], ptrs[3], output.data_ptr(), m, idx, stream,
                          a_scale=a_scale.data_ptr(), w4a8=True)
+        return output
+
+    def check_fp8(self) -> None:
+        """raise ValueError unless forward_fp8 covers this operator: A_dtype = W_dtype = "e4m3_float8", accum_dtype float32,
+        out_dtype float16 / bfloat16 / float32, N % 16 == 0 and K % 128 == 0"""
+        c = self.config
+        if c.A_dtype != "e4m3_float8" or c.W_dtype != "e4m3_float8":
+            raise ValueError(f"forward_fp8 needs A_dtype = W_dtype = 'e4m3_float8' (got {c.A_dtype}, {c.W_dtype})")
+        if c.accum_dtype != "float32":
+            raise ValueError(f"forward_fp8 needs accum_dtype='float32' (got {c.accum_dtype})")
+        if c.out_dtype not in ("float16", "bfloat16", "float32"):
+            raise ValueError(f"forward_fp8 needs out_dtype float16, bfloat16 or float32 (got {c.out_dtype})")
+        if c.N % 16 or c.K % 128:
+            raise ValueError(f"forward_fp8 needs N % 16 == 0 and K % 128 == 0 (N={c.N}, K={c.K})")
+
+    def _fp8_desc(self) -> _lib.MatmulDesc:
+        """the bb_matmul_fp8 descriptor of this operator: e4m3 x e4m3, fp32 scales in 128 x 128 blocks"""
+        d = getattr(self, "_fp8_desc_c", None)
+        if d is None:
+            c = self.config
+            d = self._fp8_desc_c = _lib.MatmulDesc()
+            d.N, d.K, d.a_dtype, d.w_fmt, d.w_bits = int(c.N), int(c.K), _lib.BB_E4M3, _lib.BB_W_FP8_E4M3, 8
+            d.accum_dtype, d.out_dtype, d.group_size = _lib.BB_F32, _lib.DTYPE_IDS[c.out_dtype], 128
+            d.with_scaling, d.with_bias = 1, int(bool(c.with_bias))
+        return d
+
+    def kernel_for_fp8(self, m: int) -> str:
+        """the kernel family forward_fp8 runs for m rows (bb_select_kernel_fp8)"""
+        self.check_fp8()
+        return _lib.kernel_name(_lib.load().bb_select_kernel_fp8(ctypes.byref(self._fp8_desc()), int(m)))
+
+    def forward_fp8(self, A_q, W, a_scale, w_scale, bias=None, output=None):
+        """Block-scaled FP8 matmul on the FP8 tensor cores in one launch (bb_matmul_fp8; two with split-K): A_q float8_e4m3fn
+        [.., K] with a_scale float32 [m, K/128] (quantize_act_fp8's transposed view of a k-block-major buffer: a_scale[r, b] at
+        b * ld + r), W float8_e4m3fn [N, K] with w_scale float32 [ceil(N/128), K/128], and output [.., N] = round(S) (+ bias, [N]
+        in the output dtype, added after the rounding) with S = sum_b P_b * (a_scale[r, b] * w_scale[n / 128, b]) in fp32 and
+        P_b the tensor core's sum over the 128 k of block b.  The kernel is kernel_for_fp8(m).  forward() on this operator
+        stays the fp16 widening path."""
+        self.check_fp8()
+        c = self.config
+        N, K, KB = int(c.N), int(c.K), int(c.K) // 128
+        e4m3 = torch.float8_e4m3fn
+        if not (isinstance(A_q, torch.Tensor) and A_q.is_cuda and A_q.dtype == e4m3 and A_q.is_contiguous()):
+            _lib.check_tensor(A_q, "A_q", e4m3)
+        if A_q.dim() < 1 or A_q.shape[-1] != K:
+            raise ValueError(f"A_q has inner dimension {A_q.shape[-1] if A_q.dim() else None}, expected K={K}")
+        m = A_q.numel() // K
+        dev = A_q.device
+        _lib.check_tensor(W, "W", e4m3, numel=N * K)
+        _lib.check_tensor(w_scale, "w_scale", torch.float32, numel=((N + 127) // 128) * KB)
+        if not isinstance(a_scale, torch.Tensor) or a_scale.dtype != torch.float32 or tuple(a_scale.shape) != (m, KB):
+            raise TypeError(f"a_scale must be a float32 [{m}, {KB}] torch.Tensor (quantize_act_fp8's scales)")
+        if not a_scale.is_cuda:
+            raise RuntimeError("a_scale must be a CUDA tensor: bitblas_b200 has no CPU path")
+        if m > 1 and a_scale.stride(0) != 1:
+            raise ValueError("a_scale must be k-block-major: the [m, K/128] transposed view of a [K/128, ld] buffer (stride(0) == 1)")
+        ld = a_scale.stride(1) if KB > 1 else (m + 3) // 4 * 4
+        if c.with_bias:
+            if bias is None:
+                raise ValueError("with_bias=True but bias is None")
+            _lib.check_tensor(bias, "bias", self.torch_output_dtype, numel=N)
+        elif bias is not None:
+            raise ValueError("the operator was built with with_bias=False but a bias was given")
+        for t in (W, w_scale, a_scale, bias):
+            if t is not None and t.device != dev:
+                raise ValueError(f"every operand must be on A_q's device {dev} (one is on {t.device})")
+        output = self._output_for(A_q, output, N)
+        _, idx, stream = _lib.device_stream(A_q)
+        ws_ptr, ws_bytes = self._workspace_for(m, idx, stream, fp8=True)
+        _lib.call("bb_matmul_fp8", idx, ctypes.byref(self._fp8_desc()), A_q.data_ptr(), a_scale.data_ptr(), ld, W.data_ptr(),
+                  w_scale.data_ptr(), bias.data_ptr() if bias is not None else 0, output.data_ptr(), m, ws_ptr, ws_bytes, stream)
         return output
 
     def forward_scatter(self, A, W, scale=None, zeros=None, bias=None, *, peer_ptrs, ldc: int, col_offset: int):

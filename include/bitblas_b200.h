@@ -35,7 +35,8 @@ typedef enum bb_dtype {
   BB_BF16 = 1,
   BB_F32 = 2,
   BB_I8 = 3,
-  BB_I32 = 4
+  BB_I32 = 4,
+  BB_E4M3 = 5  /* float8 e4m3 (OCP "fn": no infinities, max 448): activations of bb_matmul_fp8 only */
 } bb_dtype;
 
 /* weight source formats (Matmul.BITBLAS_TRICK_DTYPE_MAP, general_matmul/__init__.py:324-345) */
@@ -106,8 +107,9 @@ typedef enum bb_kernel_id {
   BB_KERNEL_GEMV_I8 = 3,   /* m <= 32, int8 A, 4/2-bit W: IMMA streaming, int32 exact         */
   BB_KERNEL_GEMM_TS = 4,   /* wgmma (W dequantised into registers as the MMA A operand) + TMA */
   BB_KERNEL_GEMM_TS_I8 = 5,/* wgmma int8 variant                                             */
-  BB_KERNEL_GEMV_SLAB = 7    /* m == 1, 4-bit W, fp16/bf16 A: per-CTA TMA slabs + CTA-level stream-K; the default
+  BB_KERNEL_GEMV_SLAB = 7,   /* m == 1, 4-bit W, fp16/bf16 A: per-CTA TMA slabs + CTA-level stream-K; the default
                               * decode kernel (needs the zero-initialised workspace of bb_workspace_bytes) */
+  BB_KERNEL_GEMM_FP8 = 8     /* bb_matmul_fp8 only: block-scaled e4m3 x e4m3 wgmma, both operands from shared memory */
 } bb_kernel_id;
 
 /* replaces `init()` (builder/wrapper/base.py:5-13): one-time per-device setup (opt-in shared memory
@@ -201,6 +203,44 @@ int bb_matmul_scaled(const bb_matmul_desc* desc, const void* A, const void* W, c
 int bb_matmul_w4a8(const bb_matmul_desc* desc, const void* A, const void* W, const float* a_scale, const float* scale,
                    const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes, void* stream);
 int bb_select_kernel_w4a8(const bb_matmul_desc* desc, int m);
+
+/* 128 x 128 block-scaled FP8 checkpoints (DeepSeek-V3 / R1, Qwen3 -FP8: weight float8_e4m3fn [N, K], weight_scale_inv fp32
+ * [ceil(N/128), K/128]) on the FP8 tensor cores, with activations quantized per (token, 128-column block) on the device.
+ *
+ * bb_quantize_act_fp8: x [rows, K] of a_dtype (float16 | bfloat16) -> q e4m3 bytes [rows, K] and one fp32 scale per (row r,
+ * block b = k / 128), each step correctly rounded in fp32 (vLLM's per_token_group_quant_fp8 with IEEE division):
+ *     amax[r, b] = max(max_{k in b} |float(x[r, k])|, 1e-10f)
+ *     s[r, b]    = amax[r, b] / 448.0f                                     (IEEE division)
+ *     q[r, k]    = e4m3_rn(clamp(float(x[r, k]) / s[r, b], -448, 448))     (IEEE division, round to nearest even)
+ * An all-zero block gives q = 0; Inf or NaN inputs give unspecified values.  The scales are k-block-major: (r, b) is
+ * scale[b * scale_ld + r], scale_ld >= rows and scale_ld % 4 == 0, so a GEMM tile's scales for one k-block are one contiguous,
+ * 16-byte-aligned run.  K % 128 == 0; x, q and scale 16-byte aligned (code 5 otherwise).  ONE launch, no workspace, CUDA-graph
+ * capturable; programmatic stream serialization as bb_quantize_act_int8.  rows == 0 validates and returns 0 without touching
+ * the device.
+ *
+ * bb_matmul_fp8: A e4m3 [m, K] with a_scale (bb_quantize_act_fp8's layout, a_scale_ld >= m, a_scale_ld % 4 == 0) against W e4m3
+ * [N, K] (the checkpoint's bytes, row-major) with w_scale fp32 [ceil(N/128), K/128] row-major.  desc: a_dtype = BB_E4M3, w_fmt =
+ * BB_W_FP8_E4M3, w_bits = 8, accum_dtype = BB_F32, out_dtype float16 | bfloat16 | float32, group_size = 128, with_scaling = 1,
+ * with_zeros = 0, compressed row-major storage; N % 16 == 0 (the last 128-row weight tile may be partial), K % 128 == 0.
+ *     P[r, n, b] = sum_{k in block b} q_a[r, k] * q_w[n, k]          tensor-core e4m3 MMA, fp32 accumulator
+ *     S[r, n]    = sum_b P[r, n, b] * (a_scale[r, b] * w_scale[n / 128, b])
+ *     C[r, n]    = round_out(S[r, n])   (+ bias[n], [N] in out_dtype, added after the rounding; an fp32 output is one sum)
+ * Each product of P is exact; how the tensor core accumulates the 128 products of a block is not specified.  S is fp32 with every
+ * product and sum rounded (no fma): S = (((0 + t_0) + t_1) + ...) with t_b = P[r, n, b] * (a_scale * w_scale), blocks ascending.
+ * Split s ways (split j owns blocks [j KB/s, (j+1) KB/s), KB = K/128), each split sums its own blocks from 0 as above, and
+ * S = ((0 + S_0) + S_1) + ... + S_{s-1}.  The split factor is gemm_ts's rule on this kernel's tiles (m <= 128, a tile grid that
+ * leaves SMs idle, at least 8 blocks per split) under bb_set_sm_count_cap; bb_workspace_bytes_fp8 is the fp32 [splits][m][N] it
+ * needs (0 without a split), and a smaller or null workspace runs unsplit.  Kernel: BB_KERNEL_GEMM_FP8 under AUTO or that
+ * override; any other override is refused (code 1), and bb_select_kernel_fp8 reports -1 then (and on an invalid desc or m < 1).
+ * Rejections, each with its own message: the descriptor, then m, then a_scale_ld, then null pointers (code 1), then A, W and
+ * a_scale not 16-byte aligned or w_scale not 4-byte aligned (code 5).  m == 0 returns 0 and launches nothing.  One launch, two
+ * with split-K, counted by bb_launch_count; no host synchronisation (CUDA-graph capturable); A and a_scale are read only after
+ * the preceding kernel has completed.  No other entry point accepts a_dtype = BB_E4M3. */
+int bb_quantize_act_fp8(const void* x, int a_dtype, int rows, int K, void* q, float* scale, int scale_ld, void* stream);
+int bb_matmul_fp8(const bb_matmul_desc* desc, const void* A, const float* a_scale, int a_scale_ld, const void* W,
+                  const float* w_scale, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes, void* stream);
+int bb_select_kernel_fp8(const bb_matmul_desc* desc, int m);
+size_t bb_workspace_bytes_fp8(const bb_matmul_desc* desc, int m);
 
 /* Grouped matmul for mixture-of-experts layers (no reference counterpart; the contract of torch._grouped_mm with offsets).
  * `num_groups` problems share `desc` and run as ONE kernel launch.  A[total_rows, K] holds the rows of every group, sorted so
