@@ -346,6 +346,24 @@ __device__ __forceinline__ uint32_t lds32(uint32_t addr) {
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
+// L2 eviction policies for the .L2::cache_hint copies below: evict_first for bytes read exactly once, evict_last for bytes that
+// later requests read again
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ void tma_load_2d_hint(uint32_t dst, const void* map, int c0, int c1, uint32_t bar, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3}], [%4], %5;"
+      ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar), "l"(policy)
+      : "memory");
+}
+__device__ __forceinline__ void bulk_g2s_hint(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint64_t policy) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "l"(policy)
+               : "memory");
+}
 
 template <typename T>
 struct TypeTraits;

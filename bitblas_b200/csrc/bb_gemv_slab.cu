@@ -28,6 +28,10 @@
 //     tensor cores and the raw parameters into fp32 (c1, c2) pairs, then completes the stage barrier.  The DRAM system runs
 //     saturated, so by Little's law EVERY request -- also a 1-byte parameter load -- takes (bytes in flight)/bandwidth, microseconds:
 //     anything fetched with plain loads "a few units ahead" stalls its warp on every unit.
+//   * L2 policy: the weight requests carry evict_first (each byte is read once).  Without it the weight stream pushes the
+//     parameter sectors out of L2 between the two units that share one, and the parameters cost 0.65-2.5 us per launch on top of
+//     the weights; tools/slab_stream.cu measures this (DESIGN.md 3.2).  Neither evict_last on the activation slab nor one L2
+//     prefetch of a row block's contiguous scale run paid in that replay, so neither is used.
 //   * stream-K fix-up: a range that starts inside a row block parks its group-reduced partial row sums in tagged 64-bit
 //     workspace slots {call nonce, fp32}; the range holding the block's first unit adds them in fixed order (bit-reproducible)
 //     and stores.  Ranges are handed out in reverse CTA order so an owner only waits for CTAs dispatched before it.
@@ -230,9 +234,11 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
     // =========================== issuer warp ===========================
     // one weight TMA box {128 x u32 = 512 B, 32 rows} -> dense [32][512 B] (rows past N / columns past K/2 are zero-filled and
     // never stored / consumed; the transaction count is always the full box), the activation slab, the raw parameters
+    // every weight byte is read exactly once: evict_first keeps the stream from displacing the parameter sectors and activation
+    // slabs that later units read again (tools/slab_stream.cu, DESIGN.md 3.2)
     auto unit_w = [&](int rb, int ku, int slot) {   // lane 0
-      if (p.Wt) gs_bulk_g2s(Wb + uint32_t(slot) * GS_WBYTES, p.Wt + (size_t(rb) * UPR + ku) * GS_WBYTES, GS_WBYTES, Bb + 8u * slot);
-      else tma_load_2d(Wb + uint32_t(slot) * GS_WBYTES, &tmW, ku * (GS_ROW_BYTES / 4), rb * GS_ROWS, Bb + 8u * slot);
+      if (p.Wt) bulk_g2s_hint(Wb + uint32_t(slot) * GS_WBYTES, p.Wt + (size_t(rb) * UPR + ku) * GS_WBYTES, GS_WBYTES, Bb + 8u * slot, l2_policy_evict_first());
+      else tma_load_2d_hint(Wb + uint32_t(slot) * GS_WBYTES, &tmW, ku * (GS_ROW_BYTES / 4), rb * GS_ROWS, Bb + 8u * slot, l2_policy_evict_first());
     };
     auto unit_params = [&](int rb, int ku, int slot) {   // all 32 lanes: lane = row of the unit
       const uint32_t bar = Bb + 8u * (2 * S + slot);
@@ -447,9 +453,10 @@ gemv_slab_kernel(const __grid_constant__ CUtensorMap tmW, const SlabParams p) {
     if (!seg_open) { seg_from0 = (ku == 0); seg_open = true; }
     const bool closes = (ku == UPR - 1);
     gs_mbar_wait(Bb + 8u * slot, fphase);   // weights + activations have landed
-    // (p.N > 0 always holds; the run-time term keeps ptxas's register allocation of the fp16 compressed-word instance: without it
-    //  that instance spills 38 / 64 B instead of 16 / 24 B, partly inside this loop, and runs 3-5 % slower on an H100)
-    const bool active = (!closes || ws < nsl_last) && rb < p.NRB && p.N > 0;
+    // (p.UPR > 0 always holds; the run-time term keeps ptxas's register allocation of the fp16 compressed-word instance: without it
+    //  that instance spills 38 / 64 B instead of 16 / 24 B, partly inside this loop, and runs 3-5 % slower on an H100.  Which term
+    //  does it depends on the rest of the kernel: since the weight copies carry an L2 policy, p.N > 0 no longer does, p.UPR > 0 does)
+    const bool active = (!closes || ws < nsl_last) && rb < p.NRB && p.UPR > 0;
     float cc[4][4];
     if (active) {
       const uint32_t wst = Wb + uint32_t(slot) * GS_WBYTES + woff;
