@@ -32,3 +32,4 @@ from .act_order import permute_cols  # noqa: E402,F401
 from .bitnet import BitLinear, quantize_act_int8  # noqa: E402,F401
 from .w4a8 import W4A8Linear  # noqa: E402,F401
 from .fp8 import FP8Linear, quantize_act_fp8  # noqa: E402,F401
+from .fp8_moe import FP8MoEExperts  # noqa: E402,F401

@@ -34,7 +34,8 @@ ZEROS_IDS = {"original": BB_ZEROS_ORIGINAL, "rescale": BB_ZEROS_RESCALE, "quanti
 
 EXPORTS = [
     "bb_init", "bb_matmul", "bb_matmul_swiglu", "bb_matmul_scaled", "bb_matmul_w4a8", "bb_select_kernel_w4a8", "bb_quantize_act_int8",
-    "bb_quantize_act_fp8", "bb_matmul_fp8", "bb_select_kernel_fp8", "bb_workspace_bytes_fp8", "bb_matmul_scatter", "bb_matmul_grouped", "bb_matmul_grouped_gemm", "bb_matmul_grouped_swiglu",
+    "bb_quantize_act_fp8", "bb_matmul_fp8", "bb_select_kernel_fp8", "bb_workspace_bytes_fp8", "bb_matmul_grouped_fp8",
+    "bb_matmul_grouped_fp8_swiglu", "bb_matmul_scatter", "bb_matmul_grouped", "bb_matmul_grouped_gemm", "bb_matmul_grouped_swiglu",
     "bb_matmul_grouped_gemm_swiglu", "bb_matmul_grouped_gemm_swiglu_gather", "bb_moe_route", "bb_moe_route_index",
     "bb_moe_combine", "bb_moe_topk", "bb_permute_cols", "bb_peer_barrier", "bb_workspace_bytes", "bb_select_kernel", "bb_kernel_name", "bb_set_kernel_override",
     "bb_set_sm_count_cap", "bb_launch_count", "bb_last_error", "bb_version", "bb_compress_host", "bb_interleave_host",
@@ -79,6 +80,8 @@ def load() -> ctypes.CDLL:
     lib.bb_matmul_fp8.argtypes = [dp, vp, vp, i32, vp, vp, vp, vp, i32, vp, sz, vp]; lib.bb_matmul_fp8.restype = i32
     lib.bb_select_kernel_fp8.argtypes = [dp, i32]; lib.bb_select_kernel_fp8.restype = i32
     lib.bb_workspace_bytes_fp8.argtypes = [dp, i32]; lib.bb_workspace_bytes_fp8.restype = sz
+    for f in (lib.bb_matmul_grouped_fp8, lib.bb_matmul_grouped_fp8_swiglu):
+        f.argtypes = [dp, i32, vp, vp, vp, i32, vp, vp, vp, i32, vp]; f.restype = i32
     lib.bb_matmul_scatter.argtypes = [dp, vp, vp, vp, vp, vp, vp, ctypes.POINTER(vp), i32, i64, i64, i32, vp, sz, vp]
     lib.bb_matmul_scatter.restype = i32
     lib.bb_matmul_grouped.argtypes = [dp, i32, vp, vp, vp, vp, vp, vp, vp, i32, vp]; lib.bb_matmul_grouped.restype = i32

@@ -494,6 +494,62 @@ size_t bb_workspace_bytes_fp8(const bb_matmul_desc* desc, int m) {
   return gemm_fp8_workspace_bytes(*desc, m);
 }
 
+// bb_matmul_grouped_fp8[_swiglu]: every rejection has its own message and code, so the order of the checks is part of the interface
+static int grouped_fp8_call(bool swiglu, const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A,
+                            const float* a_scale, int a_scale_ld, const void* W, const float* w_scale, void* C, int total_rows,
+                            void* stream) {
+  if (!fp8_desc_ok(desc)) return 1;
+  if (desc->N % 128) {
+    if (swiglu) set_error("grouped FP8 SwiGLU: desc->N = 2I needs 2I %% 128 == 0 (N=%d)", desc->N);
+    else set_error("grouped FP8: needs N %% 128 == 0 (an expert's 128-row tile must not read the next expert's rows; N=%d)", desc->N);
+    return 1;
+  }
+  if (desc->with_bias) { set_error("grouped FP8: with_bias must be 0 (expert biases are not supported)"); return 1; }
+  if (num_groups < 1 || num_groups > BB_GROUPED_MAX_GROUPS) {
+    set_error("num_groups must be in [1, %d] (got %d)", BB_GROUPED_MAX_GROUPS, num_groups);
+    return 1;
+  }
+  if (total_rows < 0) { set_error("total_rows must be >= 0 (got %d)", total_rows); return 1; }
+  if (total_rows == 0) return 0;
+  if (a_scale_ld < total_rows || a_scale_ld % 4) {
+    set_error("grouped FP8: a_scale_ld must be >= total_rows and a multiple of 4 (a_scale_ld=%d, total_rows=%d)", a_scale_ld,
+              total_rows);
+    return 1;
+  }
+  if (!offsets) { set_error("offsets must be a device pointer to num_groups + 1 int32 values"); return 1; }
+  if (!A || !W || !C) { set_error("A, W and C must be non-null"); return 1; }
+  if (!a_scale) { set_error("grouped FP8: a_scale must be non-null (fp32 [K/128][a_scale_ld], k-block-major)"); return 1; }
+  if (!w_scale) { set_error("grouped FP8: w_scale must be non-null (fp32 [E, N/128, K/128])"); return 1; }
+  if ((reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(W) & 15)) {
+    set_error("grouped FP8: A and W must be 16-byte aligned");
+    return 5;
+  }
+  if (reinterpret_cast<uintptr_t>(a_scale) & 15) { set_error("grouped FP8: a_scale must be 16-byte aligned"); return 5; }
+  if ((reinterpret_cast<uintptr_t>(w_scale) & 3) || (reinterpret_cast<uintptr_t>(offsets) & 3)) {
+    set_error("grouped FP8: w_scale and offsets must be 4-byte aligned");
+    return 5;
+  }
+  if (select_fp8(total_rows) < 0) {
+    set_error("grouped FP8: kernel override %d does not support this entry (AUTO or BB_KERNEL_GEMM_FP8)", g_override.load());
+    return 1;
+  }
+  GroupedFp8Args a;
+  a.d = *desc; a.num_groups = num_groups; a.offsets = offsets; a.A = A; a.a_scale = a_scale; a.a_scale_ld = a_scale_ld;
+  a.W = W; a.w_scale = w_scale; a.C = C; a.total_rows = total_rows; a.stream = (cudaStream_t)stream; a.swiglu = swiglu;
+  return launch_grouped_fp8(a);
+}
+
+int bb_matmul_grouped_fp8(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const float* a_scale,
+                          int a_scale_ld, const void* W, const float* w_scale, void* C, int total_rows, void* stream) {
+  return grouped_fp8_call(false, desc, num_groups, offsets, A, a_scale, a_scale_ld, W, w_scale, C, total_rows, stream);
+}
+
+int bb_matmul_grouped_fp8_swiglu(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A,
+                                 const float* a_scale, int a_scale_ld, const void* W, const float* w_scale, void* C, int total_rows,
+                                 void* stream) {
+  return grouped_fp8_call(true, desc, num_groups, offsets, A, a_scale, a_scale_ld, W, w_scale, C, total_rows, stream);
+}
+
 int bb_matmul_scatter(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
                       const void* zeros, const void* bias, void* const* peer_C, int n_peers, int64_t ldc,
                       int64_t col_offset, int m, void* workspace, size_t workspace_bytes, void* stream) {

@@ -190,6 +190,22 @@ struct Fp8Args {
 };
 int launch_gemm_fp8(const Fp8Args& a);
 size_t gemm_fp8_workspace_bytes(const bb_matmul_desc& d, int m);
+// one bb_matmul_grouped_fp8[_swiglu] call, validated by bb_api.cu (bb_grouped_fp8.cu)
+struct GroupedFp8Args {
+  bb_matmul_desc d;
+  int num_groups;
+  const int32_t* offsets;   // [num_groups + 1], device
+  const void* A;            // e4m3 [total_rows, K]
+  const float* a_scale;     // fp32, element (r, b) at a_scale[b * a_scale_ld + r]
+  int a_scale_ld;
+  const void* W;            // e4m3 [E, N, K]
+  const float* w_scale;     // fp32 [E, N / 128, K / 128]; swiglu: [E, 2 ceil(N / 256), K / 128], gate and up blocks alternating
+  void* C;                  // [total_rows, N] (swiglu: [total_rows, N / 2]) out_dtype
+  int total_rows;
+  cudaStream_t stream;
+  bool swiglu;
+};
+int launch_grouped_fp8(const GroupedFp8Args& a);
 // one grouped (mixture-of-experts) call, validated by bb_api.cu: num_groups problems of descriptor d, group e on rows
 // [offsets[e], offsets[e + 1]) of A and C; W, scale, zeros and bias are stacked over the groups
 struct GroupedArgs {

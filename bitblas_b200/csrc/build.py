@@ -9,7 +9,7 @@ PKG = os.path.dirname(HERE)
 OUT_DIR = os.path.join(PKG, "lib")
 OBJ_DIR = os.path.join(HERE, "build")
 SOURCES = ["bb_api.cu", "bb_generic.cu", "bb_gemv.cu", "bb_gemv_slab.cu", "bb_gemm_ts.cu", "bb_grouped.cu", "bb_grouped_gemm.cu",
-           "bb_moe.cu", "bb_permute.cu", "bb_prep.cu", "bb_quant.cu", "bb_gemm_fp8.cu"]
+           "bb_moe.cu", "bb_permute.cu", "bb_prep.cu", "bb_quant.cu", "bb_gemm_fp8.cu", "bb_grouped_fp8.cu"]
 HEADERS = ["bb_common.cuh", "bb_gemv_mma.cuh", "bb_gemm_ts.cuh", "bb_wgmma.inc", os.path.join(PKG, "..", "include", "bitblas_b200.h")]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v" if os.environ.get("BB_PTXAS_V") else "-O3"]

@@ -10,7 +10,10 @@ tokens), more than the copy costs, at every measured point.
 Gate/up interleave (include/bitblas_b200.h): the fused gate/up projection of I rows each is stored as 2I rows in which stored row
 16b + i is gate row 8b + i for i < 8 and up row 8b + i - 8 for i >= 8.  Every per-row buffer follows the same permutation:
 the weight, scales and zeros ([.., 2I, *]) and the bias ([.., 2I]) along their row axis; quantized zeros ([.., G, 2I*bits/8],
-packed along the rows) in whole bytes, 8 rows being `bits` bytes.
+packed along the rows) in whole bytes, 8 rows being `bits` bytes.  The 128 x 128 block scales of a block-scaled FP8 weight
+([.., ceil(I/128), K/128], kind "block_scale") alternate by block: stored scale row 2c is gate block c and row 2c + 1 up block c.
+A 128-row tile t of the stored weight holds gate rows 64t .. 64t + 63 and up rows 64t .. 64t + 63, so its scales are stored
+rows 2(t >> 1) and 2(t >> 1) + 1.
 """
 from __future__ import annotations
 
@@ -21,8 +24,10 @@ from . import _lib
 from .act_order import perm_from_g_idx, permute_cols, permute_gptq_rows
 
 INTERLEAVE_ROWS = 8
-# kind -> (axis holding the rows, rows per element along it: None = 1, "bits" = 8 / bits packed rows per byte)
-_KINDS = {"weight": (-2, None), "scale": (-2, None), "zeros": (-2, None), "bias": (-1, None), "qzeros": (-1, "bits")}
+# kind -> (axis holding the rows, rows per element along it: None = 1, "bits" = 8 / bits packed rows per byte, "block" = one
+# element per 128 rows)
+_KINDS = {"weight": (-2, None), "scale": (-2, None), "zeros": (-2, None), "bias": (-1, None), "qzeros": (-1, "bits"),
+          "block_scale": (-2, "block")}
 
 
 def _block(kind, bits):
@@ -31,6 +36,8 @@ def _block(kind, bits):
     dim, packed = _KINDS[kind]
     if packed is None:
         return dim, INTERLEAVE_ROWS
+    if packed == "block":
+        return dim, 1
     if bits not in (2, 4):
         raise ValueError("quantized zeros need bits = 4 or 2 (8 rows are `bits` whole bytes)")
     return dim, INTERLEAVE_ROWS * bits // 8
@@ -38,7 +45,8 @@ def _block(kind, bits):
 
 def interleave_gate_up(gate: torch.Tensor, up: torch.Tensor, kind: str, bits: int = None) -> torch.Tensor:
     """gate, up [.., I, ..] (the rows on the axis of `kind`) -> the stored [.., 2I, ..] of the gate/up interleave.  kind: "weight",
-    "scale", "zeros", "bias", or "qzeros" (quantized zeros packed along the rows; needs `bits`).  CPU or CUDA tensors."""
+    "scale", "zeros", "bias", "qzeros" (quantized zeros packed along the rows; needs `bits`), or "block_scale" (FP8 128 x 128
+    block scales [.., ceil(I/128), K/128] -> [.., 2 ceil(I/128), K/128]).  CPU or CUDA tensors."""
     dim, blk = _block(kind, bits)
     if gate.shape != up.shape:
         raise ValueError(f"gate and up must have the same shape (got {tuple(gate.shape)} and {tuple(up.shape)})")

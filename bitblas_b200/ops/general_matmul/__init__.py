@@ -664,13 +664,7 @@ class Matmul(Operator):
         dev = A_q.device
         _lib.check_tensor(W, "W", e4m3, numel=N * K)
         _lib.check_tensor(w_scale, "w_scale", torch.float32, numel=((N + 127) // 128) * KB)
-        if not isinstance(a_scale, torch.Tensor) or a_scale.dtype != torch.float32 or tuple(a_scale.shape) != (m, KB):
-            raise TypeError(f"a_scale must be a float32 [{m}, {KB}] torch.Tensor (quantize_act_fp8's scales)")
-        if not a_scale.is_cuda:
-            raise RuntimeError("a_scale must be a CUDA tensor: bitblas_b200 has no CPU path")
-        if m > 1 and a_scale.stride(0) != 1:
-            raise ValueError("a_scale must be k-block-major: the [m, K/128] transposed view of a [K/128, ld] buffer (stride(0) == 1)")
-        ld = a_scale.stride(1) if KB > 1 else (m + 3) // 4 * 4
+        ld = self._fp8_a_scale_ld(a_scale, m)
         if c.with_bias:
             if bias is None:
                 raise ValueError("with_bias=True but bias is None")
@@ -685,6 +679,87 @@ class Matmul(Operator):
         ws_ptr, ws_bytes = self._workspace_for(m, idx, stream, fp8=True)
         _lib.call("bb_matmul_fp8", idx, ctypes.byref(self._fp8_desc()), A_q.data_ptr(), a_scale.data_ptr(), ld, W.data_ptr(),
                   w_scale.data_ptr(), bias.data_ptr() if bias is not None else 0, output.data_ptr(), m, ws_ptr, ws_bytes, stream)
+        return output
+
+    def _fp8_a_scale_ld(self, a_scale, m: int) -> int:
+        """the a_scale_ld of quantize_act_fp8's scales for m rows: a float32 CUDA [m, K/128] transposed view of a k-block-major
+        [K/128, ld] buffer"""
+        KB = int(self.config.K) // 128
+        if not isinstance(a_scale, torch.Tensor) or a_scale.dtype != torch.float32 or tuple(a_scale.shape) != (m, KB):
+            raise TypeError(f"a_scale must be a float32 [{m}, {KB}] torch.Tensor (quantize_act_fp8's scales)")
+        if not a_scale.is_cuda:
+            raise RuntimeError("a_scale must be a CUDA tensor: bitblas_b200 has no CPU path")
+        if m > 1 and a_scale.stride(0) != 1:
+            raise ValueError("a_scale must be k-block-major: the [m, K/128] transposed view of a [K/128, ld] buffer (stride(0) == 1)")
+        return a_scale.stride(1) if KB > 1 else (m + 3) // 4 * 4
+
+    # ---- grouped (mixture-of-experts) block-scaled FP8 --------------------------------------------------------------------------
+    def check_grouped_fp8(self, num_groups: int, swiglu: bool = False) -> None:
+        """raise ValueError unless bb_matmul_grouped_fp8 (swiglu: bb_matmul_grouped_fp8_swiglu) covers this operator with
+        `num_groups` experts: check_fp8, then the library's own checks with total_rows = 0 (nothing touches the device)"""
+        self.check_fp8()
+        name = "bb_matmul_grouped_fp8_swiglu" if swiglu else "bb_matmul_grouped_fp8"
+        rc = getattr(_lib.load(), name)(ctypes.byref(self._fp8_desc()), int(num_groups), 0, 0, 0, 0, 0, 0, 0, 0, 0)
+        if rc != 0:
+            raise ValueError(f"{name} does not cover this configuration: {_lib.last_error()}")
+
+    def forward_grouped_fp8(self, A_q, W, offsets, a_scale, w_scale, output=None):
+        """Grouped block-scaled FP8 matmul for mixture-of-experts layers in ONE graph-capturable launch (bb_matmul_grouped_fp8):
+        A_q float8_e4m3fn [T, K] sorted so that expert e owns rows [offsets[e], offsets[e+1]) (offsets int32 CUDA [E + 1], read
+        on the device), a_scale quantize_act_fp8's float32 [T, K/128] scales of A_q, W float8_e4m3fn [E, N, K] and w_scale
+        float32 [E, N/128, K/128].  For every expert e, output[offsets[e]:offsets[e+1]] is forward_fp8 of those rows against W[e]
+        run unsplit, bit for bit.  Offsets are clamped to [0, T]; rows no expert claims are not written."""
+        N = int(self.config.N)
+        return self._grouped_fp8("bb_matmul_grouped_fp8", A_q, W, offsets, a_scale, w_scale, output, N // 128, N)
+
+    def forward_grouped_fp8_swiglu(self, A_q, W, offsets, a_scale, w_scale, output=None):
+        """The gate/up projection of a block-scaled FP8 SwiGLU expert block in ONE launch (bb_matmul_grouped_fp8_swiglu): this
+        operator's N = 2I rows of W [E, 2I, K] hold gate and up in the gate/up interleave (moe.interleave_gate_up kind "weight")
+        and w_scale [E, 2 ceil(I/128), K/128] their scales interleaved by block (kind "block_scale").  output [T, I] =
+        silu(g) * u, rounded once, with g and u exactly what forward_grouped_fp8 stores for the gate and up rows.  Operands and
+        offsets otherwise as forward_grouped_fp8."""
+        I = int(self.config.N) // 2
+        return self._grouped_fp8("bb_matmul_grouped_fp8_swiglu", A_q, W, offsets, a_scale, w_scale, output, 2 * -(-I // 128), I,
+                                 swiglu=True)
+
+    def _grouped_fp8(self, name, A_q, W, offsets, a_scale, w_scale, output, s_rows, out_cols, swiglu=False):
+        c = self.config
+        N, K, KB = int(c.N), int(c.K), int(c.K) // 128
+        e4m3 = torch.float8_e4m3fn
+        if not isinstance(offsets, torch.Tensor) or offsets.dtype != torch.int32:
+            raise TypeError("offsets must be an int32 torch.Tensor of num_groups + 1 row offsets")
+        if offsets.dim() != 1 or not 2 <= offsets.numel() <= _lib.BB_GROUPED_MAX_GROUPS + 1:
+            raise ValueError(f"offsets must be 1-D with num_groups + 1 entries, 1 <= num_groups <= {_lib.BB_GROUPED_MAX_GROUPS} "
+                             f"(got shape {tuple(offsets.shape)})")
+        E = offsets.numel() - 1
+        key = (name, E)
+        if key != getattr(self, "_grouped_fp8_checked", None):
+            self.check_grouped_fp8(E, swiglu)
+            self._grouped_fp8_checked = key
+        _lib.check_tensor(A_q, "A_q", e4m3, 2)
+        if A_q.shape[1] != K:
+            raise ValueError(f"A_q must be [T, K={K}], got {tuple(A_q.shape)}")
+        T = A_q.shape[0]
+        _lib.check_tensor(W, "W", e4m3, 3)
+        if tuple(W.shape) != (E, N, K):
+            raise ValueError(f"W must be [E={E}, {N}, {K}] (got {tuple(W.shape)})")
+        _lib.check_tensor(w_scale, "w_scale", torch.float32, 3)
+        if tuple(w_scale.shape) != (E, s_rows, KB):
+            raise ValueError(f"w_scale must be [E={E}, {s_rows}, {KB}] (got {tuple(w_scale.shape)})")
+        _lib.check_tensor(offsets, "offsets", torch.int32)
+        ld = self._fp8_a_scale_ld(a_scale, T)
+        if output is None:
+            output = torch.empty((T, out_cols), dtype=self.torch_output_dtype, device=A_q.device)
+        else:
+            _lib.check_tensor(output, "output", self.torch_output_dtype)
+            if tuple(output.shape) != (T, out_cols):
+                raise ValueError(f"output must be [T={T}, {out_cols}] (got {tuple(output.shape)})")
+        for t in (W, w_scale, a_scale, offsets, output):
+            if t.device != A_q.device:
+                raise ValueError(f"every operand must be on A_q's device {A_q.device} (one is on {t.device})")
+        _, idx, stream = _lib.device_stream(A_q)
+        _lib.call(name, idx, ctypes.byref(self._fp8_desc()), E, offsets.data_ptr(), A_q.data_ptr(), a_scale.data_ptr(), ld,
+                  W.data_ptr(), w_scale.data_ptr(), output.data_ptr(), T, stream)
         return output
 
     def forward_scatter(self, A, W, scale=None, zeros=None, bias=None, *, peer_ptrs, ldc: int, col_offset: int):

@@ -235,7 +235,7 @@ int bb_select_kernel_w4a8(const bb_matmul_desc* desc, int m);
  * Rejections, each with its own message: the descriptor, then m, then a_scale_ld, then null pointers (code 1), then A, W and
  * a_scale not 16-byte aligned or w_scale not 4-byte aligned (code 5).  m == 0 returns 0 and launches nothing.  One launch, two
  * with split-K, counted by bb_launch_count; no host synchronisation (CUDA-graph capturable); A and a_scale are read only after
- * the preceding kernel has completed.  No other entry point accepts a_dtype = BB_E4M3. */
+ * the preceding kernel has completed.  No other entry point but bb_matmul_grouped_fp8[_swiglu] accepts a_dtype = BB_E4M3. */
 int bb_quantize_act_fp8(const void* x, int a_dtype, int rows, int K, void* q, float* scale, int scale_ld, void* stream);
 int bb_matmul_fp8(const bb_matmul_desc* desc, const void* A, const float* a_scale, int a_scale_ld, const void* W,
                   const float* w_scale, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes, void* stream);
@@ -292,6 +292,37 @@ int bb_matmul_grouped_gemm_swiglu_gather(const bb_matmul_desc* desc, int num_gro
                                          const int32_t* row_index, const void* A, int a_rows, const void* W,
                                          const void* scale, const void* zeros, const void* bias, void* C,
                                          int total_rows, void* stream);
+
+/* Grouped block-scaled FP8 matmul for mixture-of-experts layers whose experts are 128 x 128 block-scaled e4m3 checkpoints
+ * (DeepSeek-V3 / R1, Qwen3 -FP8): ONE launch over num_groups experts with the offset contract of bb_matmul_grouped, and for
+ * every expert e the numerics of bb_matmul_fp8 without a split:
+ *     C[r, n] = round_out(S[r, n]),  S[r, n] = sum_b P[r, n, b] * (a_scale[r, b] * w_scale[e, n / 128, b])   for offsets[e] <= r < offsets[e+1]
+ * P the tensor core's e4m3 sum over block b (each product exact; its order within the block unspecified); S is fp32 with every
+ * product and sum rounded (no fma), S = (((0 + t_0) + t_1) + ...), blocks ascending; round_out casts to out_dtype (fp32 stays).
+ * So each expert's rows equal bb_matmul_fp8 on those rows and W[e] run unsplit (without a workspace), bit for bit.
+ *   - A e4m3 [total_rows, K], sorted by expert; a_scale its bb_quantize_act_fp8 scales, k-block-major: (r, b) at
+ *     a_scale[b * a_scale_ld + r], a_scale_ld >= total_rows, a_scale_ld % 4 == 0.
+ *   - W e4m3 [E, N, K], the checkpoint's per-expert [N, K] bytes stacked; w_scale fp32 [E, N/128, K/128].
+ *   - offsets: a DEVICE int32 array of num_groups + 1 entries, read by the kernel; clamped to [0, total_rows], a group whose end
+ *     is below its start is empty, rows no group claims are not written.  1 <= num_groups <= BB_GROUPED_MAX_GROUPS.
+ *   - desc: that of bb_matmul_fp8, with N % 128 == 0 (an expert's 128-row tile must not read the next expert's rows) and
+ *     with_bias = 0.  No workspace.
+ * bb_matmul_grouped_fp8_swiglu, the gate/up projection: desc->N = 2I rows of W[e] in the gate/up interleave (stored row 16b + i
+ * is gate row 8b + i for i < 8 and up row 8b + i - 8 for i >= 8; 2I % 128 == 0), so stored 128-row tile t holds gate and up rows
+ * 64t .. 64t + 63.  Its scales are interleaved by block: w_scale fp32 [E, 2 ceil(I/128), K/128], row 2c the gate block c and row
+ * 2c + 1 the up block c, so tile t reads rows 2(t >> 1) and 2(t >> 1) + 1.  C is [total_rows, I]:
+ *     C[r, c] = round_out(silu(g) * u),   silu(g) = g / (1 + exp(-g)) in fp32, one rounding,
+ * with g and u exactly what the plain call would store for gate row c and up row c of the de-interleaved weights and scales.
+ * Rejections, each with its own message: the descriptor (bb_matmul_fp8's checks), N % 128, with_bias, num_groups, total_rows < 0
+ * (code 1); total_rows == 0 then validates and returns 0 without touching the device; then a_scale_ld, null pointers (code 1),
+ * A, W and a_scale not 16-byte aligned or w_scale and offsets not 4-byte aligned (code 5), and a kernel override other than AUTO
+ * or BB_KERNEL_GEMM_FP8 (code 1).  ONE launch counted by bb_launch_count, no host synchronisation (CUDA-graph capturable),
+ * programmatic stream serialization; offsets, A, a_scale and W are read only after the preceding kernel has completed. */
+int bb_matmul_grouped_fp8(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A, const float* a_scale,
+                          int a_scale_ld, const void* W, const float* w_scale, void* C, int total_rows, void* stream);
+int bb_matmul_grouped_fp8_swiglu(const bb_matmul_desc* desc, int num_groups, const int32_t* offsets, const void* A,
+                                 const float* a_scale, int a_scale_ld, const void* W, const float* w_scale, void* C, int total_rows,
+                                 void* stream);
 
 /* Mixture-of-experts routing on the device: slot s = t * top_k + j of the DEVICE int32 table topk_ids [num_tokens, top_k] goes to
  * expert topk_ids[s].  Writes offsets [num_experts + 1] (the offsets of bb_matmul_grouped), slot_rows [T * top_k] (the sorted row
