@@ -1,8 +1,11 @@
 """GPU: block-scaled FP8 (bb_quantize_act_fp8, bb_matmul_fp8, FP8Linear).
 
-  * quantization bit for bit against the torch restatement of the rule (include/bitblas_b200.h), edge values included;
+  * quantization bit for bit against the torch restatement of the rule (include/bitblas_b200.h), edge values included, and
+    every finite float16 and bfloat16 encoding as a block's amax and beneath nine others;
   * the GEMM bit for bit on exactly representable inputs: every BM instance, split and unsplit (asserted), every output type,
     with and without bias, N % 128 != 0, K = 128 and 512, at capped SM counts;
+  * the GEMM bit for bit on exact block sums with inexact scales against the header's fp32 order (fp8_restate): every BM
+    instance, every output type, with and without bias, a_scale_ld > m, every split factor 2 .. 8 and the unsplit C call;
   * random inputs against float64 with a per-element bound (the accumulation assumption is stated at ACC_REL);
   * determinism, graph replay, launch counts and a PDL chain through reused buffers;
   * FP8Linear end to end and its float-weight loader.
@@ -14,12 +17,13 @@ import torch
 
 from bitblas_b200 import _lib
 from bitblas_b200.fp8 import FP8Linear, quantize_act_fp8, quantize_weight_blocks
+import fp8_restate as R
+from fp8_restate import OUT, round_out
 from test_fp8_api import fp8_splits
 
 pytestmark = pytest.mark.gpu
 
 E4M3 = torch.float8_e4m3fn
-OUT = {"float16": torch.float16, "bfloat16": torch.bfloat16, "float32": torch.float32}
 # How the tensor core sums the 128 products of one k-block is not specified.  Measured on an H100 (tools/fp8_accum_probe.py,
 # DESIGN.md §3.2.6): each k32 step aligns its 32 products and the running sum to the largest of them and drops what lies more
 # than 13 binades below it.  So each of the 4 steps loses less than 33 * 2^-13 of a value no larger than sum_k |a_k w_k|, and the
@@ -89,6 +93,45 @@ def test_quant_edges(dtype):
     assert qf.abs().max() <= 448 and not torch.isnan(qf).any()
 
 
+def _every_finite(dtype):
+    v = torch.arange(-32768, 32768, dtype=torch.int32).to(torch.int16).view(dtype)
+    return v[torch.isfinite(v)]
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16], ids=str)
+def test_quant_every_encoding(dtype):
+    """every finite bit pattern of the input type, once as its block's amax (with 127 smaller values of either sign beside it)
+    and once as a smaller element of blocks whose amax is 448 * 2^j (the scale a power of two: quotients land exactly on every
+    e4m3 value, the ties between them and the subnormals), 1, 0.1, 1000, the type's largest and smallest normal value and, in
+    bfloat16, amax values below the 1e-10 floor -- byte for byte against the CPU restatement"""
+    g = torch.Generator().manual_seed(5)
+    v = _every_finite(dtype)
+    # 1. each value as the amax of its block, at a position that moves with the value
+    frac = torch.rand(127, generator=g) * 2 - 1
+    blk = torch.cat([v[:, None], (v.float()[:, None] * frac[None, :]).to(dtype)], 1)
+    shift = (torch.arange(128)[None, :] + torch.arange(v.numel())[:, None]) % 128
+    blocks = [torch.gather(blk, 1, shift)]
+    assert torch.equal(blocks[0].float().abs().amax(1), v.float().abs())
+    # 2. each value under larger amax values
+    fi = torch.finfo(dtype)
+    amaxes = [448.0 * 2.0 ** j for j in (-24, -8, 0, 7)] + [1.0, 0.1, 1000.0, fi.max, fi.tiny]
+    if dtype == torch.bfloat16:
+        amaxes += [448.0 * 2.0 ** 100, 448.0 * 2.0 ** -120, 1e-12]
+    for a in torch.tensor(amaxes).to(dtype):
+        x = v[v.float().abs() <= a.float()]
+        x = torch.cat([x, torch.zeros((-x.numel()) % 127, dtype=dtype)]).view(-1, 127)
+        blocks.append(torch.cat([a.expand(x.shape[0], 1), x], 1))
+    blocks = torch.cat(blocks)
+    blocks = torch.cat([blocks, torch.zeros((-blocks.shape[0]) % 64, 128, dtype=dtype)])
+    x = blocks.view(-1, 64 * 128)
+    q, s = quantize_act_fp8(x.cuda())
+    qr, sr = quant_ref(x)
+    bad = (_bytes(q).cpu() != _bytes(qr)).nonzero()
+    assert bad.numel() == 0, f"{bad.shape[0]} bytes differ, first at {bad[:4].tolist()}: x = {x[tuple(bad[0])].item()!r}"
+    assert torch.equal(s.cpu(), sr)
+    assert torch.equal(torch.unique(_bytes(qr)), torch.tensor([b for b in range(256) if b & 0x7f != 0x7f], dtype=torch.uint8))
+
+
 def test_quant_scale_ld_and_pdl_order():
     """scale_ld > rows through the C entry: the gap between the rows' scales is not written"""
     lib = _lib.load()
@@ -132,13 +175,6 @@ def exact_S(qa, qw, sa, sw):
     terms = P * sa.double()[:, None, :] * swn[None, :, :]
     assert float(terms.abs().sum(-1).max()) < 2.0 ** 17      # every fp32 partial sum of S is a multiple of 2^-6 below 2^17
     return terms.sum(-1)
-
-
-def round_out(S, out, bias):
-    y = S.to(OUT[out])
-    if bias is not None:
-        y = y + bias
-    return y
 
 
 def _dev(qa, qw, sa, sw):
@@ -222,6 +258,66 @@ def test_split_and_unsplit_forced():
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     assert n_split == (2 if fp8_splits(N, K, m, sms) > 1 else 1)
     assert torch.equal(y, y_split) and torch.equal(y, exact_S(qa, qw, sa, sw).float().cuda())
+
+
+# ---- inexact scales: the header's fp32 order, bit for bit (fp8_restate) ----------------------------------------------------------
+def _sms():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+@pytest.mark.parametrize("m,N,K", R.FP8_CASES, ids=lambda v: str(v))
+def test_inexact_scales_restated(m, N, K):
+    """integer operands (the block sums exact) with inexact scales, so the promotion, block order, split reduce and output
+    rounding decide every bit: every output type, with and without a bias, the latter with a_scale_ld > m and NaN in the gap"""
+    qa, qw, sa, sw = R.fp8_case(m, N, K)
+    sp = fp8_splits(N, K, m, _sms())
+    S = R.restate(qa.cuda(), qw.cuda(), sa.cuda(), sw.cuda(), sp)
+    A, W, w_scale = qa.to(E4M3).cuda(), qw.to(E4M3).cuda(), sw.cuda()
+    for out in OUT:
+        for bias in (False, True):
+            b = R.bias_for(N, out, m + N).cuda() if bias else None
+            a_scale = R.a_scale_view(sa, 8 if bias else 0, "cuda")
+            y, launches = _run_counted(_op(N, K, out, bias), A, W, a_scale, w_scale, b)
+            assert launches == (2 if sp > 1 else 1)
+            assert torch.equal(y, round_out(S, out, b)), (out, bias, int((y != round_out(S, out, b)).sum()))
+
+
+@pytest.mark.parametrize("f,m,N,K,cap", R.SPLIT_CASES, ids=lambda v: str(v))
+def test_split_factors_restated(f, m, N, K, cap):
+    """every split factor 2 .. 8, asserted through bb_workspace_bytes_fp8, against the restated per-split sums and ordered
+    reduce; the same call through the C ABI without a workspace runs unsplit and matches the unsplit restatement"""
+    lib = _lib.load()
+    cap = cap or 132
+    if cap > _sms():
+        pytest.skip("the split factors are those of 132 SMs")
+    qa, qw, sa, sw = R.split_case(f, m, N, K, cap)
+    P, swn = R.block_sums(qa.cuda(), qw.cuda()), R.scale_rows(sw.cuda(), N)
+    R.prove_exact(qa, qw)
+    S_split, S_one = R.promote(P, sa.cuda(), swn, f), R.promote(P, sa.cuda(), swn, 1)
+    A, W, w_scale = qa.to(E4M3).cuda(), qw.to(E4M3).cuda(), sw.cuda()
+    a_scale = R.a_scale_view(sa, 4, "cuda")
+    stream = torch.cuda.current_stream().cuda_stream
+    prev = lib.bb_set_sm_count_cap(cap)
+    try:
+        for out in OUT:
+            for bias in (False, True):
+                op = _op(N, K, out, bias)
+                assert lib.bb_workspace_bytes_fp8(ctypes.byref(op._fp8_desc()), m) == f * m * N * 4
+                b = R.bias_for(N, out, f).cuda() if bias else None
+                y, launches = _run_counted(op, A, W, a_scale, w_scale, b)
+                assert launches == 2 and torch.equal(y, round_out(S_split, out, b)), (out, bias)
+                y1 = torch.empty_like(y)
+                n0 = lib.bb_launch_count()
+                rc = lib.bb_matmul_fp8(ctypes.byref(op._fp8_desc()), A.data_ptr(), a_scale.data_ptr(), a_scale.stride(1),
+                                       W.data_ptr(), w_scale.data_ptr(), b.data_ptr() if bias else 0, y1.data_ptr(), m, 0, 0,
+                                       stream)
+                torch.cuda.synchronize()
+                assert rc == 0 and lib.bb_launch_count() - n0 == 1
+                assert torch.equal(y1, round_out(S_one, out, b)), (out, bias)
+                if out == "float32":
+                    assert not torch.equal(y, y1)   # the split order shows in the bits
+    finally:
+        lib.bb_set_sm_count_cap(prev)
 
 
 # ---- random inputs against float64 ---------------------------------------------------------------------------------------------

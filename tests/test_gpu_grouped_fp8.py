@@ -4,6 +4,8 @@
     every BM instance (asserted through the mirror grouped_bm), both forms, every output type, empty experts, all rows in one
     expert, descending and out-of-range offsets with unclaimed rows left untouched, E = 1 and E = 256, N = 128 and K = 128, T not
     a multiple of BM, and capped SM counts;
+  * exact block sums with inexact scales (fp8_restate), bit for bit against the header's fp32 order restated per expert: every
+    BM bucket, both forms, every output type, experts starting at rows not = 0 mod 4, E = 1 and 256, capped SM counts;
   * random inputs: bit-identical to per-expert bb_matmul_fp8 run unsplit where every expert is in the instance's BM bucket,
     within test_gpu_fp8's float64 bound elsewhere; the SwiGLU form bit-identical to torch silu * mul on the plain call's output
     for the de-interleaved weights;
@@ -21,6 +23,8 @@ from bitblas_b200 import _lib
 from bitblas_b200.fp8 import quantize_act_fp8, quantize_weight_blocks
 from bitblas_b200.fp8_moe import FP8MoEExperts
 from bitblas_b200.moe import deinterleave_gate_up, interleave_gate_up, moe_combine, moe_route
+import fp8_restate as R
+from fp8_restate import silu_mul
 from test_gpu_fp8 import ACC_REL, OUT, exact_case, exact_S, float64_bound
 
 pytestmark = pytest.mark.gpu
@@ -86,12 +90,6 @@ def exact_grouped(counts_or_offsets, T, N, K, seed, swiglu=False):
     dev = (qa.to(E4M3).to(DEV), _a_scale(sa), W.to(E4M3).to(DEV), ws.to(DEV).contiguous(),
            torch.tensor(offsets, dtype=torch.int32, device=DEV))
     return dev, qa, sa, host
-
-
-def silu_mul(g, u, out):
-    """the header's SwiGLU rule: g and u as stored (out_dtype), silu in fp32, one rounding"""
-    gf, uf = g.float(), u.float()
-    return (gf / (1 + torch.exp(-gf)) * uf).to(OUT[out])
 
 
 def exact_reference(qa, sa, host, offsets, T, N, out, swiglu, sentinel):
@@ -182,6 +180,47 @@ def test_exact_capped_sm_counts(cap):
         for bm, counts in ROUTINGS.items():
             for swiglu in (False, True):
                 run_exact(_offsets(counts), sum(counts), 384, 1024, "bfloat16", swiglu, seed=bm * 3 + swiglu)
+    finally:
+        lib.bb_set_sm_count_cap(prev)
+
+
+# ---- inexact scales: the header's fp32 order, bit for bit (fp8_restate) ----------------------------------------------------------
+@pytest.mark.parametrize("swiglu", [False, True], ids=["plain", "swiglu"])
+@pytest.mark.parametrize("case", list(R.GROUPED_CASES))
+def test_inexact_scales_restated(case, swiglu):
+    """integer operands (the block sums exact) with inexact scales, every output type, a_scale_ld > T with NaN in the gap:
+    each expert's rows equal the restated order on those rows (the SwiGLU form: g and u restated on the de-interleaved gate
+    and up rows, rounded to out_dtype, then silu(g) * u on the device)"""
+    counts, N, K, cap, bm = R.GROUPED_CASES[case]
+    off = R.offsets_of(counts)
+    T, E = off[-1], len(counts)
+    assert grouped_bm(T, E) == bm
+    qa, sa, experts = R.grouped_case(counts, N, K, swiglu)
+    stack = lambda i, j: torch.stack([halves[i][j] for halves in experts])
+    if swiglu:
+        W = interleave_gate_up(stack(0, 0), stack(1, 0), "weight")
+        ws = interleave_gate_up(stack(0, 1), stack(1, 1), "block_scale")
+    else:
+        W, ws = stack(0, 0), stack(0, 1)
+    A, a_scale = qa.to(E4M3).to(DEV), R.a_scale_view(sa, 8, DEV)
+    W, ws, offsets = W.to(E4M3).to(DEV), ws.to(DEV), torch.tensor(off, dtype=torch.int32, device=DEV)
+    qa, sa = qa.to(DEV), sa.to(DEV)
+    S = [[R.restate(qa[off[e]:off[e + 1]], qw.to(DEV), sa[off[e]:off[e + 1]], sw.to(DEV)) for qw, sw in halves]
+         if off[e + 1] > off[e] else None for e, halves in enumerate(experts)]
+    lib = _lib.load()
+    prev = lib.bb_set_sm_count_cap(cap)
+    try:
+        for out in OUT:
+            op = _op(N, K, out)
+            fwd = op.forward_grouped_fp8_swiglu if swiglu else op.forward_grouped_fp8
+            y, n = _launches(lambda: fwd(A, W, offsets, a_scale, ws))
+            assert n == 1
+            for e, Se in enumerate(S):
+                if Se is None:
+                    continue
+                Ye = [R.round_out(s, out) for s in Se]
+                ref = silu_mul(*Ye, out) if swiglu else Ye[0]
+                assert torch.equal(y[off[e]:off[e + 1]], ref), (out, e, int((y[off[e]:off[e + 1]] != ref).sum()))
     finally:
         lib.bb_set_sm_count_cap(prev)
 
