@@ -321,31 +321,32 @@ static int select_w4a8(const bb_matmul_desc& d, int m) {
   return k;
 }
 
-// scaled: bb_matmul_scaled's two scales, or (w4a8) bb_matmul_w4a8's a_scale and group scales (null for every other entry point)
-static int matmul_impl(bool swiglu, const ScaledArgs* scaled, bool w4a8, const bb_matmul_desc* desc, const void* A, const void* W,
+// scaled: the scales of the Scaled and W4A8 forms (null in the other two)
+static int matmul_impl(MatmulForm form, const ScaledArgs& scaled, const bb_matmul_desc* desc, const void* A, const void* W,
                        const void* lut, const void* scale, const void* zeros, const void* bias, void* C, void* const* peer_C,
                        int n_peers, long long ldc, long long col_offset, int m, void* workspace, size_t workspace_bytes,
                        void* stream) {
   if (validate(desc)) return 1;
-  if (swiglu) {
+  if (form == MatmulForm::SwiGLU) {
     if (desc->a_dtype == BB_I8) { set_error("bb_matmul_swiglu: int8 activations are not supported (float16 | bfloat16)"); return 1; }
     if (!swiglu_shape_ok(desc)) return 1;
   }
-  if (scaled && !(w4a8 ? w4a8_desc_ok(desc) : scaled_desc_ok(desc))) return 1;
+  if (form == MatmulForm::Scaled && !scaled_desc_ok(desc)) return 1;
+  if (form == MatmulForm::W4A8 && !w4a8_desc_ok(desc)) return 1;
   if (m == 0) return 0;  // wrapper/tl.py:156-157
   if (m < 0) { set_error("m must be >= 0 (got %d)", m); return 1; }
   if (!A || !W || (!C && n_peers == 0)) { set_error("A, W and C must be non-null"); return 1; }
-  if (w4a8) {
-    if (!scaled->a_scale) { set_error("bb_matmul_w4a8: a_scale must be non-null (fp32 [m], one scale per row of A)"); return 1; }
-    if (!scaled->w_scale) { set_error("bb_matmul_w4a8: scale must be non-null (fp32 [N, K/g] group scales)"); return 1; }
-    if ((reinterpret_cast<uintptr_t>(scaled->a_scale) & 3) || (reinterpret_cast<uintptr_t>(scaled->w_scale) & 3)) {
+  if (form == MatmulForm::W4A8) {
+    if (!scaled.a_scale) { set_error("bb_matmul_w4a8: a_scale must be non-null (fp32 [m], one scale per row of A)"); return 1; }
+    if (!scaled.w_scale) { set_error("bb_matmul_w4a8: scale must be non-null (fp32 [N, K/g] group scales)"); return 1; }
+    if ((reinterpret_cast<uintptr_t>(scaled.a_scale) & 3) || (reinterpret_cast<uintptr_t>(scaled.w_scale) & 3)) {
       set_error("bb_matmul_w4a8: a_scale and scale must be 4-byte aligned");
       return 5;
     }
-  } else if (scaled) {
-    if (!scaled->a_scale) { set_error("bb_matmul_scaled: a_scale must be non-null (fp32 [m], one scale per row of A)"); return 1; }
-    if (!scaled->w_scale) { set_error("bb_matmul_scaled: w_scale must be non-null (fp32 [N], one scale per output column)"); return 1; }
-    if ((reinterpret_cast<uintptr_t>(scaled->a_scale) & 3) || (reinterpret_cast<uintptr_t>(scaled->w_scale) & 3)) {
+  } else if (form == MatmulForm::Scaled) {
+    if (!scaled.a_scale) { set_error("bb_matmul_scaled: a_scale must be non-null (fp32 [m], one scale per row of A)"); return 1; }
+    if (!scaled.w_scale) { set_error("bb_matmul_scaled: w_scale must be non-null (fp32 [N], one scale per output column)"); return 1; }
+    if ((reinterpret_cast<uintptr_t>(scaled.a_scale) & 3) || (reinterpret_cast<uintptr_t>(scaled.w_scale) & 3)) {
       set_error("bb_matmul_scaled: a_scale and w_scale must be 4-byte aligned");
       return 5;
     }
@@ -365,10 +366,9 @@ static int matmul_impl(bool swiglu, const ScaledArgs* scaled, bool w4a8, const b
   a.n_peers = n_peers; a.ldc = n_peers ? ldc : desc->N; a.col_offset = n_peers ? col_offset : 0;
   for (int i = 0; i < BB_MAX_PEERS; ++i) a.peer_C[i] = (i < n_peers) ? peer_C[i] : nullptr;
   a.workspace = workspace; a.workspace_bytes = workspace_bytes; a.stream = (cudaStream_t)stream;
-  a.swiglu = swiglu;
-  if (scaled) a.scaled = *scaled;
-  a.w4a8 = w4a8;
-  const int k = w4a8 ? select_w4a8(a.d, m) : select(a.d, m);
+  a.form = form;
+  a.scaled = scaled;
+  const int k = form == MatmulForm::W4A8 ? select_w4a8(a.d, m) : select(a.d, m);
   if (n_peers > 0 && k == BB_KERNEL_GENERIC) {
     set_error("the column-parallel scatter epilogue needs a fast kernel (gemv_mma / gemv_i8 / gemm_ts); this configuration dispatches to generic_simt");
     return 1;
@@ -388,31 +388,27 @@ static int matmul_impl(bool swiglu, const ScaledArgs* scaled, bool w4a8, const b
 int bb_matmul(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
               const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes,
               void* stream) {
-  return matmul_impl(false, nullptr, false, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
+  return matmul_impl(MatmulForm::Plain, {}, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
                      stream);
 }
 
 int bb_matmul_swiglu(const bb_matmul_desc* desc, const void* A, const void* W, const void* lut, const void* scale,
                      const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes,
                      void* stream) {
-  return matmul_impl(true, nullptr, false, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
+  return matmul_impl(MatmulForm::SwiGLU, {}, desc, A, W, lut, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
                      stream);
 }
 
 int bb_matmul_scaled(const bb_matmul_desc* desc, const void* A, const void* W, const float* a_scale, const float* w_scale,
                      const void* bias, void* C, int m, void* workspace, size_t workspace_bytes, void* stream) {
-  ScaledArgs sc;
-  sc.a_scale = a_scale; sc.w_scale = w_scale;
-  return matmul_impl(false, &sc, false, desc, A, W, nullptr, nullptr, nullptr, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
-                     stream);
+  return matmul_impl(MatmulForm::Scaled, {a_scale, w_scale}, desc, A, W, nullptr, nullptr, nullptr, bias, C, nullptr, 0, 0, 0, m,
+                     workspace, workspace_bytes, stream);
 }
 
 int bb_matmul_w4a8(const bb_matmul_desc* desc, const void* A, const void* W, const float* a_scale, const float* scale,
                    const void* zeros, const void* bias, void* C, int m, void* workspace, size_t workspace_bytes, void* stream) {
-  ScaledArgs sc;
-  sc.a_scale = a_scale; sc.w_scale = scale;
-  return matmul_impl(false, &sc, true, desc, A, W, nullptr, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace, workspace_bytes,
-                     stream);
+  return matmul_impl(MatmulForm::W4A8, {a_scale, scale}, desc, A, W, nullptr, scale, zeros, bias, C, nullptr, 0, 0, 0, m, workspace,
+                     workspace_bytes, stream);
 }
 
 int bb_select_kernel_w4a8(const bb_matmul_desc* desc, int m) {
@@ -554,7 +550,7 @@ int bb_matmul_scatter(const bb_matmul_desc* desc, const void* A, const void* W, 
                       const void* zeros, const void* bias, void* const* peer_C, int n_peers, int64_t ldc,
                       int64_t col_offset, int m, void* workspace, size_t workspace_bytes, void* stream) {
   if (n_peers < 1) { set_error("bb_matmul_scatter needs n_peers >= 1"); return 1; }
-  return matmul_impl(false, nullptr, false, desc, A, W, lut, scale, zeros, bias, nullptr, peer_C, n_peers, ldc, col_offset, m, workspace,
+  return matmul_impl(MatmulForm::Plain, {}, desc, A, W, lut, scale, zeros, bias, nullptr, peer_C, n_peers, ldc, col_offset, m, workspace,
                      workspace_bytes, stream);
 }
 

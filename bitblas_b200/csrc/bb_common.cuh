@@ -39,8 +39,12 @@ extern std::atomic<uint64_t> g_launches;
     }                                                                                        \
   } while (0)
 
-// the two fp32 quantization scales of bb_matmul_scaled: a_scale [m] (the preceding kernel's output, read after the PDL wait) and
-// w_scale [N]; both null for every other call
+// The output form of a single-matrix matmul: Plain (bb_matmul, bb_matmul_scatter), SwiGLU (bb_matmul_swiglu: W holds gate/up
+// interleaved, d.N = 2I rows, and C is [m, d.N / 2] = silu(gate) * up), Scaled (bb_matmul_scaled: the dequantizing epilogue
+// store_out_scaled) and W4A8 (bb_matmul_w4a8: per-group fp32 weight scales, store_out_dequant)
+enum class MatmulForm : int { Plain, SwiGLU, Scaled, W4A8 };
+// the fp32 scales the Scaled and W4A8 forms read (both null in the other forms): a_scale [m], one per row of A (the preceding
+// kernel's output, read after the PDL wait); w_scale: Scaled's per-column weight scales [N], W4A8's group scales [N, K/g]
 struct ScaledArgs {
   const float* a_scale = nullptr;
   const float* w_scale = nullptr;
@@ -64,11 +68,8 @@ struct MatmulArgs {
   void* workspace;
   size_t workspace_bytes;
   cudaStream_t stream;
-  bool swiglu;           // bb_matmul_swiglu: W holds gate/up interleaved (d.N = 2I rows), C is [m, d.N / 2] = silu(gate) * up
-  ScaledArgs scaled;     // bb_matmul_scaled (int8 activations): the dequantizing epilogue store_out_scaled
-  // bb_matmul_w4a8: per-group fp32 weight scales; `scaled` then holds a_scale [m] and, as w_scale, the group scales [N, K/g]
-  bool w4a8 = false;
-  bool is_scaled() const { return scaled.a_scale != nullptr; }
+  MatmulForm form;
+  ScaledArgs scaled;
   int groups() const { return d.K / (d.group_size <= 0 ? d.K : d.group_size); }
   int gsize() const { return d.group_size <= 0 ? d.K : d.group_size; }
 };
@@ -296,7 +297,7 @@ inline OutSpec make_outspec(void* C, long long ld) {   // the single output C
   return o;
 }
 inline OutSpec make_outspec(const MatmulArgs& a) {
-  if (a.n_peers == 0) return make_outspec(a.C, a.swiglu ? a.d.N / 2 : a.d.N);
+  if (a.n_peers == 0) return make_outspec(a.C, a.form == MatmulForm::SwiGLU ? a.d.N / 2 : a.d.N);
   OutSpec o;
   o.n = a.n_peers;
   for (int i = 0; i < BB_MAX_PEERS; ++i) o.ptr[i] = i < a.n_peers ? a.peer_C[i] : nullptr;

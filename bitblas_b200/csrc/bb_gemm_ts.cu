@@ -27,15 +27,15 @@ namespace bb {
 namespace {
 
 // FMT: 0 = integer formats (LOP3 magic-number decode), 1 = 16-entry table formats (NF4 / fp4; BITS = 4, compressed storage),
-//      2 = 8-bit float weights (e4m3 / e5m2; BITS = 8).  SWIGLU (16-bit activations only): bb_matmul_swiglu -- without split-K the
-//      epilogue is store_tile_swiglu; with it the raw partials are written as in the plain instance and splitk_reduce_kernel forms
-//      silu(gate) * up.  SCALED (int8 activations only): bb_matmul_scaled -- without split-K the tile is stored through
+//      2 = 8-bit float weights (e4m3 / e5m2; BITS = 8).  F = SwiGLU (16-bit activations only): bb_matmul_swiglu -- without split-K
+//      the epilogue is store_tile_swiglu; with it the raw partials are written as in the plain instance and splitk_reduce_kernel
+//      forms silu(gate) * up.  F = Scaled (int8 activations only): bb_matmul_scaled -- without split-K the tile is stored through
 //      store_out_scaled; with it the raw int32 partials are written as in the plain instance and splitk_reduce_kernel scales them.
 //      The scales are a parameter of their own (null in every other instance): TsParams is also the grouped GEMM's.
-//      W4A8 (int8 activations, 4-bit weights): bb_matmul_w4a8 -- per-group fp32 scales (sc.w_scale [N, G]) and zero points,
+//      F = W4A8 (int8 activations, 4-bit weights): bb_matmul_w4a8 -- per-group fp32 scales (sc.w_scale [N, G]) and zero points,
 //      promoted from exact int32 group sums into fp32 (main loop below); the tile, or the split's fp32 partial, ends in
 //      store_out_dequant / splitk_reduce_w4a8.
-template <typename T, int BITS, int BM, bool IL, int FMT = 0, bool SWIGLU = false, bool SCALED = false, bool W4A8 = false>
+template <typename T, int BITS, int BM, bool IL, int FMT, MatmulForm F>
 __global__ void __launch_bounds__(TS_THREADS, 1)
 gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const TsParams p,
                const ScaledArgs sc) {
@@ -109,7 +109,7 @@ gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const uint32_t zp4 = uint32_t(p.zp_const) * 0x01010101u;
   const uint32_t srcA = smem_u32(sW) + uint32_t(rA * PRB), srcB = srcA + 8u * PRB;
 
-  if constexpr (W4A8) {
+  if constexpr (F == MatmulForm::W4A8) {
     // Each group's k-blocks accumulate, exactly, into acc; the first wgmma of a group overwrites it (scale-d = 0).  Every k-block
     // decodes its fragments while the previous k-block's MMAs run, then wait<0> retires those MMAs; at a group's first k-block
     // the finished group is promoted into facc with its scale, and the new MMAs are issued.  So one k-block's MMAs are in flight
@@ -292,13 +292,13 @@ gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 
   // ----- epilogue: acc[4i + 2h + j] = C^T[row rA + 8h][column 8i + 2t + j] -> C[m, n] -----
-  if constexpr (SWIGLU) {
+  if constexpr (F == MatmulForm::SwiGLU) {
     if (p.splits == 1) {
       store_tile_swiglu<T, BM>(acc, p, reinterpret_cast<const T*>(p.bias), m0, p.M, nA, nB, t);
       return;
     }
   }
-  if constexpr (SCALED) {
+  if constexpr (F == MatmulForm::Scaled) {
     if (p.splits == 1) {
       const float swA = sc.w_scale[nA], swB = sc.w_scale[nB];
 #pragma unroll
@@ -316,7 +316,7 @@ gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
   }
   float bias_f[2] = {0.f, 0.f};
-  if (!SCALED && p.bias) {   // (a scaled call's bias is out_dtype, read by splitk_reduce_scaled)
+  if (F != MatmulForm::Scaled && p.bias) {   // (a scaled call's bias is out_dtype, read by splitk_reduce_scaled)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int n = h ? nB : nA;
@@ -372,7 +372,7 @@ gemm_ts_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 }
 
-// splitk_reduce_kernel of the SWIGLU instances: out[m, c] = silu(g) * u for the output columns c = 8b + i, with g and u the plain
+// splitk_reduce_kernel of the SwiGLU instances: out[m, c] = silu(g) * u for the output columns c = 8b + i, with g and u the plain
 // reduce's values of rows 16b + i and 16b + i + 8 (the same split order and rounding).  One thread = 4 consecutive c, which never
 // straddle a block of 8 (N / 2 % 4 == 0): one 128-bit load of gate and one of up partials per split.
 __device__ __forceinline__ void splitk_reduce_swiglu(const TsParams& p) {
@@ -409,7 +409,7 @@ __device__ __forceinline__ void splitk_reduce_swiglu(const TsParams& p) {
   }
 }
 
-// splitk_reduce_kernel of the SCALED int8 instances: the exact int32 sum of the partials through store_out_scaled, so split and
+// splitk_reduce_kernel of the Scaled int8 instances: the exact int32 sum of the partials through store_out_scaled, so split and
 // unsplit calls store the same bits
 __device__ __forceinline__ void splitk_reduce_scaled(const TsParams& p, const ScaledArgs& sc) {
   const unsigned n4 = unsigned(p.N) >> 2;
@@ -450,18 +450,18 @@ __device__ __forceinline__ void splitk_reduce_w4a8(const TsParams& p, const Scal
 
 // out[m, n] = cast(sum_s ws[s][m][n]) (+ bias), stored to every destination of the OutSpec.  One thread = 4 consecutive n
 // (N is a multiple of 128 here): 128-bit loads of the partials, 32-bit index arithmetic, one vector store per destination.
-// SWIGLU: splitk_reduce_swiglu; SCALED: splitk_reduce_scaled; W4A8: splitk_reduce_w4a8.
-template <bool INT8, bool SWIGLU = false, bool SCALED = false, bool W4A8 = false>
+// F = SwiGLU: splitk_reduce_swiglu; Scaled: splitk_reduce_scaled; W4A8: splitk_reduce_w4a8.
+template <bool INT8, MatmulForm F>
 __global__ void splitk_reduce_kernel(const TsParams p, const ScaledArgs sc) {
-  if constexpr (W4A8) {
+  if constexpr (F == MatmulForm::W4A8) {
     splitk_reduce_w4a8(p, sc);
     return;
   }
-  if constexpr (SWIGLU) {
+  if constexpr (F == MatmulForm::SwiGLU) {
     splitk_reduce_swiglu(p);
     return;
   }
-  if constexpr (SCALED) {
+  if constexpr (F == MatmulForm::Scaled) {
     splitk_reduce_scaled(p, sc);
     return;
   }
@@ -584,11 +584,11 @@ int choose_splits_w4a8(int tiles, int num_kb, int groups, int sms) {
   return sp;
 }
 
-template <typename T, int BITS, int BM, bool IL, int FMT, bool SWIGLU, bool SCALED, bool W4A8 = false>
+template <typename T, int BITS, int BM, bool IL, int FMT, MatmulForm F>
 int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
   using SM = TsSmem<T, BITS, BM>;
   using EI = ElemInfo<T>;
-  auto kernel = gemm_ts_kernel<T, BITS, BM, IL, FMT, SWIGLU, SCALED, W4A8>;
+  auto kernel = gemm_ts_kernel<T, BITS, BM, IL, FMT, F>;
   static KernelCache<> cache;
   if (!kernel_setup(cache, kernel, SM::kTotal)) {
     set_error("gemm_ts: cannot raise the kernel's dynamic shared memory to %d bytes on this device", SM::kTotal);
@@ -598,7 +598,7 @@ int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
   p.m_tiles = (a.m + BM - 1) / BM;
   const int num_kb_total = a.d.K / EI::kKB;
   const int tiles = p.m_tiles * (a.d.N / TS_ROWS);
-  if constexpr (W4A8) p.splits = a.m <= 128 ? choose_splits_w4a8(tiles, num_kb_total, p.G, device_sm_count()) : 1;
+  if constexpr (F == MatmulForm::W4A8) p.splits = a.m <= 128 ? choose_splits_w4a8(tiles, num_kb_total, p.G, device_sm_count()) : 1;
   else p.splits = a.m <= 128 ? choose_splits(tiles, num_kb_total, device_sm_count()) : 1;
   const size_t ws_off = splitk_partials_offset();
   if (p.splits > 1 && a.workspace_bytes < ws_off + size_t(p.splits) * a.m * a.d.N * 4) p.splits = 1;  // no scratch given
@@ -622,47 +622,40 @@ int launch_ts_inst(const MatmulArgs& a, const TsParams& p0) {
   kernel<<<grid, TS_THREADS, smem_bytes, a.stream>>>(tmA, tmW, p, a.scaled);
   BB_LAUNCH_CHECK();
   if (p.splits > 1) {
-    const size_t total = size_t(a.m) * a.d.N / (SWIGLU ? 8 : 4);   // one thread per 4 consecutive output columns
+    const size_t total = size_t(a.m) * a.d.N / (F == MatmulForm::SwiGLU ? 8 : 4);   // one thread per 4 consecutive output columns
     const int rthreads = 256;
     const int rblocks = int(std::min<size_t>((total + rthreads - 1) / rthreads, size_t(device_sm_count()) * 8));
-    if constexpr (W4A8) splitk_reduce_kernel<true, false, false, true><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
-    else if constexpr (SCALED) splitk_reduce_kernel<true, false, true><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
-    else if (EI::kInt8) splitk_reduce_kernel<true><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
-    else if (SWIGLU) splitk_reduce_kernel<false, true><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
-    else splitk_reduce_kernel<false><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
+    splitk_reduce_kernel<EI::kInt8, F><<<rblocks, rthreads, 0, a.stream>>>(p, a.scaled);
     BB_LAUNCH_CHECK();
   }
   return 0;
 }
 
-// activation rows per CTA: the wgmma N extent (m > 128 runs several 128-row tiles)
-template <typename T, int BITS, bool IL, int FMT, bool SWIGLU, bool SCALED>
-int launch_ts_bm_sw(const MatmulArgs& a, const TsParams& p) {
-  if (a.m <= 32) return launch_ts_inst<T, BITS, 32, IL, FMT, SWIGLU, SCALED>(a, p);
-  if (a.m <= 64) return launch_ts_inst<T, BITS, 64, IL, FMT, SWIGLU, SCALED>(a, p);
-  return launch_ts_inst<T, BITS, 128, IL, FMT, SWIGLU, SCALED>(a, p);
-}
-// (the int8 instances have no SWIGLU form: bb_matmul_swiglu rejects int8 activations; only they have a SCALED form:
-// bb_matmul_scaled rejects 16-bit ones)
-template <typename T, int BITS, bool IL, int FMT>
+// activation rows per CTA: the wgmma N extent (m > 128 runs several 128-row tiles).  W4A8 stops at 64: at 128 its fp32 group sums
+// do not fit beside the int32 accumulators (ptxas spills)
+template <typename T, int BITS, bool IL, int FMT, MatmulForm F>
 int launch_ts_bm(const MatmulArgs& a, const TsParams& p) {
-  if constexpr (!std::is_same<T, int8_t>::value) {
-    if (a.swiglu) return launch_ts_bm_sw<T, BITS, IL, FMT, true, false>(a, p);
-  } else {
-    if (a.is_scaled()) return launch_ts_bm_sw<T, BITS, IL, FMT, false, true>(a, p);
+  if (a.m <= 32) return launch_ts_inst<T, BITS, 32, IL, FMT, F>(a, p);
+  if constexpr (F != MatmulForm::W4A8) {
+    if (a.m > 64) return launch_ts_inst<T, BITS, 128, IL, FMT, F>(a, p);
   }
-  return launch_ts_bm_sw<T, BITS, IL, FMT, false, false>(a, p);
+  return launch_ts_inst<T, BITS, 64, IL, FMT, F>(a, p);
+}
+// the forms built for each activation type: 16-bit ones run Plain and SwiGLU (bb_matmul_swiglu rejects int8 activations), int8
+// ones Plain, Scaled and W4A8 (bb_matmul_scaled and bb_matmul_w4a8 reject 16-bit ones; bb_matmul_w4a8 takes 4-bit weights only)
+template <typename T, int BITS, bool IL, int FMT>
+int launch_ts_form(const MatmulArgs& a, const TsParams& p) {
+  if constexpr (!std::is_same<T, int8_t>::value) {
+    if (a.form == MatmulForm::SwiGLU) return launch_ts_bm<T, BITS, IL, FMT, MatmulForm::SwiGLU>(a, p);
+  } else {
+    if (a.form == MatmulForm::Scaled) return launch_ts_bm<T, BITS, IL, FMT, MatmulForm::Scaled>(a, p);
+    if (a.form == MatmulForm::W4A8) return launch_ts_bm<T, 4, IL, FMT, MatmulForm::W4A8>(a, p);
+  }
+  return launch_ts_bm<T, BITS, IL, FMT, MatmulForm::Plain>(a, p);
 }
 template <typename T, int BITS>
 int launch_ts_layout(const MatmulArgs& a, const TsParams& p) {
-  return a.d.w_layout == BB_LAYOUT_COMPRESSED ? launch_ts_bm<T, BITS, false, 0>(a, p) : launch_ts_bm<T, BITS, true, 0>(a, p);
-}
-// bb_matmul_w4a8 (int8 activations, 4-bit weights): 32 activation rows per CTA up to m = 32, else 64 (at 128 the fp32 group sums
-// do not fit beside the int32 accumulators: ptxas spills)
-template <bool IL>
-int launch_ts_w4a8(const MatmulArgs& a, const TsParams& p) {
-  if (a.m <= 32) return launch_ts_inst<int8_t, 4, 32, IL, 0, false, false, true>(a, p);
-  return launch_ts_inst<int8_t, 4, 64, IL, 0, false, false, true>(a, p);
+  return a.d.w_layout == BB_LAYOUT_COMPRESSED ? launch_ts_form<T, BITS, false, 0>(a, p) : launch_ts_form<T, BITS, true, 0>(a, p);
 }
 
 }  // namespace
@@ -715,10 +708,9 @@ int launch_gemm_ts(const MatmulArgs& a) {
   }
   const TsParams p = make_ts_params(d, a.scale, a.zeros, a.bias, a.lut, make_outspec(a), a.m);
   if (d.w_fmt == BB_W_NF || d.w_fmt == BB_W_FP4)
-    return d.a_dtype == BB_F16 ? launch_ts_bm<__half, 4, false, 1>(a, p) : launch_ts_bm<__nv_bfloat16, 4, false, 1>(a, p);
+    return d.a_dtype == BB_F16 ? launch_ts_form<__half, 4, false, 1>(a, p) : launch_ts_form<__nv_bfloat16, 4, false, 1>(a, p);
   if (d.w_fmt == BB_W_FP8_E4M3 || d.w_fmt == BB_W_FP8_E5M2)
-    return d.a_dtype == BB_F16 ? launch_ts_bm<__half, 8, false, 2>(a, p) : launch_ts_bm<__nv_bfloat16, 8, false, 2>(a, p);
-  if (a.w4a8) return d.w_layout == BB_LAYOUT_COMPRESSED ? launch_ts_w4a8<false>(a, p) : launch_ts_w4a8<true>(a, p);
+    return d.a_dtype == BB_F16 ? launch_ts_form<__half, 8, false, 2>(a, p) : launch_ts_form<__nv_bfloat16, 8, false, 2>(a, p);
   if (d.a_dtype == BB_I8) return d.w_bits == 4 ? launch_ts_layout<int8_t, 4>(a, p) : launch_ts_layout<int8_t, 2>(a, p);
   if (d.a_dtype == BB_F16) return d.w_bits == 4 ? launch_ts_layout<__half, 4>(a, p) : launch_ts_layout<__half, 2>(a, p);
   return d.w_bits == 4 ? launch_ts_layout<__nv_bfloat16, 4>(a, p) : launch_ts_layout<__nv_bfloat16, 2>(a, p);

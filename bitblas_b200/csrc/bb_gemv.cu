@@ -189,17 +189,17 @@ __device__ __forceinline__ void gemv_i8_w4a8(const GemvParams& p, const ScaledAr
 // int8 activations (W2A8 / W4A8), exact int32 accumulation.  Weights are used as raw unsigned fields
 // (mma .u8.s8); the constant zero point of the signed formats is removed with zp * sum_k(a), the sum
 // produced on the tensor cores with an all-ones A fragment.
-// SCALED: bb_matmul_scaled -- the epilogue divides by sc.a_scale[m] (read after the PDL wait) and sc.w_scale[n] (store_out_scaled;
+// Scaled: bb_matmul_scaled -- the epilogue divides by sc.a_scale[m] (read after the PDL wait) and sc.w_scale[n] (store_out_scaled;
 // bias in out_dtype).  The scales are a parameter of their own: GemvParams is also the grouped GEMV's, whose layout stays put.
 // ---------------------------------------------------------------------------------------------
 // W4A8 (BITS = 4): bb_matmul_w4a8, gemv_i8_w4a8 (red then holds fp32 bits).
-template <int BITS, int NT, bool SCALED = false, bool W4A8 = false>
-__global__ void __launch_bounds__(gemv_max_ks(NT) * 32) __maxnreg__(gemv_i8_maxnreg(NT, W4A8))
+template <int BITS, int NT, MatmulForm F>
+__global__ void __launch_bounds__(gemv_max_ks(NT) * 32) __maxnreg__(gemv_i8_maxnreg(NT, F == MatmulForm::W4A8))
 gemv_i8_kernel(const GemvParams p, const ScaledArgs sc) {
   constexpr int WPS = BITS;            // words per thread per row per step (32 k)
   constexpr int STEP_BYTES = 16 * BITS;
   __shared__ int red[MAX_KS][16][8 * NT];
-  if constexpr (W4A8) {
+  if constexpr (F == MatmulForm::W4A8) {
     gemv_i8_w4a8<NT>(p, sc, red);
     return;
   }
@@ -304,7 +304,7 @@ gemv_i8_kernel(const GemvParams p, const ScaledArgs sc) {
     int v = 0;
     for (int w = 0; w < p.ks; ++w) v += red[w][row][m];
     const int n = rb * 16 + row;
-    if constexpr (SCALED) {
+    if constexpr (F == MatmulForm::Scaled) {
       store_out_scaled(p.out.ptr[0], size_t(m) * size_t(p.out.ld) + n, v, sc.a_scale[m], sc.w_scale[n], p.bias, n,
                        p.out_dtype);
       continue;
@@ -331,6 +331,15 @@ int launch_mma_nt(const MatmulArgs& a, const GemvParams& p) {
     return launch_gemv_kernel<NT>(gemv_mma_kernel<T, BITS, IL, NT, decltype(zk)::value, decltype(sc)::value, SWIGLU>, cache, p,
                                   a.stream);
   });
+}
+
+// W4A8: the warps split the groups, not the steps (ks <= G)
+template <int BITS, int NT, MatmulForm F>
+int launch_i8_inst(const MatmulArgs& a, GemvParams p) {
+  auto kernel = gemv_i8_kernel<BITS, NT, F>;
+  static KernelCache<MAX_KS + 1> cache;
+  p.ks = pick_ks(cache, kernel, gemv_max_ks(NT), p.N / 16, F == MatmulForm::W4A8 ? p.G : p.K / 128);
+  return launch_pdl(kernel, p.N / 16, p.ks * 32, 0, a.stream, pdl_enabled(), p, a.scaled);
 }
 
 GemvParams make_params(const MatmulArgs& a) { return make_params(a.d, a.A, a.W, a.scale, a.zeros, a.bias, make_outspec(a), a.m); }
@@ -364,7 +373,7 @@ int launch_gemv_mma(const MatmulArgs& a) {
     using T = typename decltype(t)::type;
     constexpr int BITS = decltype(bits)::value;
     constexpr bool IL = decltype(il)::value;
-    return a.swiglu ? launch_mma_nt<T, BITS, IL, true>(a, p) : launch_mma_nt<T, BITS, IL, false>(a, p);
+    return a.form == MatmulForm::SwiGLU ? launch_mma_nt<T, BITS, IL, true>(a, p) : launch_mma_nt<T, BITS, IL, false>(a, p);
   });
 }
 
@@ -388,18 +397,13 @@ int launch_gemv_i8(const MatmulArgs& a) {
   const GemvParams p = make_params(a);
   return gemv_nt(p.M, [&](auto nt) {
     constexpr int NT = decltype(nt)::value;
-    static KernelCache<MAX_KS + 1> cache2, cache4, cache2s, cache4s, cache_w4a8;
-    if (a.w4a8) {   // the warps split the groups, not the steps: ks <= G
-      auto kernel = gemv_i8_kernel<4, NT, false, true>;
-      GemvParams pw = p;
-      pw.ks = pick_ks(cache_w4a8, kernel, gemv_max_ks(NT), pw.N / 16, pw.G);
-      return launch_pdl(kernel, pw.N / 16, pw.ks * 32, 0, a.stream, pdl_enabled(), pw, a.scaled);
+    switch (a.form) {   // (bb_matmul_swiglu rejects int8 activations; bb_matmul_w4a8 takes 4-bit weights only)
+      case MatmulForm::W4A8: return launch_i8_inst<4, NT, MatmulForm::W4A8>(a, p);
+      case MatmulForm::Scaled:
+        return a.d.w_bits == 2 ? launch_i8_inst<2, NT, MatmulForm::Scaled>(a, p) : launch_i8_inst<4, NT, MatmulForm::Scaled>(a, p);
+      default:
+        return a.d.w_bits == 2 ? launch_i8_inst<2, NT, MatmulForm::Plain>(a, p) : launch_i8_inst<4, NT, MatmulForm::Plain>(a, p);
     }
-    if (a.is_scaled())
-      return a.d.w_bits == 2 ? launch_gemv_kernel<NT>(gemv_i8_kernel<2, NT, true>, cache2s, p, a.stream, a.scaled)
-                             : launch_gemv_kernel<NT>(gemv_i8_kernel<4, NT, true>, cache4s, p, a.stream, a.scaled);
-    return a.d.w_bits == 2 ? launch_gemv_kernel<NT>(gemv_i8_kernel<2, NT>, cache2, p, a.stream, a.scaled)
-                           : launch_gemv_kernel<NT>(gemv_i8_kernel<4, NT>, cache4, p, a.stream, a.scaled);
   });
 }
 

@@ -653,7 +653,7 @@ int launch_slab_inst(const MatmulArgs& a, const CUtensorMap& tm, const SlabParam
 }
 template <typename T, bool IL, int FMT>
 int launch_slab(const MatmulArgs& a, const CUtensorMap& tm, const SlabParams& p) {
-  return a.swiglu ? launch_slab_inst<T, IL, FMT, true>(a, tm, p) : launch_slab_inst<T, IL, FMT, false>(a, tm, p);
+  return a.form == MatmulForm::SwiGLU ? launch_slab_inst<T, IL, FMT, true>(a, tm, p) : launch_slab_inst<T, IL, FMT, false>(a, tm, p);
 }
 
 }  // namespace

@@ -195,9 +195,9 @@ generic_float_kernel(const bb_matmul_desc d, const T* __restrict__ A, const uint
   }
 }
 
-// int8 activations, exact int32 accumulate.  SCALED: bb_matmul_scaled -- store_out_scaled with a_scale [M], w_scale [N] and a bias
+// int8 activations, exact int32 accumulate.  Scaled: bb_matmul_scaled -- store_out_scaled with a_scale [M], w_scale [N] and a bias
 // in out_dtype.  W4A8: bb_matmul_w4a8 -- 4-bit weights, fp32 group scales sc.w_scale [N, G], zero points, store_out_dequant
-template <bool SCALED = false, bool W4A8 = false>
+template <MatmulForm F>
 __global__ void __launch_bounds__(WARPS * 32)
 generic_int_kernel(const bb_matmul_desc d, const int8_t* __restrict__ A, const uint8_t* __restrict__ W,
                    const int8_t* __restrict__ scale, const void* __restrict__ zeros,
@@ -206,7 +206,7 @@ generic_int_kernel(const bb_matmul_desc d, const int8_t* __restrict__ A, const u
   const int n = blockIdx.x * WARPS + warp;
   const int m0 = blockIdx.y * MT;
   if (n >= d.N) return;
-  if constexpr (W4A8) {
+  if constexpr (F == MatmulForm::W4A8) {
     // group by group: the exact int32 sum of the group (lanes stride k, then a butterfly sum), promoted into fp32 with the
     // group's scale in group order -- the order of gemm_ts_kernel without split-K
     const int K = d.K, g = d.group_size <= 0 ? K : d.group_size, G = K / g;
@@ -288,7 +288,7 @@ generic_int_kernel(const bb_matmul_desc d, const int8_t* __restrict__ A, const u
     for (int i = 0; i < MT; ++i) {
       if (m0 + i >= M) continue;
       const size_t idx = size_t(m0 + i) * d.N + n;
-      if constexpr (SCALED) {
+      if constexpr (F == MatmulForm::Scaled) {
         store_out_scaled(C, idx, acc[i], sc.a_scale[m0 + i], sc.w_scale[n], d.with_bias ? bias : nullptr, n, d.out_dtype);
         continue;
       }
@@ -321,11 +321,11 @@ int launch_generic(const MatmulArgs& a) {
     set_error("generic_simt: W must be 4-byte aligned for %d-bit weights (they are read as 32-bit words)", d.w_bits);
     return 5;
   }
-  dim3 grid(((a.swiglu ? d.N / 2 : d.N) + WARPS - 1) / WARPS, (a.m + MT - 1) / MT);
+  dim3 grid(((a.form == MatmulForm::SwiGLU ? d.N / 2 : d.N) + WARPS - 1) / WARPS, (a.m + MT - 1) / MT);
   dim3 block(WARPS * 32);
   auto run_float = [&](auto t) {
     using T = typename decltype(t)::type;
-    auto kernel = a.swiglu ? generic_float_kernel<T, true> : generic_float_kernel<T, false>;
+    auto kernel = a.form == MatmulForm::SwiGLU ? generic_float_kernel<T, true> : generic_float_kernel<T, false>;
     kernel<<<grid, block, 0, a.stream>>>(d, (const T*)a.A, (const uint8_t*)a.W, (const T*)a.lut, (const T*)a.scale, a.zeros, a.bias,
                                          a.C, a.m);
   };
@@ -334,7 +334,9 @@ int launch_generic(const MatmulArgs& a) {
   } else if (d.a_dtype == BB_BF16) {
     run_float(TypeTag<__nv_bfloat16>{});
   } else {
-    auto kernel = a.w4a8 ? generic_int_kernel<false, true> : (a.is_scaled() ? generic_int_kernel<true> : generic_int_kernel<false>);
+    auto kernel = a.form == MatmulForm::Scaled ? generic_int_kernel<MatmulForm::Scaled>
+                  : a.form == MatmulForm::W4A8 ? generic_int_kernel<MatmulForm::W4A8>
+                                               : generic_int_kernel<MatmulForm::Plain>;
     kernel<<<grid, block, 0, a.stream>>>(d, (const int8_t*)a.A, (const uint8_t*)a.W, (const int8_t*)a.scale, a.zeros,
                                          (const int8_t*)a.bias, a.C, a.m, a.scaled);
   }
